@@ -1,10 +1,10 @@
 #!/usr/bin/env python
-"""bench.py -- benchmark of the TecoGAN recurrent video-SR hot path on B200.
+"""bench.py -- benchmark of the TecoGAN recurrent video-SR hot path on H100.
 
 Headline (BASELINE.json `metric`: "HR frames/sec (4x SR, 10-frame clips)", north_star: "synthetic 32x32 -> 128x128
 x10-frame clips at 1/2/4/8 GPUs"): every rank owns CLIPS independent synthetic clips of 10 LR frames 32x32 and runs them
 in lock-step through the full recurrence (fnet on every consecutive pair -> upscale_four/warp/space-to-depth feedback ->
-generator_F, 16 res-blocks, seeded random weights), bf16 tcgen05 convolutions, one CUDA-graph replay per clip batch.
+generator_F, 16 res-blocks, seeded random weights), bf16 wgmma convolutions, one CUDA-graph replay per clip batch.
 A "step" = one batch of CLIPS clips x 10 frames per rank.
   value = HR frames of all ranks / max-over-ranks device time, LR clips resident in HBM;
   e2e   = the same through the public ClipEngine API from pinned HOST clips: H2D of every LR clip and D2H of every uint8
@@ -18,6 +18,7 @@ Extra objects in the same JSON line (each timed the same way: CUDA events, max o
   python bench.py --gpus 1 --steps 10 --warmup 3
   python -m torch.distributed.run --nproc-per-node N ... bench.py --gpus N ...
   python bench.py --impl reference        # CPU restatement of the reference (oracle/) on the host cores, same workload
+  python bench.py ... --dump-outputs DIR   # after the timed steps: DIR/<name>.npy of what the last timed step returned
 """
 import argparse
 import json
@@ -36,7 +37,7 @@ import torch  # noqa: E402
 LR = 32                      # metric config: 32x32 LR -> 128x128 HR
 CLIP_T = 10                  # frames per clip
 NUM_RESBLOCK = 16
-DEFAULT_CLIPS = 296          # clips per GPU = 2 x 148 SMs (each clip is 4 tiles of 16x16 LR pixels per layer)
+DEFAULT_CLIPS = 264          # clips per GPU = 2 x 132 SMs
 # algorithmic MACs per LR pixel (SURVEY.md Appendix B): generator N=16, fnet
 GEN_MACS, FNET_MACS = 1420992, 126720
 WORKLOAD = ("metric config: 4x SR inference of synthetic 10-frame clips 32x32->128x128, %d clips per GPU in lock-step "
@@ -67,7 +68,7 @@ def synthetic_clips(T, B, h, w, seed):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons during the timed region (read-only queries)."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -210,11 +211,15 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--headline-only", action="store_true", help="skip configs[1], the config-5 sweep and the training steps")
     ap.add_argument("--train-steps", type=int, default=4)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed headline step returned as DIR/<name>.npy (float32, seeded sample of clips)")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
     if args.impl == "reference":
+        if args.dump_outputs:
+            ap.error("--dump-outputs writes the CUDA path's outputs; it does not apply to --impl reference")
         run_reference(args, rank, world)
         return
     if args.warmup < 3:
@@ -275,10 +280,11 @@ def main():
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak_tf = float(peaks.get("bf16_tflops", 1590.0))
-    peak_tf_sus = float(peaks.get("bf16_tflops_sustained", 1400.0))
-    peak_gbs = float(peaks.get("hbm_gbs", 6650.0))
-    peak_src = "measured (MEASURED_PEAKS.json)" if peaks else "fallback 1.59 PFLOP/s / 6.65 TB/s"
+    # fallback: NVIDIA data sheet of the H100 SXM (dense bf16, HBM3), not a measured rate
+    peak_tf = float(peaks.get("bf16_tflops", 989.0))
+    peak_tf_sus = float(peaks.get("bf16_tflops_sustained", 989.0))
+    peak_gbs = float(peaks.get("hbm_gbs", 3350.0))
+    peak_src = "measured (MEASURED_PEAKS.json)" if peaks else "H100 SXM data sheet 989 TFLOP/s / 3.35 TB/s"
 
     config.set_precision("bf16")
     st = V.set_default_store(V.VariableStore())
@@ -356,9 +362,11 @@ def main():
     note("headline: resident %.2f ms/step, e2e %.2f ms/step" % (ms_res / args.steps, ms_e2e / args.steps))
     # the e2e leg really moved the bytes: spot-check the host copy against the device result of the last batch
     assert torch.equal(host_out[(args.steps - 1) & 1][-1, 0], eng.clip_u8[-1, 0].cpu()), "e2e: host frames differ from device frames"
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, rank, host_out[(args.steps - 1) & 1], eng.out01)
 
     # --- dominant kernel: the generator trunk (input conv + 16 residual blocks = 33 layers of 3x3 64->64) on the whole clip
-    # batch [B,32,32,64] -- ONE launch of conv3x3_lin_kernel (kx-fused N=192 MMAs, CTA-local clips) -- timed alone (graph replay).
+    # batch [B,32,32,64] -- ONE launch of conv3x3_chain_kernel (CTA-local clips across layers) -- timed alone (graph replay).
     g = eng.gen
     reps = 16
 
@@ -381,15 +389,15 @@ def main():
         return graph_us(lambda: trunk_pairs(gp, n), n)
     layer_flop = 2.0 * B * LR * LR * 576 * 64
     per_layer_us = kernel_us(g, reps)                     # the per-layer persistent kernel (N = 64 MMAs), for comparison
-    if getattr(g, "lin", False):
+    if hasattr(g, "trunk_plan"):   # 32-pixel-wide frames: the one-launch chain, timed whether or not the engine uses it
         n_layers = len(g.trunk_plan)
         k_us = graph_us(lambda: [K.conv3x3_lin_chain(g.x_in, g.a, g.b, g.trunk_w, g.trunk_b, g.trunk_plan) for _ in range(2)], 2)
         k_flop = layer_flop * n_layers
-        k_name = ("conv3x3_lin_kernel (generator trunk: %d layers of 3x3 64->64 on the clip batch [%d,32,32,64] in one launch; "
-                  "kx-fused N=192 tcgen05.mma, x-shift by warp shuffles)" % (n_layers, B))
+        k_name = ("conv3x3_chain_kernel (generator trunk: %d layers of 3x3 64->64 on the clip batch [%d,32,32,64] in one launch, "
+                  "CTA-local clips across layers)" % (n_layers, B))
     else:
         k_us, k_flop = per_layer_us, layer_flop
-        k_name = "conv3x3_tc_kernel (3x3 64->64 res-block layer on the clip batch [%d,32,32,64])" % B
+        k_name = "conv3x3_wgmma_kernel (3x3 64->64 res-block layer on the clip batch [%d,32,32,64])" % B
 
     # --- HBM-bound kernel of the path: fused upscale_four + warp + space-to-depth feedback on a batch larger than L2
     # (32 clips of 256x256 LR -> 1024x1024 HR: 403 MB read + 201 MB written), algorithmic 18.5 B per HR pixel
@@ -424,7 +432,7 @@ def main():
         "config": {"workload": WORKLOAD % B, "num_resblock": NUM_RESBLOCK, "clips_per_gpu": B, "frames_per_clip": CLIP_T,
                    "frames_per_step": B * CLIP_T,
                    "l2": "no flush needed: one step streams %.0f MB of activations (64-channel HR buffer alone %.0f MB), larger "
-                         "than the 126 MB L2" % (B * 128 * 128 * (128 + 128 + 24) / 1e6, B * 128 * 128 * 128 / 1e6),
+                         "than the 50 MB L2" % (B * 128 * 128 * (128 + 128 + 24) / 1e6, B * 128 * 128 * 128 / 1e6),
                    "weights": "seeded random init (xavier, res-block/output weights x0.5)", "cuda_graph": True,
                    "fnet": "all consecutive pairs of a clip first (lib/Teco.py:102-117 order), then the generator recurrence"},
         "clocks": clocks,
@@ -434,10 +442,11 @@ def main():
                        "separate streams overlapping the next batch"},
         "gpu_launches": int(launches_per_step * args.steps),
         "roofline": {"bound": "tensor", "kernel": k_name,
+                     "engine_trunk": "one-launch chain" if getattr(g, "lin", False) else "per-layer launches",
                      "achieved": ach_tf, "peak": peak_tf, "unit": "TFLOP/s", "frac": ach_tf / peak_tf,
                      "peak_source": peak_src + ", burst bf16 (kernel timed alone)", "us_per_launch": k_us,
-                     "flop_per_launch": k_flop, "traffic": _traffic("r02_conv_lin_traffic.json"),
-                     "per_layer_kernel": {"kernel": "conv3x3_tc_kernel (same layers, one launch each, N=64 MMAs)", "us_per_layer": per_layer_us,
+                     "flop_per_launch": k_flop,
+                     "per_layer_kernel": {"kernel": "conv3x3_wgmma_kernel (same layers, one launch each, N=64 MMAs)", "us_per_layer": per_layer_us,
                                           "achieved": layer_flop / (per_layer_us * 1e-6) / 1e12, "frac": layer_flop / (per_layer_us * 1e-6) / 1e12 / peak_tf},
                      "whole_step": {"algorithmic_gflop_per_clip": clip_flop() / 1e9, "achieved_tflops": whole_tf,
                                     "frac_of_sustained": whole_tf / peak_tf_sus}},
@@ -445,7 +454,7 @@ def main():
                                                      "space_to_depth), 32 x 1024x1024 HR frames, smooth motion field, working set 604 MB > L2",
                          "achieved": warp_bytes / (warp_us * 1e-6) / 1e9, "peak": peak_gbs, "unit": "GB/s",
                          "frac": warp_bytes / (warp_us * 1e-6) / 1e9 / peak_gbs, "us_per_launch": warp_us,
-                         "algorithmic_bytes_per_launch": warp_bytes, "traffic": _traffic("r02_warp_v2_traffic.json"),
+                         "algorithmic_bytes_per_launch": warp_bytes,
                          "rough_motion": {"us_per_launch": warp_rough_us, "achieved": warp_bytes / (warp_rough_us * 1e-6) / 1e9,
                                           "frac": warp_bytes / (warp_rough_us * 1e-6) / 1e9 / peak_gbs},
                          "peak_source": peak_src + ", copy bandwidth"},
@@ -487,7 +496,7 @@ def main():
             "workload": "configs[1]: 4x SR inference 128x128->512x512, one 120-frame synthetic clip per GPU (streaming, batch 1)",
             "value": F1 * n1 * world / (t_res / 1000.0), "e2e": F1 * n1 * world / (t_e2e / 1000.0), "unit": "frames/s",
             "ms_per_clip": t_res / n1, "fnet_lookahead": True,
-            "roofline": {"bound": "tensor", "kernel": "conv3x3_tc_kernel (3x3 64->64 @128x128, one tile per CTA)",
+            "roofline": {"bound": "tensor", "kernel": "conv3x3_wgmma_kernel (3x3 64->64 @128x128)",
                          "achieved": k1_flop / (k1_us * 1e-6) / 1e12, "peak": peak_tf, "unit": "TFLOP/s",
                          "frac": k1_flop / (k1_us * 1e-6) / 1e12 / peak_tf, "us_per_launch": k1_us}}
         note("configs[1]: %.1f ms/clip resident" % (t_res / n1))
@@ -530,12 +539,19 @@ def main():
         dist.destroy_process_group()
 
 
-def _traffic(name):
-    """DRAM bytes per launch of the kernel from the committed `ncu --set full` capture (profiles/), or None."""
-    try:
-        return json.load(open(os.path.join(ROOT, "profiles", name)))["traffic_bytes_per_launch"]
-    except Exception:
-        return None
+DUMP_CLIPS = 8               # clips sampled for --dump-outputs (10 x 8 HR frames of 128x128x3 as float32: 15.7 MB)
+
+
+def dump_outputs(out_dir, rank, frames_u8, last01):
+    """What the headline path returned in its last timed step, for output-by-output comparison of two builds: the uint8 HR
+    frames [T,B,128,128,3] of the clip batch and the fp32 [0,1] last frame [B,128,128,3], on a fixed seeded sample of clips."""
+    os.makedirs(out_dir, exist_ok=True)
+    B = frames_u8.shape[1]
+    idx = torch.randperm(B, generator=torch.Generator().manual_seed(2024))[:min(DUMP_CLIPS, B)].sort().values
+    sfx = "" if rank == 0 else "_rank%d" % rank
+    np.save(os.path.join(out_dir, "clip_indices%s.npy" % sfx), idx.numpy().astype(np.float64))
+    np.save(os.path.join(out_dir, "hr_frames%s.npy" % sfx), frames_u8[:, idx].cpu().numpy().astype(np.float32))
+    np.save(os.path.join(out_dir, "last_frame01%s.npy" % sfx), last01[idx.to(last01.device)].cpu().numpy().astype(np.float32))
 
 
 def bench_train(args, rank, world, dev, dist, ev_time, max_over_ranks, note, peak_tf_sus):

@@ -1,10 +1,10 @@
 /*
- * teco.h -- C ABI of libteco.so: hand-written sm_100a kernels for the TecoGAN recurrent
+ * teco.h -- C ABI of libteco.so: hand-written sm_90a kernels for the TecoGAN recurrent
  * video-SR hot path (SURVEY.md section 8).  Plain pointers and sizes only; no torch types.
  *
  * The reference (thunil/TecoGAN) has no FFI layer: its "operator API" is Python functions
  * that build TensorFlow graph ops.  Each entry point below names the reference call site
- * (file:line under /root/reference) whose TensorFlow/cuDNN arithmetic it replaces; the Python
+ * (file:line in the reference repository) whose TensorFlow/cuDNN arithmetic it replaces; the Python
  * mirror in tecogan_b200/lib/{ops,frvsr,Teco}.py keeps the reference's function names and
  * binds these symbols through ctypes (see INTEGRATION.md).
  *
@@ -72,10 +72,10 @@ int teco_conv2d_wgrad_f32(const teco_conv_desc* d, const float* x, const float* 
                           int accumulate, void* stream);
 
 /* ---------------------------------------------------------------------------------------
- * bf16 tensor-core convolution (tcgen05.mma kind::f16, fp32 accumulation in TMEM).
+ * bf16 tensor-core convolution (wgmma m64nNk16, fp32 accumulation in registers).
  * 3x3, stride 1, SAME: the generator / FNet layers (lib/frvsr.py:5-41, 50-63, 79-80).
  * x: NHWC bf16 with Cin (multiple of 16); y: NHWC bf16 with Cout channels.
- * wpk: weights pre-packed by teco_pack_conv3x3_bf16 (UMMA canonical K-major core matrices).
+ * wpk: weights pre-packed by teco_pack_conv3x3_bf16 (K-major SWIZZLE_128B core matrices).
  * res (bf16, optional) is added after the activation; out_f32 (optional, [N,H,W,out_f32_c])
  * receives post_scale*(value + res_f32) + post_shift for the first out_f32_c channels
  * (used by the generator's output stage: + bicubic, *2-1  lib/frvsr.py:85-87).
@@ -99,7 +99,7 @@ int teco_conv3x3_tc(const teco_tc_desc* d, const void* x, const void* wpk, const
 /* Bias gradient of conv2() (slim.conv2d biases, reference lib/ops.py:47-56): db[c] (+)= sum over npix pixels of dy[pixel*cpitch + c]. */
 int teco_bias_grad_f32(const float* dy, float* db, int64_t npix, int32_t C, int32_t cpitch, int32_t accumulate, void* stream);
 
-/* Weight gradient of conv2() 3x3 stride 1 SAME on tcgen05 (the gradient tf.train.AdamOptimizer.compute_gradients takes
+/* Weight gradient of conv2() 3x3 stride 1 SAME on the tensor cores (the gradient tf.train.AdamOptimizer.compute_gradients takes
  * through slim.conv2d: reference lib/ops.py:47-56, lib/Teco.py:426,446-447):
  *   dw[ky][kx][ci][co] (+)= sum_p x[p + (ky-1,kx-1)][ci] * dz[p][co],  dw fp32 in TF layout [3,3,cin,cout].
  * x [N,H,W,cin_pad], dz [N,H,W,cout_pad]: NHWC bf16, channel counts padded to multiples of 64; cout % 4 == 0.
@@ -107,23 +107,17 @@ int teco_bias_grad_f32(const float* dy, float* db, int64_t npix, int32_t C, int3
 int teco_conv3x3_wgrad_tc(int32_t N, int32_t H, int32_t W, int32_t cin_pad, int32_t cout_pad, int32_t cin, int32_t cout,
                           const void* x, const void* dz, float* dw, int32_t accumulate, void* stream);
 
-/* Row-linearised multi-layer 3x3 64->64 chain for 32-pixel-wide images (the metric configuration's 32x32 LR clips): the same
+/* Multi-layer 3x3 64->64 chain for 32-pixel-wide images (the metric configuration's 32x32 LR clips): the same
  * layers of generator_F (input conv + residual blocks, reference lib/frvsr.py:59-70) -- or any chain of conv2(3x3, 64->64) + bias + ReLU /
- * LeakyReLU / none + optional residual -- in ONE launch.  One tcgen05.mma covers the three horizontal taps of a kernel row
- * (N = 192, runs at the tensor floor; N = 64 cannot), the epilogue recombines them with warp shuffles; every CTA keeps its own
- * images for all layers, so there is no grid-wide dependency between layers.
+ * LeakyReLU / none + optional residual -- in ONE launch.  Every CTA keeps its own images for all layers, so there is no
+ * grid-wide dependency between layers; the next layer's weights are prefetched while a layer computes.
  * x_in / buf_a / buf_b: NHWC bf16 [N,H,32,64] (buffer ids 0 / 1 / 2; x_in is never written).
  * plan_host: HOST array [num_layers][4] = {input buffer id, output buffer id, residual buffer id or -1, TECO_ACT_*}.
- *   A residual may be added in place (residual id == output id) but may not be the previous layer's output.
+ *   A residual may be added in place (residual id == output id); the input is never the output.
  * wpk_all: num_layers packed layers back to back (teco_pack_conv3x3_bf16, 64x64 -> 73728 bytes each); bias_all [num_layers][64]. */
 int teco_conv3x3_lin_supported(int32_t N, int32_t H, int32_t W, int32_t num_layers);
 int teco_conv3x3_lin_tc(int32_t N, int32_t H, int32_t W, int32_t num_layers, const void* x_in, void* buf_a, void* buf_b,
                         const void* wpk_all, const float* bias_all, const int32_t* plan_host, void* stream);
-
-/* Developer hook: when buf != NULL every teco_conv3x3_tc CTA writes clock64() stamps to buf[cta*32 ..] (phase
- * boundaries: start, setup done, halo landed, first/last weight slab landed, MMAs issued, accumulator ready,
- * epilogue done, teardown).  buf must hold gridDim*32 int64.  Pass NULL to switch it off. */
-int teco_debug_timing(void* buf);
 
 /* ---------------------------------------------------------------------------------------
  * Warp / resample family (HBM-bound).

@@ -12,7 +12,7 @@ Differences forced by the environment, stated once:
     runners; an empty flag raises as in the reference unless --synthetic_data is given (seeded synthetic HR clips and,
     without --vgg_ckpt, a seeded random frozen VGG -- for benchmarks and tests only); the device half (Gaussian
     down-sampling, crops) is the same either way;
-  * --precision {bf16,fp32} selects tcgen05 tensor-core or fp32 CUDA-core convolutions for inference;
+  * --precision {bf16,fp32} selects wgmma tensor-core or fp32 CUDA-core convolutions for inference;
     --train_precision {fp32,bf16} does the same for training (default fp32, the reference's arithmetic);
   * under `torchrun` each rank trains on its own clip shard with one NCCL all-reduce per step.
 """
@@ -40,8 +40,8 @@ FLAG_DEFS = [  # (name, type, default) -- reference main.py:32-103
     ('display_freq', int, 20), ('summary_freq', int, 100), ('save_freq', int, 10000), ('ratio', float, 0.01),
     ('Dt_mergeDs', bool, True), ('Dt_ratio_0', float, 1.0), ('Dt_ratio_add', float, 0.0), ('Dt_ratio_max', float, 1.0),
     ('Dbalance', float, 0.4), ('crop_dt', float, 0.75), ('D_LAYERLOSS', bool, True),
-    ('precision', str, 'bf16'),          # extension: inference arithmetic (bf16 tcgen05 | fp32 CUDA cores)
-    ('train_precision', str, 'fp32'),    # extension: training convolutions (fp32 as the reference | bf16 tcgen05)
+    ('precision', str, 'bf16'),          # extension: inference arithmetic (bf16 wgmma | fp32 CUDA cores)
+    ('train_precision', str, 'fp32'),    # extension: training convolutions (fp32 as the reference | bf16 wgmma)
     ('synthetic_data', bool, False),     # extension: seeded synthetic HR clips / random frozen VGG instead of raising
 ]
 
@@ -247,7 +247,7 @@ def train(FLAGS):
     if world > 1:
         dist.init_process_group('nccl', device_id=torch.device('cuda', local_rank))
     from tecogan_b200 import config
-    config.set_train_precision(FLAGS.train_precision)   # fp32 as the reference; bf16: tcgen05 convolutions, fp32 master weights
+    config.set_train_precision(FLAGS.train_precision)   # fp32 as the reference; bf16: wgmma convolutions, fp32 master weights
     store = V.set_default_store(V.VariableStore(seed=FLAGS.rand_seed))   # same seed on every rank -> identical init
     gan = FLAGS.ratio > 0
     if FLAGS.checkpoint is not None:

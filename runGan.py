@@ -49,7 +49,7 @@ elif runcase == 1:   # inference a trained model
     dirstr = './results/'
     testpre = ['calendar']
     os.makedirs(dirstr, exist_ok=True)
-    lr_root = "./LR/" if os.path.exists("./LR/") else "/root/reference/LR/"
+    lr_root = "./LR/"   # the Vid4 LR frames, laid out as the reference's case 0 download leaves them
     # reference runGan.py:87: --checkpoint ./model/TecoGAN (a TF V2 bundle, read without TensorFlow); then our .pt; else seeded init
     ckpt = ('./model/TecoGAN' if os.path.exists('./model/TecoGAN.index') else
             './model/TecoGAN.pt' if os.path.exists('./model/TecoGAN.pt') else 'random:1234')

@@ -1,4 +1,4 @@
-"""tecogan_b200 -- B200-native (sm_100a) implementation of TecoGAN's recurrent video-SR hot path.
+"""tecogan_b200 -- H100-native (sm_90a) implementation of TecoGAN's recurrent video-SR hot path.
 
 Layout: csrc/ (CUDA kernels + C ABI -> libteco.so), _ffi.py (ctypes binding), variables.py (TF-style
 variable scopes holding the weights), lib/{ops,frvsr,Teco,dataloader}.py (host-side mirror of the reference's

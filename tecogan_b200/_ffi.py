@@ -44,7 +44,6 @@ SIGNATURES = {
     "teco_conv3x3_tc": [C.POINTER(TcDesc), _P, _P, _P, _P, _P, _P, _P, _P],
     "teco_bias_grad_f32": [_P, _P, _I64, _I32, _I32, _I32, _P],
     "teco_conv3x3_wgrad_tc": [_I32, _I32, _I32, _I32, _I32, _I32, _I32, _P, _P, _P, _I32, _P],
-    "teco_debug_timing": [_P],
     "teco_conv3x3_lin_supported": [_I32, _I32, _I32, _I32],
     "teco_conv3x3_lin_tc": [_I32, _I32, _I32, _I32, _P, _P, _P, _P, _P, _P, _P],
     "teco_warp_f32": [_P, _P, _P, _I32, _I32, _I32, _I32, _P],
@@ -92,7 +91,7 @@ def lib():
         if not os.path.exists(LIB_PATH):
             raise RuntimeError(
                 "tecogan_b200: %s not found -- build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-                "(nvcc, sm_100a).  There is no CPU or PyTorch fallback." % LIB_PATH)
+                "(nvcc, sm_90a).  There is no CPU or PyTorch fallback." % LIB_PATH)
         l = C.CDLL(LIB_PATH)
         for name, args in SIGNATURES.items():
             fn = getattr(l, name)

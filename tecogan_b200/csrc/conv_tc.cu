@@ -1,714 +1,322 @@
-// bf16 3x3 convolution / 3x3-stride-2 transposed convolution on the 5th-gen tensor cores (sm_100a):
-// TMA halo tiles -> shared memory -> tcgen05.mma (kind::f16, fp32 accumulators in TMEM) -> tcgen05.ld
+// bf16 3x3 convolution / 3x3-stride-2 transposed convolution on the Hopper tensor cores (sm_90a):
+// TMA halo tiles -> shared memory -> wgmma (m64nNk16, bf16 operands, fp32 accumulators in registers) -> register
 // epilogue (bias, activation, residual, bf16 store; or fp32 "+bicubic, *2-1" output stage).
 //
 // Replaces, layer by layer, the cuDNN convolutions behind conv2()/conv2_tran() of the reference
 // (lib/ops.py:35-56) as used by generator_F (lib/frvsr.py:44-88) and fnet (lib/frvsr.py:4-41).
 //
 // Implicit GEMM, no im2col buffer:
-//   CTA tile  = 16 image rows x (8*J) pixels; every 16x8 sub-tile is one UMMA accumulator with M = 128.
-//   A operand = NHWC bf16 activations, 64 channels = one 128-byte row per pixel.  Per 64-channel block the halo is
-//               staged by THREE 4-D TMA boxes (64 ch, 8J px, 18 rows, 1 image), one per horizontal tap offset kx,
-//               with SWIZZLE_128B.  Each box is the UMMA canonical K-major SW128 layout as it lands
-//               (8 consecutive pixels = one 1024-byte swizzle atom, SBO = one box row).  Vertical taps ky are
-//               descriptor start-address offsets of whole box rows (atom aligned), so 3 loads serve 9 taps.
-//               TMA out-of-bounds zero fill implements TF 'SAME' padding.
-//   B operand = weights pre-packed on the device as [cin/64][tap][cout][64 cin] bf16 in the same SW128 image,
-//               streamed by 1-D bulk copies.  When a whole layer fits (64->64: 72 KB) the slabs are fetched once,
-//               BEFORE the programmatic-dependent-launch wait, and multicast across a 4-CTA cluster.
-//   D         = fp32 in TMEM, column block (sub-tile, phase) * Cout.
-// Transposed conv (stride 2, TF 'SAME', y[i] = sum_j x[j] w[i-2j]) is the same loop with the nine taps routed to
-// four sub-pixel phase accumulators (SURVEY.md A.3) and a 2x interleaving epilogue.
+//   CTA tile  = 16 image rows x 8 pixels = 128 output pixels; warpgroup g (two per CTA) owns rows 8g..8g+7, i.e. one
+//               M = 64 accumulator (8 image rows x 8 pixels).
+//   A operand = NHWC bf16 activations, 64 channels = one 128-byte row per pixel.  Per 64-channel block the halo (18 rows x
+//               10 pixels) is staged by ONE 4-D TMA box with SWIZZLE_128B; TMA out-of-bounds zero fill implements TF
+//               'SAME' padding.  Tap (ky, kx) is the descriptor start address of halo row ky, pixel kx: 8 pixels of one
+//               image row are one 8 x 128 B core-matrix group, SBO = one halo row (10 x 128 B).
+//   B operand = weights pre-packed on the device as [cin/64][tap][cout][64 cin] bf16 in the same SW128 image, fetched by
+//               1-D bulk copies: once per CTA when the layer's Cout slice fits next to the halo ring (every 64 -> 64 layer),
+//               otherwise with each 64-channel block.
+//   D         = fp32 registers, NT / 2 per thread per accumulator (NT = output channels per CTA: 64, 32 or 16).
+// Transposed conv (stride 2, TF 'SAME', y[i] = sum_j x[j] w[i-2j]) is the same loop with the nine taps routed to four
+// sub-pixel phase accumulators (SURVEY.md A.3) and a 2x interleaving epilogue.
 //
-// Why SW128 and not the no-swizzle layout (round-1 measurement, profiles/conv_tc_r01_notes.md): with 16-byte core
-// matrix rows every tcgen05.mma took ~250 cycles instead of ~32-48, and the 16-byte TMA rows ran at ~10 B/clk/SM.
-//
-// Warp roles (320 threads): warp 0 = TMA producer, warp 1 = TMEM owner + MMA issuer, warps 2..9 = epilogue
-// (one epilogue warp per scheduler is latency-bound: ~1000 clk per 32 channels; two per scheduler halve it).
+// Persistent CTAs walk tiles c, c + G, ...; the halo (and weight) ring has two stages, so the TMA of the next 64-channel
+// block or tile is in flight while the warpgroups run the MMAs and the epilogue of the current one.
 #include <cuda.h>
-#include <cstdlib>
-#include <type_traits>
 #include "teco_common.cuh"
 #include "tc_ptx.cuh"
 
 namespace {
 
+using namespace tcptx;
+
 constexpr int TILE_ROWS = 16;
+constexpr int TILE_COLS = 8;
 constexpr int HALO_ROWS = TILE_ROWS + 2;
-constexpr int CB = 64;                 // channels per K block = one 128-byte swizzled row
-constexpr int MAX_WST = 12;
-constexpr int MAX_HST = 4;             // halo ring depth: 2 when the input is L2-resident, up to 4 when it streams from HBM
-constexpr int NUM_EPI_WARPS = 8;       // two warps per TMEM lane quarter, each taking half of the output channels
-constexpr int NUM_THREADS = 64 + 32 * NUM_EPI_WARPS + 32;   // + the output-store warp (staged epilogue)
-constexpr int STORE_WARP = 2 + NUM_EPI_WARPS;
+constexpr int HALO_COLS = TILE_COLS + 2;
+constexpr int CB = 64;                                                 // channels per K block = one 128-byte swizzled row
+constexpr uint32_t HALO_BYTES = HALO_ROWS * HALO_COLS * 128;           // 23040
+constexpr uint32_t HALO_STAGE = (HALO_BYTES + 1023u) & ~1023u;         // 24576: stages stay 1024-byte aligned
+constexpr int NUM_THREADS = 256;                                       // two warpgroups
+constexpr size_t SMEM_MAX = 232448;                                    // 227 KB: opt-in maximum per block on sm_90
 
 struct TcParams {
-  int N, H, W, Cin, Cout;             // Cout = channel pitch of y / res / bias (all output channels)
-  int Ncta, nsplit, G, AS;            // output channels per CTA (UMMA N), Cout splits, CTAs per split (persistent: each
-                                      // walks tiles c, c+G, ...), TMEM accumulator stages (1 or 2)
-  int tiles_x, tiles_y, J;
-  int mode, act, out_f32_c;
+  int N, H, W, Cout;          // Cout = channel pitch of y / res / bias (all output channels)
+  int nblk, act, out_f32_c;   // Cin / 64
+  int tiles_x, tiles_y, num_tiles, resident;
   float post_scale, post_shift;
-  int nblk, WST, TPS, KS;              // Cin/64, weight ring stages, taps per weight slab (1 or 3), K-split chains
-  int HST, CS, mcast, num_tiles;       // halo stages, cluster size, resident+multicast weights, real tile count
-  uint32_t copy_bytes, halo_stage_bytes, w_slab_bytes, tmem_cols;
-  int tma_out, tma_res;                // staged epilogue: bf16 output / residual tiles through swizzled smem + TMA (see conv_tc_sw.cu)
+  uint32_t w_blk_bytes, stage_bytes;   // 9 taps x NT x 128 B; one ring stage (halo, + weights unless resident)
   const uint8_t* wpk;
   const float* bias;
   const __nv_bfloat16* res;
   __nv_bfloat16* y;
   const float* res_f32;
   float* out_f32;
-  long long* dbg;                      // optional [gridDim][32] clock64 stamps (teco_debug_timing)
 };
 
-using namespace tcptx;   // mbarrier / TMA / tcgen05 wrappers and the UMMA descriptors: tc_ptx.cuh
+// tap (ky, kx) -> halo offset (ry, rx) and accumulator.  Transposed conv: output pixel (2i + py, 2j + px) collects the taps
+// with ky == 1 (py = 1) or ky in {0, 2} (py = 0), reading input row i (ky != 2) or i - 1 (ky == 2); the same for x.
+template <int MODE>
+__device__ __forceinline__ void tap_route(int t, int& ry, int& rx, int& ph) {
+  const int ky = t / 3, kx = t % 3;
+  if (MODE == 1) {
+    ry = ky == 2 ? 0 : 1;
+    rx = kx == 2 ? 0 : 1;
+    ph = (ky == 1 ? 2 : 0) + (kx == 1 ? 1 : 0);
+  } else {
+    ry = ky; rx = kx; ph = 0;
+  }
+}
 
-// ------------------------------------------------------------------ the kernel
-// MODE 0 conv / 1 transposed conv; TPS taps per weight slab; J sub-tiles per CTA; KS K-split accumulator chains.
-// They are compile-time so that the MMA issue loop is a fully unrolled stream of UTCHMMA whose descriptors differ
-// from per-stage bases by immediates (uniform-datapath adds, no per-instruction R2UR).
-//
-// Persistent and pipelined: a CTA walks tiles c, c+G, c+2G, ... of its Cout split.  The halo ring (HST stages), the
-// weight ring (or the resident layer, loaded once) and AS TMEM accumulator stages let the TMA producer, the MMA
-// issuer and the epilogue warps work on three different tiles at the same time.
-// H1: single halo box per block, horizontal taps as 128-byte descriptor start offsets (see conv_tc_sw.cu)
-template <int MODE, int TPS, int J, int KS, int H1>
-__global__ void __launch_bounds__(NUM_THREADS, 1)
-conv3x3_tc_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ CUtensorMap tmap_y,
-                  const __grid_constant__ CUtensorMap tmap_r, const TcParams p) {
+// The nine taps x four K-steps of one 64-channel block for warpgroup wg: halo stage at halo_a, the block's packed
+// weights [tap][NT][64] at w_a.
+template <int MODE, int NT, int NACC>
+__device__ __forceinline__ void mma_block(float (&acc)[NACC][NT / 2], uint32_t halo_a, uint32_t w_a, int wg) {
+  wgmma_fence();
+#pragma unroll
+  for (int t = 0; t < 9; ++t) {
+    int ry, rx, ph;
+    tap_route<MODE>(t, ry, rx, ph);
+    const uint32_t a0 = halo_a + (uint32_t)(((8 * wg + ry) * HALO_COLS + rx) * 128);
+    const uint32_t b0 = w_a + (uint32_t)t * (uint32_t)NT * 128u;
+#pragma unroll
+    for (int k = 0; k < CB / 16; ++k)
+      Wgmma<NT, 0, 0>::run(acc[ph], gmma_desc_sw128(a0 + 32u * k, 16u, HALO_COLS * 128u), gmma_desc_sw128(b0 + 32u * k, 16u, 1024u), 1u);
+  }
+  wgmma_commit();
+  wgmma_wait_all();
+}
+
+// Epilogue of one tile: this thread holds pixels (row 8 wg + 2 wq + i, column lane / 4), channels 8 j + 2 (lane % 4) + {0, 1}
+// of the NT-channel slice starting at n0.  bias points at that slice.
+template <int MODE, int NT, int NACC>
+__device__ __forceinline__ void epilogue(const float (&acc)[NACC][NT / 2], const TcParams& p, const float* bias, int n0, int n,
+                                         int y0, int x0) {
+  const int tid = threadIdx.x, wg = tid >> 7, wq = (tid >> 5) & 3, lane = tid & 31;
+  const int ox_in = x0 + (lane >> 2);
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    const int oy_in = y0 + 8 * wg + 2 * wq + i;
+    const bool in_img = oy_in < p.H && ox_in < p.W;
+#pragma unroll
+    for (int ph = 0; ph < NACC; ++ph) {
+      const int OH = MODE == 1 ? 2 * p.H : p.H, OW = MODE == 1 ? 2 * p.W : p.W;
+      const int oy = MODE == 1 ? 2 * oy_in + (ph >> 1) : oy_in, ox = MODE == 1 ? 2 * ox_in + (ph & 1) : ox_in;
+      const size_t pix = ((size_t)n * OH + oy) * OW + ox;
+#pragma unroll
+      for (int j = 0; j < NT / 8; ++j) {
+        const int c = 8 * j + 2 * (lane & 3);
+        float v0 = teco_act(acc[ph][4 * j + 2 * i] + bias[c], p.act);
+        float v1 = teco_act(acc[ph][4 * j + 2 * i + 1] + bias[c + 1], p.act);
+        if (!in_img) continue;
+        if (p.out_f32) {
+          const int C = p.out_f32_c, ch = n0 + c;
+          if (ch < C)
+            p.out_f32[pix * C + ch] = (v0 + (p.res_f32 ? p.res_f32[pix * C + ch] : 0.f)) * p.post_scale + p.post_shift;
+          if (ch + 1 < C)
+            p.out_f32[pix * C + ch + 1] = (v1 + (p.res_f32 ? p.res_f32[pix * C + ch + 1] : 0.f)) * p.post_scale + p.post_shift;
+        }
+        if (p.y) {
+          const size_t o = pix * p.Cout + n0 + c;
+          if (p.res) {   // in-place residual (res == y) is safe: this thread reads the element before it writes it
+            const float2 r = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(p.res + o));
+            v0 += r.x;
+            v1 += r.y;
+          }
+          *reinterpret_cast<__nv_bfloat162*>(p.y + o) = __floats2bfloat162_rn(v0, v1);
+        }
+      }
+    }
+  }
+}
+
+template <int MODE, int NT>
+__global__ void __launch_bounds__(NUM_THREADS, MODE == 1 ? 1 : 2)
+conv3x3_wgmma_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
+  constexpr int NACC = MODE == 1 ? 4 : 1;
+  constexpr int NR = NT / 2;                    // accumulator registers per thread
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  uint8_t* ring = smem;                                                        // 2 stages
+  uint8_t* w_res = smem + 2 * (size_t)p.stage_bytes;                           // resident weights, all blocks
+  uint64_t* bars = reinterpret_cast<uint64_t*>(w_res + (p.resident ? (size_t)p.nblk * p.w_blk_bytes : 0));
+  uint64_t* full = bars;                                                       // [2]
+  uint64_t* w_full = bars + 2;
+  float* s_bias = reinterpret_cast<float*>(bars + 4);                          // [NT]
 
-  uint8_t* halo_base = smem;                                             // HST stages x 3 kx-copies
-  uint8_t* w_base = smem + (size_t)p.HST * p.halo_stage_bytes;           // WST weight slabs
-  uint64_t* bars = reinterpret_cast<uint64_t*>(w_base + (size_t)p.WST * p.w_slab_bytes);
-  uint64_t* halo_full = bars;                    // [MAX_HST]
-  uint64_t* halo_empty = bars + MAX_HST;         // [MAX_HST]
-  uint64_t* w_full = bars + 2 * MAX_HST;         // [MAX_WST]
-  uint64_t* w_empty = w_full + MAX_WST;          // [MAX_WST]
-  uint64_t* acc_full = w_empty + MAX_WST;        // [2]
-  uint64_t* acc_empty = acc_full + 2;            // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 2);
-  float* s_bias = reinterpret_cast<float*>(acc_empty + 3);   // [Ncta]
-  uint64_t* res_full = acc_empty + 3 + 128;      // [2] after 256 floats of bias
-  uint64_t* stage_free = res_full + 2;           // [4] the TMA store of this staging tile has finished reading it
-  uint64_t* out_full = res_full + 6;             // [4] all epilogue warps have written their part of the staging tile
-  // Staged epilogue: two staging tiles (tile it uses it & 1), each J x [128 pixels][128 B] in the SWIZZLE_128B image of the
-  // TMA box (64 ch, 8 px, 16 rows).  A residual tile is TMA-loaded INTO the staging tile and the epilogue adds in place
-  // (same thread, same address), so residual and output share one buffer and both are double-buffered.
-  // Transposed conv (MODE 1, J == 1): four staging tiles, one per output phase (each the 16x8 pixels of that phase).
-  uint8_t* stage_base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(res_full + 10) + 1023) & ~(uintptr_t)1023);
+  const int tid = threadIdx.x, wg = tid >> 7;
+  const int n0 = blockIdx.y * NT;
+  const int G = gridDim.x;
+  const int my_tiles = (int)blockIdx.x < p.num_tiles ? (p.num_tiles - (int)blockIdx.x + G - 1) / G : 0;
+  const int nsteps = my_tiles * p.nblk;
 
-  // work assignment: grid = nsplit x G CTAs; CTA c of a split owns tiles c, c+G, ...
-  const int c_in_split = blockIdx.x % p.G;
-  const int n0 = (blockIdx.x / p.G) * p.Ncta;   // first output channel of this CTA (all CTAs of a cluster share it)
-  const int my_tiles = c_in_split < p.num_tiles ? (p.num_tiles - c_in_split + p.G - 1) / p.G : 0;
-  long long* dbg = p.dbg ? p.dbg + (size_t)blockIdx.x * 64 : nullptr;   // [0,32) phase stamps, [32,64) per-tile stamps
-#define STAMP(i) do { if (dbg) dbg[i] = clock64(); } while (0)
-#define TSTAMP(it, i) do { if (dbg && (it) < 8) dbg[32 + (it) * 4 + (i)] = clock64(); } while (0)
-  if (threadIdx.x == 0) STAMP(0);
-
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < p.HST; ++i) {
-      mbar_init(smem_u32(&halo_full[i]), 1);
-      mbar_init(smem_u32(&halo_empty[i]), 1);
-    }
-    for (int i = 0; i < p.WST; ++i) {
-      mbar_init(smem_u32(&w_full[i]), 1);
-      mbar_init(smem_u32(&w_empty[i]), 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(smem_u32(&acc_full[i]), 1);
-      mbar_init(smem_u32(&acc_empty[i]), NUM_EPI_WARPS);
-    }
-    for (int i = 0; i < 4; ++i) {
-      if (i < 2) mbar_init(smem_u32(&res_full[i]), 1);
-      mbar_init(smem_u32(&stage_free[i]), 1);
-      mbar_init(smem_u32(&out_full[i]), NUM_EPI_WARPS);
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap) : "memory");
-    if (p.tma_out) asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_y) : "memory");
-    if (p.tma_res) asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_r) : "memory");
+  for (int c = tid; c < NT; c += NUM_THREADS) s_bias[c] = p.bias ? p.bias[n0 + c] : 0.f;
+  if (tid == 0) {
+    mbar_init(smem_u32(&full[0]), 1);
+    mbar_init(smem_u32(&full[1]), 1);
+    mbar_init(smem_u32(w_full), 1);
+    fence_mbar_init();
   }
-  if (warp == 1) {  // TMEM allocation (one full warp), result lands in smem
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)),
-                 "r"(p.tmem_cols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tcgen05_fence_before();
-  if (p.CS > 1) cluster_sync_all();   // every CTA's mbarriers are initialised before any multicast may signal them
-  else __syncthreads();
-  tcgen05_fence_after();
-  pdl_launch_dependents();
-  const uint32_t tmem_base = *tmem_slot;
-  if (threadIdx.x == 0) STAMP(1);
-
-  // MODE 2 ("kx-fused" conv for a narrow output: Cout padded to 16): ONE tcgen05.mma covers the three horizontal taps of a
-  // kernel row -- B = [3 taps x Ncta] rows (the packed slab of row ky as it is), N = 3*Ncta, A = the halo pixels of the
-  // sub-tile WITHOUT a horizontal shift.  D block kx at halo column c then holds tap kx's contribution to output column
-  // c - kx, and the epilogue forms out(x) = D0(x) + D1(x+1) + D2(x+2) with warp shuffles.  A tile is 8J halo columns wide and
-  // yields 8J-2 output columns.  Why: an MMA costs ~60 clk whatever N is (the 4 KB A tile read bounds it), so the 64->3
-  // output stage at HR resolution used to cost as much per pixel as a 64->64 layer; this needs 12 MMAs per sub-tile, not 36.
-  constexpr int nacc = MODE == 1 ? 4 : (MODE == 2 ? 3 : 1);
-  constexpr int ncopies = H1 ? 1 : (MODE == 1 ? 2 : 3);   // horizontal tap offsets that occur (tconv only reads x-1, x)
-  constexpr int slabs_per_blk = 9 / TPS;
-  constexpr int row_bytes = ((H1 && MODE != 2) ? 8 * J + 2 : 8 * J) * 128;   // one box row (pixels x 128 B)
-  constexpr int tile_w = MODE == 2 ? 8 * J - 2 : 8 * J;                      // output columns per tile
-  constexpr uint32_t copy_bytes = (uint32_t)(HALO_ROWS * row_bytes);
-  const int slabs_per_tile = slabs_per_blk * p.nblk;
-  const uint32_t acc_stage_cols = (uint32_t)(J * nacc * KS * p.Ncta);   // TMEM columns of one accumulator stage
+  __syncthreads();
 
   auto tile_coords = [&](int it, int& n, int& y0, int& x0) {
-    int tile = c_in_split + it * p.G;
+    int tile = (int)blockIdx.x + it * G;
     const int tx = tile % p.tiles_x;
     tile /= p.tiles_x;
     const int ty = tile % p.tiles_y;
     n = tile / p.tiles_y;
-    x0 = tx * tile_w;
+    x0 = tx * TILE_COLS;
     y0 = ty * TILE_ROWS;
   };
-
-  if (warp == 0) {
-    // ===================== TMA producer =====================
-    // Issue cost of one bulk/tensor copy is a few hundred cycles, so independent copies are issued by different lanes.
-    if (p.mcast) {
-      // Resident weights (whole layer fits): they do not depend on the previous layer -> fetch them once, before the
-      // dependency wait.  With CS > 1 each CTA of the cluster fetches 1/CS of every slab and multicasts it.
-      const int sidx = lane;
-      if (sidx < slabs_per_tile) {
-        const uint32_t crank = p.CS > 1 ? cluster_ctarank() : 0;
-        const uint32_t part = p.w_slab_bytes / (uint32_t)p.CS;
-        const uint16_t mask = (uint16_t)((1u << p.CS) - 1u);
-        const int b = sidx / slabs_per_blk, g = sidx - slabs_per_blk * b;
-        mbar_expect_tx(smem_u32(&w_full[sidx]), p.w_slab_bytes);
-        // global layout [blk][tap][cout][64]: a slab = TPS consecutive taps of one block (TPS == 3 only when nsplit == 1)
-        const uint8_t* src = p.wpk + ((size_t)(b * 9 + g * TPS) * p.Cout + n0) * 128 + (size_t)crank * part;
-        const uint32_t dst = smem_u32(w_base + (size_t)sidx * p.w_slab_bytes) + crank * part;
-        if (p.CS > 1) bulk_load_1d_mcast(dst, src, part, smem_u32(&w_full[sidx]), mask);
-        else bulk_load_1d(dst, src, part, smem_u32(&w_full[sidx]));
-      }
-      __syncwarp();
+  const uint32_t tap_bytes = (uint32_t)NT * 128u;
+  // step s = (tile s / nblk, channel block s % nblk) into ring stage s & 1; issued by thread 0
+  auto issue = [&](int s) {
+    const int st = s & 1, it = s / p.nblk, b = s - it * p.nblk;
+    int n, y0, x0;
+    tile_coords(it, n, y0, x0);
+    uint8_t* base = ring + (size_t)st * p.stage_bytes;
+    const uint32_t bar = smem_u32(&full[st]);
+    mbar_expect_tx(bar, HALO_BYTES + (p.resident ? 0u : p.w_blk_bytes));
+    tma_load_4d(smem_u32(base), &tmap, bar, b * CB, x0 - 1, y0 - 1, n);
+    if (!p.resident)
+      for (int t = 0; t < 9; ++t)
+        bulk_load_1d(smem_u32(base + HALO_STAGE + t * tap_bytes), p.wpk + ((size_t)(b * 9 + t) * p.Cout + n0) * 128, tap_bytes, bar);
+  };
+  if (tid == 0 && nsteps > 0) {
+    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap) : "memory");
+    if (p.resident) {
+      mbar_expect_tx(smem_u32(w_full), (uint32_t)p.nblk * p.w_blk_bytes);
+      for (int bt = 0; bt < 9 * p.nblk; ++bt)
+        bulk_load_1d(smem_u32(w_res + (size_t)bt * tap_bytes), p.wpk + ((size_t)bt * p.Cout + n0) * 128, tap_bytes, smem_u32(w_full));
     }
-    // Ring mode: slab sequence q = 0 .. my_tiles*slabs_per_tile-1 through WST stages; the first WST do not depend on
-    // the previous layer either -> issue them before the wait.
-    const int total_slabs = my_tiles * slabs_per_tile;
-    int next_slab = 0;
-    auto issue_slab = [&](int q) {
-      const int st = q % p.WST, use = q / p.WST, sl = q % slabs_per_tile;
-      const int b = sl / slabs_per_blk, g = sl - slabs_per_blk * b;
-      if (use > 0) mbar_wait(smem_u32(&w_empty[st]), (uint32_t)((use - 1) & 1));   // MMAs of the previous use have retired
-      mbar_expect_tx(smem_u32(&w_full[st]), p.w_slab_bytes);
-      const uint8_t* src = p.wpk + ((size_t)(b * 9 + g * TPS) * p.Cout + n0) * 128;
-      bulk_load_1d(smem_u32(w_base + (size_t)st * p.w_slab_bytes), src, p.w_slab_bytes, smem_u32(&w_full[st]));
-    };
-    if (!p.mcast && lane == 0)
-      for (; next_slab < total_slabs && next_slab < p.WST; ++next_slab) issue_slab(next_slab);
-    if (lane == 0) STAMP(9);
-    pdl_wait();   // the previous kernel's output (our input x) is complete and visible from here on
-    if (lane == 0) STAMP(10);
-    int hs = 0;
-    uint32_t hph = 0;
-    for (int it = 0; it < my_tiles; ++it) {
+    issue(0);
+  }
+  if (p.resident && nsteps > 0) mbar_wait(smem_u32(w_full), 0);
+
+  float acc[NACC][NR];
+  for (int s = 0; s < nsteps; ++s) {
+    const int it = s / p.nblk, b = s - it * p.nblk;
+    if (tid == 0 && s + 1 < nsteps) issue(s + 1);   // its stage was released by the __syncthreads() closing step s - 1
+    if (b == 0) {
+#pragma unroll
+      for (int a = 0; a < NACC; ++a)
+#pragma unroll
+        for (int r = 0; r < NR; ++r) acc[a][r] = 0.f;
+    }
+    mbar_wait(smem_u32(&full[s & 1]), (uint32_t)((s >> 1) & 1));
+    uint8_t* base = ring + (size_t)(s & 1) * p.stage_bytes;
+    const uint32_t halo_a = smem_u32(base);
+    const uint32_t w_a = p.resident ? smem_u32(w_res + (size_t)b * p.w_blk_bytes) : smem_u32(base + HALO_STAGE);
+    mma_block<MODE, NT, NACC>(acc, halo_a, w_a, wg);
+    if (b == p.nblk - 1) {
       int n, y0, x0;
       tile_coords(it, n, y0, x0);
-      for (int b = 0; b < p.nblk; ++b) {
-        if (lane == 0) {
-          mbar_wait(smem_u32(&halo_empty[hs]), hph ^ 1);
-          mbar_expect_tx(smem_u32(&halo_full[hs]), copy_bytes * ncopies);
-        }
-        __syncwarp();
-        if (lane < ncopies)
-          tma_load_4d(smem_u32(halo_base + (size_t)hs * p.halo_stage_bytes + (size_t)lane * copy_bytes), &tmap,
-                      smem_u32(&halo_full[hs]), b * CB, x0 - 1 + lane, y0 - 1, n);
-        if (!p.mcast && lane == 0)   // slabs up to the end of this block that are not in flight yet
-          for (; next_slab < it * slabs_per_tile + (b + 1) * slabs_per_blk; ++next_slab) issue_slab(next_slab);
-        __syncwarp();
-        if (++hs == p.HST) { hs = 0; hph ^= 1; }
-      }
-      if (p.tma_res) {   // residual tile(s) of this output tile straight into staging tile it & 1: free once the store of tile it - 2 has read it
-        const int sg = it & 1;
-        if (lane == 0) {
-          mbar_wait(smem_u32(&stage_free[sg]), (uint32_t)(((it >> 1) & 1) ^ 1));
-          mbar_expect_tx(smem_u32(&res_full[sg]), (uint32_t)(J * 16384));
-        }
-        __syncwarp();
-        if (lane < J)
-          tma_load_4d(smem_u32(stage_base + (size_t)(sg * J + lane) * 16384), &tmap_r, smem_u32(&res_full[sg]), n0, x0 + 8 * lane, y0, n);
-      }
+      epilogue<MODE, NT, NACC>(acc, p, s_bias, n0, n, y0, x0);
     }
-    if (my_tiles == 0 && p.mcast && lane == 0) {
-      // padding CTA of a cluster: it only relays its share of the weights; stay until they have landed here too
-      for (int sidx = 0; sidx < slabs_per_tile; ++sidx) mbar_wait(smem_u32(&w_full[sidx]), 0);
+    __syncthreads();   // every warpgroup's MMAs on this stage have completed: it may be refilled
+  }
+}
+
+// ------------------------------------------------------------------ multi-layer chain (generator trunk)
+// L consecutive 3x3 64 -> 64 layers (bias, ReLU / LeakyReLU / none, optional residual) on 32-pixel-wide images in ONE
+// launch.  CTA c owns images c, c + G, ... for EVERY layer, so the input tiles of layer l + 1 were written by this very
+// CTA: a CTA-wide barrier (after a generic -> async proxy fence, because the next layer's halo arrives by TMA) is the only
+// dependency between layers, there is no grid-wide one and no kernel boundary.  Weights of layer l + 1 are in flight in
+// the second weight buffer while layer l computes; within a layer the halo of the next tile is in flight while the
+// current one runs its MMAs and epilogue.  Same MMA and epilogue code as conv3x3_wgmma_kernel.
+constexpr int LIN_W = 32, LIN_ROWS = 4, LIN_MAX_LAYERS = 40;
+constexpr uint32_t LAYER_W_BYTES = 9u * 64u * 128u;   // one packed 64 x 64 layer: 73728
+
+struct ChainParams {
+  int N, H, L, tiles_y;
+  int8_t plan[LIN_MAX_LAYERS][4];   // input buffer, output buffer, residual buffer or -1, activation
+  __nv_bfloat16* bufs[3];
+  const uint8_t* wpk;
+  const float* bias;
+};
+
+__global__ void __launch_bounds__(NUM_THREADS, 1)
+conv3x3_chain_kernel(const __grid_constant__ CUtensorMap tmap0, const __grid_constant__ CUtensorMap tmap1,
+                     const __grid_constant__ CUtensorMap tmap2, const ChainParams p) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  uint8_t* ring = smem;                                   // 2 halo stages
+  uint8_t* wbuf = smem + 2 * HALO_STAGE;                  // 2 layers of weights
+  uint64_t* full = reinterpret_cast<uint64_t*>(wbuf + 2 * LAYER_W_BYTES);   // [2]
+  uint64_t* w_full = full + 2;                                              // [2]
+  const int tid = threadIdx.x, wg = tid >> 7;
+  const int G = gridDim.x;
+  const int tiles_per_image = (LIN_W / TILE_COLS) * p.tiles_y;
+  const int my_images = (int)blockIdx.x < p.N ? (p.N - (int)blockIdx.x + G - 1) / G : 0;
+  const int T = my_images * tiles_per_image;              // tiles of this CTA per layer
+  const int nsteps = p.L * T;
+
+  if (tid == 0) {
+    for (int i = 0; i < 2; ++i) {
+      mbar_init(smem_u32(&full[i]), 1);
+      mbar_init(smem_u32(&w_full[i]), 1);
     }
-    __syncwarp();
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    const uint32_t idesc = umma_idesc(p.Ncta);
-    constexpr uint32_t a_sbo = (uint32_t)row_bytes;   // next 8-pixel group of the M=128 sub-tile = next image row
-    constexpr uint32_t b_sbo = 1024u;                 // next 8 output channels
-    int hs = 0, ws = 0;
-    uint32_t hph = 0, wph = 0;
-    for (int it = 0; it < my_tiles; ++it) {
-      const int as = (p.AS == 2) ? (it & 1) : 0;
-      const uint32_t ause = (uint32_t)((p.AS == 2) ? (it >> 1) : it);
-      mbar_wait_warp(smem_u32(&acc_empty[as]), (ause & 1u) ^ 1u);   // the epilogue has drained this accumulator stage
-      tcgen05_fence_after();
-      const uint32_t tmem_acc = tmem_base + (uint32_t)as * acc_stage_cols;
-      uint32_t started = 0;  // bit (j*nacc+phase): accumulator already written once (for this tile)
-      for (int b = 0; b < p.nblk; ++b) {
-        mbar_wait_warp(smem_u32(&halo_full[hs]), hph);
-        tcgen05_fence_after();
-        if (lane == 0 && b == 0 && it == 0) STAMP(2);
-        if (lane == 0 && b == 0) TSTAMP(it, 0);
-        const uint32_t halo_addr = smem_u32(halo_base + (size_t)hs * p.halo_stage_bytes);
-        for (int g = 0; g < slabs_per_blk; ++g) {
-          if (p.mcast) {   // resident: slab index is fixed, the barrier completes exactly once
-            ws = b * slabs_per_blk + g;
-            if (it == 0) mbar_wait_warp(smem_u32(&w_full[ws]), 0);
-          } else {
-            mbar_wait_warp(smem_u32(&w_full[ws]), wph);
-          }
-          tcgen05_fence_after();
-          if (lane == 0 && b == 0 && it == 0) STAMP(16 + g);
-          if (MODE == 2) {
-            const uint32_t slab_addr = smem_u32(w_base + (size_t)ws * p.w_slab_bytes);
-            const uint64_t a_row = umma_desc_sw128(halo_addr, a_sbo) + (uint64_t)((uint32_t)(g * row_bytes) >> 4);
-            const uint64_t b3 = umma_desc_sw128(slab_addr, b_sbo);
-            const uint32_t idesc3 = umma_idesc(3 * p.Ncta);
-            const uint32_t first = (b == 0 && g == 0) ? 1u : 0u;
-            if (elect_one()) {
-#pragma unroll
-              for (int s = 0; s < CB / 16; ++s)
-#pragma unroll
-                for (int j = 0; j < J; ++j)
-                  umma_bf16(tmem_acc + (uint32_t)(j * 3) * (uint32_t)p.Ncta, a_row + (uint32_t)((j * 1024 + s * 32) >> 4),
-                            b3 + (uint32_t)((s * 32) >> 4), idesc3, (first && s == 0) ? 0u : 1u);
-            }
-            __syncwarp();
-          } else {
-            // Whole (converged) warp computes the warp-uniform bases; one elected lane issues the unrolled MMA stream.
-            const uint32_t slab_addr = smem_u32(w_base + (size_t)ws * p.w_slab_bytes);
-            const uint64_t a_base = umma_desc_sw128(halo_addr, a_sbo);
-            const uint64_t b_base = umma_desc_sw128(slab_addr, b_sbo);
-            const uint32_t tap_stride16 = (uint32_t)(p.Ncta * 128) >> 4;   // weight bytes per tap, in descriptor units
-            // per-tap row/copy/phase (TPS == 3: ky = g, kx = tt; TPS == 1: tap = g)
-            uint32_t a_off16[TPS], acc_idx[TPS];
-#pragma unroll
-            for (int tt = 0; tt < TPS; ++tt) {
-              const int t = g * TPS + tt;
-              const int ky = (TPS == 3) ? g : t / 3, kx = (TPS == 3) ? tt : t - 3 * (t / 3);
-              int ry, rx, phase;
-              if (MODE == 1) {  // transposed conv: tap -> (input offset, output phase)
-                ry = (ky == 2) ? 0 : 1;
-                rx = (kx == 2) ? 0 : 1;
-                phase = ((ky == 1) ? 2 : 0) + ((kx == 1) ? 1 : 0);
-              } else {
-                ry = ky; rx = kx; phase = 0;
-              }
-              a_off16[tt] = H1 ? ((uint32_t)(rx * 128 + ry * row_bytes)) >> 4
-                               : ((uint32_t)rx * copy_bytes + (uint32_t)(ry * row_bytes)) >> 4;
-              acc_idx[tt] = (uint32_t)(phase * KS);   // first chain of this tap's accumulator
-            }
-            // K-split chain of an MMA: KS == 3 -> the tap within the slab (kx), KS == 2 -> parity of the k-step.
-            // Order k-step, tap, sub-tile: consecutive MMAs hit J x KS different accumulators (dependent MMAs on one
-            // accumulator cost ~125 cycles each; 3 chains ~72, 6 chains ~59: profiles/conv_tc_r01_notes.md).
-            const uint32_t started_now = started;
-            uint32_t touched = 0;
-#pragma unroll
-            for (int s = 0; s < CB / 16; ++s)
-#pragma unroll
-              for (int tt = 0; tt < TPS; ++tt)
-#pragma unroll
-                for (int j = 0; j < J; ++j)
-                  touched |= 1u << ((uint32_t)(j * nacc * KS) + acc_idx[tt] + (uint32_t)(KS == 3 ? tt : (KS == 2 ? (s & 1) : 0)));
-            if (elect_one()) {
-              uint32_t seen = started_now;   // accumulators written so far (this tile); folds to constants when unrolled
-#pragma unroll
-              for (int s = 0; s < CB / 16; ++s) {
-#pragma unroll
-                for (int tt = 0; tt < TPS; ++tt) {
-#pragma unroll
-                  for (int j = 0; j < J; ++j) {
-                    const uint32_t acc = (uint32_t)(j * nacc * KS) + acc_idx[tt] + (uint32_t)(KS == 3 ? tt : (KS == 2 ? (s & 1) : 0));
-                    const uint32_t accum = (seen >> acc) & 1u;
-                    seen |= 1u << acc;
-                    umma_bf16(tmem_acc + acc * (uint32_t)p.Ncta, a_base + a_off16[tt] + (uint32_t)((j * 1024 + s * 32) >> 4),
-                              b_base + tt * tap_stride16 + (uint32_t)((s * 32) >> 4), idesc, accum);
-                  }
-                }
-              }
-            }
-            __syncwarp();
-            started |= touched;
-            if (!p.mcast && elect_one()) tcgen05_commit(smem_u32(&w_empty[ws]));  // frees the slab when these MMAs retire
-          }
-          __syncwarp();
-          if (!p.mcast && ++ws == p.WST) { ws = 0; wph ^= 1; }
-        }
-        if (elect_one()) tcgen05_commit(smem_u32(&halo_empty[hs]));
-        __syncwarp();
-        if (++hs == p.HST) { hs = 0; hph ^= 1; }
-      }
-      if (elect_one()) tcgen05_commit(smem_u32(&acc_full[as]));
-      if (lane == 0 && it == 0) STAMP(5);
-      if (lane == 0) TSTAMP(it, 1);
-      __syncwarp();
-    }
-  } else if (warp == STORE_WARP) {
-    // ===================== output store (staged epilogue only) =====================
-    if (MODE == 0 && p.tma_out && lane == 0) {
-      for (int it = 0; it < my_tiles; ++it) {
-        int n, y0, x0;
-        tile_coords(it, n, y0, x0);
-        const int sg = it & 1;
-        mbar_wait(smem_u32(&out_full[sg]), (uint32_t)((it >> 1) & 1));   // every epilogue warp has fenced and arrived
-        for (int j = 0; j < J; ++j) tma_store_4d(&tmap_y, smem_u32(stage_base + (size_t)(sg * J + j) * 16384), n0, x0 + 8 * j, y0, n);
-        bulk_commit();
-        bulk_wait_read();                                                 // the staging tile may be overwritten again
-        mbar_arrive(smem_u32(&stage_free[sg]));
-      }
-    }
-    if (MODE == 1 && p.tma_out && lane == 0) {
-      for (int it = 0; it < my_tiles; ++it) {
-        int n, y0, x0;
-        tile_coords(it, n, y0, x0);
-        for (int ph = 0; ph < 4; ++ph) {   // one 16x8-pixel box per sub-pixel phase through the 5-D map {C, px, x, py, n*H + y}
-          mbar_wait(smem_u32(&out_full[ph]), (uint32_t)(it & 1));
-          tma_store_5d(&tmap_y, smem_u32(stage_base + (size_t)ph * 16384), n0, ph & 1, x0, ph >> 1, n * p.H + y0);
-          bulk_commit();
-          bulk_wait_read();
-          mbar_arrive(smem_u32(&stage_free[ph]));
-        }
-      }
-    }
-    __syncwarp();
-  } else {
-    // ===================== epilogue (warps 2..9) =====================
-    for (int c = (int)threadIdx.x - 64; c < p.Ncta; c += 32 * NUM_EPI_WARPS) s_bias[c] = p.bias ? p.bias[n0 + c] : 0.f;
-    asm volatile("bar.sync 1, %0;" ::"n"(32 * NUM_EPI_WARPS) : "memory");   // the epilogue warps only
-    pdl_wait();                                        // res / y belong to the dependency chain
-    if (threadIdx.x == 64) STAMP(25);
-    const int q = warp & 3;            // TMEM lane quarter this warp may access
-    const int chalf = (warp - 2) >> 2; // which half of the channel steps this warp takes (0 or 1)
-    const int m = 32 * q + lane;       // accumulator row = pixel within the 16x8 sub-tile
-    const int ry = m >> 3, rx = m & 7;
-    const float act_slope = p.act == TECO_ACT_RELU ? 0.f : (p.act == TECO_ACT_LRELU02 ? 0.2f : 1.f);
-    // EW output channels per step: 32 (two steps for 64 channels) or 16 (the 16-channel fp32 output stage)
-    auto run = [&](auto ew_tag) {
-      constexpr int EW = decltype(ew_tag)::value;
-      for (int it = 0; it < my_tiles; ++it) {
-        int n, y0, x0;
-        tile_coords(it, n, y0, x0);
-        const int as = (p.AS == 2) ? (it & 1) : 0;
-        const uint32_t ause = (uint32_t)((p.AS == 2) ? (it >> 1) : it);
-        mbar_wait_warp(smem_u32(&acc_full[as]), ause & 1u);
-        tcgen05_fence_after();
-        if (threadIdx.x == 64 && it == 0) STAMP(6);
-        if (threadIdx.x == 64) TSTAMP(it, 2);
-        const uint32_t tmem_acc = tmem_base + (uint32_t)as * acc_stage_cols;
-        const int oy_in = y0 + ry;
-        for (int j = 0; j < J; ++j) {
-          const int ox_in = x0 + 8 * j + rx;
-          const bool in_img = (oy_in < p.H) && (ox_in < p.W);
-          for (int ph = 0; ph < nacc; ++ph) {
-            int oy, ox, OH, OW;
-            if (MODE == 1) {
-              oy = 2 * oy_in + (ph >> 1); ox = 2 * ox_in + (ph & 1); OH = 2 * p.H; OW = 2 * p.W;
-            } else {
-              oy = oy_in; ox = ox_in; OH = p.H; OW = p.W;
-            }
-            const size_t pix = ((size_t)n * OH + oy) * OW + ox;
-            const uint32_t tcol = tmem_acc + ((uint32_t)(32 * q) << 16) + (uint32_t)((j * nacc + ph) * KS * p.Ncta);
-            for (int c0 = chalf * EW; c0 < p.Ncta; c0 += 2 * EW) {
-              uint32_t r[EW];
-              __syncwarp();
-              if (EW == 32) tmem_ld32(tcol + (uint32_t)c0, r); else tmem_ld16(tcol + (uint32_t)c0, r);
-              if (KS == 3) {   // K-split chains: issue all the TMEM loads, wait once, add
-                uint32_t r2[EW], r3[EW];
-                if (EW == 32) { tmem_ld32(tcol + (uint32_t)(p.Ncta + c0), r2); tmem_ld32(tcol + (uint32_t)(2 * p.Ncta + c0), r3); }
-                else { tmem_ld16(tcol + (uint32_t)(p.Ncta + c0), r2); tmem_ld16(tcol + (uint32_t)(2 * p.Ncta + c0), r3); }
-                tmem_wait_ld();
-#pragma unroll
-                for (int i = 0; i < EW; ++i)
-                  r[i] = __float_as_uint(__uint_as_float(r[i]) + __uint_as_float(r2[i]) + __uint_as_float(r3[i]));
-              } else if (KS == 2) {
-                uint32_t r2[EW];
-                if (EW == 32) tmem_ld32(tcol + (uint32_t)(p.Ncta + c0), r2); else tmem_ld16(tcol + (uint32_t)(p.Ncta + c0), r2);
-                tmem_wait_ld();
-#pragma unroll
-                for (int i = 0; i < EW; ++i) r[i] = __float_as_uint(__uint_as_float(r[i]) + __uint_as_float(r2[i]));
-              } else {
-                tmem_wait_ld();
-              }
-              if (threadIdx.x == 64 && it == 0 && j == 0 && ph == 0 && c0 == 0) STAMP(11);
-              // last TMEM read of this tile by this warp -> hand the accumulator stage back to the MMA issuer
-              if (j == J - 1 && ph == nacc - 1 && c0 + 2 * EW >= p.Ncta) {
-                tcgen05_fence_before();
-                if (lane == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(&acc_empty[as])) : "memory");
-              }
-              float v[EW];
-#pragma unroll
-              for (int i = 0; i < EW; ++i) {
-                const float a = __uint_as_float(r[i]) + s_bias[c0 + i];
-                v[i] = fmaxf(a, a * act_slope);      // none: slope 1, relu: 0, lrelu: 0.2 -- no per-element branch
-              }
-              if (p.act >= TECO_ACT_TANH24) {        // uniform, outside the element loop; rare (FNet head).  Unrolled: a rolled
-#pragma unroll                                       // loop indexes v[] dynamically and drags it into local memory for every layer
-                for (int i = 0; i < EW; ++i) v[i] = teco_act(v[i], p.act);
-              }
-              if (!in_img) continue;
-              if (p.out_f32) {
-#pragma unroll
-                for (int i = 0; i < EW; ++i) {
-                  const int c = n0 + c0 + i;
-                  if (c < p.out_f32_c) {
-                    const float a = v[i] + (p.res_f32 ? p.res_f32[pix * p.out_f32_c + c] : 0.f);
-                    p.out_f32[pix * p.out_f32_c + c] = a * p.post_scale + p.post_shift;
-                  }
-                }
-              }
-              if (p.y) {
-                if (p.res) {
-                  const uint4* rp = reinterpret_cast<const uint4*>(p.res + pix * p.Cout + n0 + c0);
-#pragma unroll
-                  for (int k = 0; k < EW / 8; ++k) {
-                    const uint4 rr = rp[k];
-                    const uint32_t rw[4] = {rr.x, rr.y, rr.z, rr.w};
-#pragma unroll
-                    for (int i = 0; i < 4; ++i) {
-                      float2 f = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&rw[i]));
-                      v[8 * k + 2 * i] += f.x;
-                      v[8 * k + 2 * i + 1] += f.y;
-                    }
-                  }
-                }
-                uint4* yp = reinterpret_cast<uint4*>(p.y + pix * p.Cout + n0 + c0);
-#pragma unroll
-                for (int k = 0; k < EW / 8; ++k) {
-                  uint32_t o[4];
-#pragma unroll
-                  for (int i = 0; i < 4; ++i) {
-                    __nv_bfloat162 h = __floats2bfloat162_rn(v[8 * k + 2 * i], v[8 * k + 2 * i + 1]);
-                    o[i] = *reinterpret_cast<uint32_t*>(&h);
-                  }
-                  yp[k] = make_uint4(o[0], o[1], o[2], o[3]);
-                }
-              }
-              if (threadIdx.x == 64 && it == 0 && j == 0 && ph == 0) STAMP(12 + ((c0 / EW) & 3));
-            }
-          }
-        }
-        if (threadIdx.x == 64) TSTAMP(it, 3);
-        // warps with no channel step of their own (16-channel output stage: chalf == 1) still release the stage
-        if (chalf * EW >= p.Ncta) {
-          if (lane == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(&acc_empty[as])) : "memory");
-        }
-      }
-    };
-    if (MODE == 0 && p.tma_out) {
-      // ---- staged epilogue (Ncta == 64): this warp owns channels [32*chalf, +32) of pixel row m of every sub-tile.
-      // TMEM -> registers -> (+ bias, activation, + residual read from the staging tile) -> bf16 into the staging tile in
-      // place; the store warp sends the tile out.  The TMEM loads of sub-tile 1 are in flight while sub-tile 0 is
-      // processed (the epilogue was latency-bound: load -> wait -> math -> store per step, ~2300 clk per step).
-      constexpr bool PREF = (J == 2 && KS <= 2);
-      const uint32_t rowoff = (uint32_t)m * 128u, sw = (uint32_t)m & 7u;
-      float bias_r[32];      // this thread's 32 output channels: registers, not a shared-memory read per tile (the L1/smem
-#pragma unroll             // data pipe is what bounds this kernel: 48 operand wavefronts per N=64 MMA)
-      for (int i = 0; i < 32; ++i) bias_r[i] = s_bias[32 * chalf + i];
-      auto process = [&](uint32_t (&r)[KS][32], uint8_t* tile) {
-        float v[32];
-#pragma unroll
-        for (int i = 0; i < 32; ++i) {
-          float a = __uint_as_float(r[0][i]);
-#pragma unroll
-          for (int k = 1; k < KS; ++k) a += __uint_as_float(r[k][i]);
-          a += bias_r[i];
-          v[i] = fmaxf(a, a * act_slope);      // none: slope 1, relu: 0, lrelu: 0.2 -- no per-element branch
-        }
-        uint8_t* row = tile + rowoff;   // (tanh/sigmoid layers never take the staged path: a rolled loop would put v[] in local memory)
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          uint4* cell = reinterpret_cast<uint4*>(row + ((((uint32_t)(4 * chalf + k)) ^ sw) << 4));   // XOR swizzle of the TMA box
-          if (p.tma_res) {
-            const uint4 rr = *cell;
-            const uint32_t rw[4] = {rr.x, rr.y, rr.z, rr.w};
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              const float2 f = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&rw[i]));
-              v[8 * k + 2 * i] += f.x;
-              v[8 * k + 2 * i + 1] += f.y;
-            }
-          }
-          uint32_t o[4];
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            __nv_bfloat162 h = __floats2bfloat162_rn(v[8 * k + 2 * i], v[8 * k + 2 * i + 1]);
-            o[i] = *reinterpret_cast<uint32_t*>(&h);
-          }
-          *cell = make_uint4(o[0], o[1], o[2], o[3]);
-        }
-      };
-      for (int it = 0; it < my_tiles; ++it) {
-        const int as = (p.AS == 2) ? (it & 1) : 0;
-        const uint32_t ause = (uint32_t)((p.AS == 2) ? (it >> 1) : it);
-        const int sg = it & 1;
-        const uint32_t suse = (uint32_t)(it >> 1);
-        mbar_wait_warp(smem_u32(&acc_full[as]), ause & 1u);
-        tcgen05_fence_after();
-        if (threadIdx.x == 64 && it == 0) STAMP(6);
-        if (threadIdx.x == 64) TSTAMP(it, 2);
-        const uint32_t tb = tmem_base + (uint32_t)as * acc_stage_cols + ((uint32_t)(32 * q) << 16) + (uint32_t)(32 * chalf);
-        auto release_acc = [&]() {     // last TMEM read of this tile by this warp -> hand the stage back to the MMA issuer
-          tcgen05_fence_before();
-          if (lane == 0) mbar_arrive(smem_u32(&acc_empty[as]));
-        };
-        uint8_t* tile0 = stage_base + (size_t)(sg * J) * 16384;
-        uint32_t ra[KS][32];
-#pragma unroll
-        for (int k = 0; k < KS; ++k) tmem_ld32(tb + (uint32_t)(k * 64), ra[k]);
-        tmem_wait_ld();
-        if (PREF) {
-          uint32_t rb[KS][32];
-#pragma unroll
-          for (int k = 0; k < KS; ++k) tmem_ld32(tb + (uint32_t)((KS + k) * 64), rb[k]);
-          // the staging tile: residual landed (which implies it was free), or free of the store of tile it - 2
-          if (p.tma_res) mbar_wait_warp(smem_u32(&res_full[sg]), suse & 1u);
-          else mbar_wait_warp(smem_u32(&stage_free[sg]), (suse & 1u) ^ 1u);
-          process(ra, tile0);
-          tmem_wait_ld();
-          release_acc();
-          process(rb, tile0 + 16384);
-        } else {
-          if (J == 1) release_acc();
-          if (p.tma_res) mbar_wait_warp(smem_u32(&res_full[sg]), suse & 1u);
-          else mbar_wait_warp(smem_u32(&stage_free[sg]), (suse & 1u) ^ 1u);
-          process(ra, tile0);
-          if (J == 2) {
-#pragma unroll
-            for (int k = 0; k < KS; ++k) tmem_ld32(tb + (uint32_t)((KS + k) * 64), ra[k]);
-            tmem_wait_ld();
-            release_acc();
-            process(ra, tile0 + 16384);
-          }
-        }
-        fence_async_smem();            // generic-proxy writes -> visible to the TMA store
-        __syncwarp();
-        if (lane == 0) mbar_arrive(smem_u32(&out_full[sg]));
-        if (threadIdx.x == 64) TSTAMP(it, 3);
-      }
-    } else if (MODE == 2) {
-      // ---- kx-fused narrow output stage (fp32 output, <= 4 channels): out(x) = D0(x) + D1(x+1) + D2(x+2)
-      const int C = p.out_f32_c;
-      for (int it = 0; it < my_tiles; ++it) {
-        int n, y0, x0;
-        tile_coords(it, n, y0, x0);
-        const int as = (p.AS == 2) ? (it & 1) : 0;
-        const uint32_t ause = (uint32_t)((p.AS == 2) ? (it >> 1) : it);
-        mbar_wait_warp(smem_u32(&acc_full[as]), ause & 1u);
-        tcgen05_fence_after();
-        if (threadIdx.x == 64) TSTAMP(it, 2);
-        const uint32_t tb = tmem_base + (uint32_t)as * acc_stage_cols + ((uint32_t)(32 * q) << 16);
-        uint32_t d[J][3][4];
-#pragma unroll
-        for (int j = 0; j < J; ++j)
-#pragma unroll
-          for (int kx = 0; kx < 3; ++kx) tmem_ld4(tb + (uint32_t)((j * 3 + kx) * p.Ncta), d[j][kx]);
-        tmem_wait_ld();
-        tcgen05_fence_before();
-        if (lane == 0) mbar_arrive(smem_u32(&acc_empty[as]));
-        const int oy = y0 + ry;
-#pragma unroll
-        for (int j = 0; j < J; ++j) {
-          float v[4];
-#pragma unroll
-          for (int c = 0; c < 4; ++c) {
-            // neighbours one and two halo columns to the right: the same sub-tile (lane + 1, + 2) or the next one (lane - 7, - 6)
-            const float s1 = __shfl_sync(0xffffffffu, __uint_as_float(d[j][1][c]), (lane + 1) & 31);
-            const float s2 = __shfl_sync(0xffffffffu, __uint_as_float(d[j][2][c]), (lane + 2) & 31);
-            float n1 = 0.f, n2 = 0.f;
-            if (j + 1 < J) {
-              n1 = __shfl_sync(0xffffffffu, __uint_as_float(d[j + 1 < J ? j + 1 : j][1][c]), (lane - 7) & 31);
-              n2 = __shfl_sync(0xffffffffu, __uint_as_float(d[j + 1 < J ? j + 1 : j][2][c]), (lane - 6) & 31);
-            }
-            const float a = __uint_as_float(d[j][0][c]) + (rx < 7 ? s1 : n1) + (rx < 6 ? s2 : n2) + s_bias[c];
-            v[c] = fmaxf(a, a * act_slope);
-          }
-          if (p.act >= TECO_ACT_TANH24) {
-#pragma unroll
-            for (int c = 0; c < 4; ++c) v[c] = teco_act(v[c], p.act);
-          }
-          const int tc = 8 * j + rx, ox = x0 + tc;
-          // the two warps of a lane quarter take alternate sub-tiles (no early exit: the shuffles above are warp-collective)
-          const bool mine = ((warp - 2) >> 2) == (j & 1) && tc < tile_w && ox < p.W && oy < p.H;
-          const size_t pix = ((size_t)n * p.H + oy) * p.W + ox;
-#pragma unroll
-          for (int c = 0; c < 4; ++c)
-            if (mine && c < C) {
-              const float a = v[c] + (p.res_f32 ? p.res_f32[pix * C + c] : 0.f);
-              p.out_f32[pix * C + c] = a * p.post_scale + p.post_shift;
-            }
-        }
-        if (threadIdx.x == 64) TSTAMP(it, 3);
-      }
-    } else if (MODE == 1 && p.tma_out) {
-      // ---- staged epilogue of the transposed conv (J == 1, KS == 1, Ncta == 64): the four phase accumulators of the tile
-      // one after the other, the next phase's TMEM load in flight while this one is converted and written to its staging tile
-      const uint32_t rowoff = (uint32_t)m * 128u, sw = (uint32_t)m & 7u;
-      float bias_r[32];
-#pragma unroll
-      for (int i = 0; i < 32; ++i) bias_r[i] = s_bias[32 * chalf + i];
-      for (int it = 0; it < my_tiles; ++it) {
-        const int as = (p.AS == 2) ? (it & 1) : 0;
-        const uint32_t ause = (uint32_t)((p.AS == 2) ? (it >> 1) : it);
-        mbar_wait_warp(smem_u32(&acc_full[as]), ause & 1u);
-        tcgen05_fence_after();
-        if (threadIdx.x == 64) TSTAMP(it, 2);
-        const uint32_t tb = tmem_base + (uint32_t)as * acc_stage_cols + ((uint32_t)(32 * q) << 16) + (uint32_t)(32 * chalf);
-        uint32_t r[2][32];
-        tmem_ld32(tb, r[0]);
-#pragma unroll
-        for (int ph = 0; ph < 4; ++ph) {
-          tmem_wait_ld();
-          if (ph < 3) {
-            tmem_ld32(tb + (uint32_t)((ph + 1) * 64), r[(ph + 1) & 1]);
-          } else {
-            tcgen05_fence_before();
-            if (lane == 0) mbar_arrive(smem_u32(&acc_empty[as]));
-          }
-          mbar_wait_warp(smem_u32(&stage_free[ph]), (uint32_t)((it & 1) ^ 1));
-          uint8_t* row = stage_base + (size_t)ph * 16384 + rowoff;
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            uint32_t o[4];
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              const float a0 = __uint_as_float(r[ph & 1][8 * k + 2 * i]) + bias_r[8 * k + 2 * i];
-              const float a1 = __uint_as_float(r[ph & 1][8 * k + 2 * i + 1]) + bias_r[8 * k + 2 * i + 1];
-              __nv_bfloat162 h = __floats2bfloat162_rn(fmaxf(a0, a0 * act_slope), fmaxf(a1, a1 * act_slope));
-              o[i] = *reinterpret_cast<uint32_t*>(&h);
-            }
-            *reinterpret_cast<uint4*>(row + ((((uint32_t)(4 * chalf + k)) ^ sw) << 4)) = make_uint4(o[0], o[1], o[2], o[3]);
-          }
-          fence_async_smem();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(smem_u32(&out_full[ph]));
-        }
-        if (threadIdx.x == 64) TSTAMP(it, 3);
-      }
-    } else if (p.Ncta % 32 == 0) run(std::integral_constant<int, 32>{});   // (a single EW = 16 instantiation halves the SASS but
-    else run(std::integral_constant<int, 16>{});                           //  measured 7.4 us vs 6.9 us on the 64->64 layer)
+    fence_mbar_init();
+  }
+  __syncthreads();
+  if (T == 0) return;
+
+  auto tile_coords = [&](int it, int& n, int& y0, int& x0) {
+    const int k = it / tiles_per_image, r = it - k * tiles_per_image;
+    n = (int)blockIdx.x + k * G;
+    x0 = (r % (LIN_W / TILE_COLS)) * TILE_COLS;
+    y0 = (r / (LIN_W / TILE_COLS)) * TILE_ROWS;
+  };
+  auto issue = [&](int s) {     // halo of step s = (layer s / T, tile s % T) into ring stage s & 1
+    const int l = s / T;
+    int n, y0, x0;
+    tile_coords(s - l * T, n, y0, x0);
+    const int in = p.plan[l][0];
+    const CUtensorMap* map = in == 0 ? &tmap0 : (in == 1 ? &tmap1 : &tmap2);
+    const uint32_t bar = smem_u32(&full[s & 1]);
+    mbar_expect_tx(bar, HALO_BYTES);
+    tma_load_4d(smem_u32(ring + (size_t)(s & 1) * HALO_STAGE), map, bar, 0, x0 - 1, y0 - 1, n);
+  };
+  auto issue_weights = [&](int l) {   // layer l into weight buffer l & 1
+    const uint32_t bar = smem_u32(&w_full[l & 1]);
+    mbar_expect_tx(bar, LAYER_W_BYTES);
+    for (int t = 0; t < 9; ++t)
+      bulk_load_1d(smem_u32(wbuf + (size_t)(l & 1) * LAYER_W_BYTES + t * 8192u), p.wpk + (size_t)l * LAYER_W_BYTES + t * 8192u,
+                   8192u, bar);
+  };
+  if (tid == 0) {
+    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap0) : "memory");
+    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap1) : "memory");
+    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap2) : "memory");
+    issue_weights(0);
+    if (p.L > 1) issue_weights(1);
+    issue(0);
   }
 
-  if (threadIdx.x == 64) STAMP(7);
-  tcgen05_fence_before();
-  __syncthreads();
-  if (threadIdx.x == 0) STAMP(8);
-  if (warp == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(p.tmem_cols) : "memory");
+  TcParams q = {};
+  q.H = p.H; q.W = LIN_W; q.Cout = 64;
+  float acc[1][32];
+  for (int s = 0; s < nsteps; ++s) {
+    const int l = s / T, it = s - l * T;
+    // the next tile of the same layer: its input does not change during this layer, its stage was released at the end of
+    // step s - 1.  The first tile of the next layer waits for this layer's last outputs (below).
+    if (tid == 0 && it + 1 < T) issue(s + 1);
+    if (it == 0) mbar_wait(smem_u32(&w_full[l & 1]), (uint32_t)((l >> 1) & 1));
+#pragma unroll
+    for (int r = 0; r < 32; ++r) acc[0][r] = 0.f;
+    mbar_wait(smem_u32(&full[s & 1]), (uint32_t)((s >> 1) & 1));
+    mma_block<0, 64, 1>(acc, smem_u32(ring + (size_t)(s & 1) * HALO_STAGE), smem_u32(wbuf + (size_t)(l & 1) * LAYER_W_BYTES), wg);
+    q.act = p.plan[l][3];
+    q.y = p.bufs[p.plan[l][1]];
+    q.res = p.plan[l][2] >= 0 ? p.bufs[p.plan[l][2]] : nullptr;
+    int n, y0, x0;
+    tile_coords(it, n, y0, x0);
+    epilogue<0, 64, 1>(acc, q, p.bias + 64 * l, 0, n, y0, x0);
+    if (it == T - 1) fence_proxy_async_global();   // this layer's stores -> visible to the next layer's TMA loads
+    __syncthreads();
+    if (tid == 0 && it == T - 1) {
+      if (l + 2 < p.L) issue_weights(l + 2);         // buffer l & 1 is free: every MMA of layer l has completed
+      if (s + 1 < nsteps) issue(s + 1);
+    }
   }
 }
 
@@ -753,16 +361,95 @@ PFN_encodeTiled get_encode() {
   return fn;
 }
 
-}  // namespace
-
-long long* teco_g_dbg_timing = nullptr;   // shared with conv_tc_sw.cu
-int teco_conv3x3_tc_one_tile(const teco_tc_desc* d, const void* x, const void* wpk, const float* bias, const void* res,
-                             void* y, const float* res_f32, float* out_f32, void* stream);   // conv_tc_sw.cu
-
-extern "C" int teco_debug_timing(void* buf) {
-  teco_g_dbg_timing = (long long*)buf;
+// NHWC bf16 activations [N,H,W,C] as a 4-D map whose box is one tile's halo of 64 channels (SWIZZLE_128B, zero fill)
+int encode_halo_map(CUtensorMap* map, const void* x, int N, int H, int W, int C, const char* who) {
+  PFN_encodeTiled enc = get_encode();
+  if (!enc) {
+    teco_set_error("%s: cuTensorMapEncodeTiled is unavailable (no CUDA driver?)", who);
+    return TECO_E_CUDA;
+  }
+  const cuuint64_t gdim[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)N};
+  const cuuint64_t gstr[3] = {(cuuint64_t)C * 2, (cuuint64_t)W * C * 2, (cuuint64_t)H * W * C * 2};
+  const cuuint32_t box[4] = {(cuuint32_t)CB, (cuuint32_t)HALO_COLS, (cuuint32_t)HALO_ROWS, 1};
+  const cuuint32_t estr[4] = {1, 1, 1, 1};
+  const CUresult cr = enc(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(x), gdim, gstr, box, estr,
+                          CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (cr != CUDA_SUCCESS) {
+    teco_set_error("%s: cuTensorMapEncodeTiled failed with CUresult %d (N=%d H=%d W=%d C=%d)", who, (int)cr, N, H, W, C);
+    return TECO_E_CUDA;
+  }
   return TECO_OK;
 }
+
+using KernelT = void (*)(const CUtensorMap, const TcParams);
+
+KernelT pick_kernel(int mode, int nt) {
+  if (mode == 1) return nt == 32 ? conv3x3_wgmma_kernel<1, 32> : conv3x3_wgmma_kernel<1, 16>;
+  if (nt == 64) return conv3x3_wgmma_kernel<0, 64>;
+  if (nt == 32) return conv3x3_wgmma_kernel<0, 32>;
+  return conv3x3_wgmma_kernel<0, 16>;
+}
+
+// CTAs of `kern` resident per SM at `smem` bytes of dynamic shared memory; the opt-in shared-memory attribute is set on
+// first use and the answer cached per (kernel, size), so a launch costs no extra driver calls.
+int resident_ctas(const void* kern, size_t smem, int* per_sm) {
+  struct Entry { const void* kern; size_t smem; int per_sm; };
+  static Entry cache[32];
+  static int used = 0;
+  for (int i = 0; i < used; ++i)
+    if (cache[i].kern == kern && cache[i].smem == smem) { *per_sm = cache[i].per_sm; return TECO_OK; }
+  bool attr_set = false;
+  for (int i = 0; i < used; ++i) attr_set |= cache[i].kern == kern;
+  if (!attr_set) TECO_CUDA_CALL(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_MAX));
+  int n = 0;
+  TECO_CUDA_CALL(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, kern, NUM_THREADS, smem));
+  if (n < 1) n = 1;
+  if (used < 32) cache[used++] = {kern, smem, n};
+  *per_sm = n;
+  return TECO_OK;
+}
+
+int launch_conv3x3(const teco_tc_desc* d, const void* x, const void* wpk, const float* bias, const void* res, void* y,
+                   const float* res_f32, float* out_f32, cudaStream_t stream) {
+  TcParams p;
+  p.N = d->N; p.H = d->H; p.W = d->W; p.Cout = d->Cout;
+  p.act = d->act; p.out_f32_c = d->out_f32_c;
+  p.post_scale = d->post_scale; p.post_shift = d->post_shift;
+  p.wpk = (const uint8_t*)wpk; p.bias = bias; p.res = (const __nv_bfloat16*)res; p.y = (__nv_bfloat16*)y;
+  p.res_f32 = res_f32; p.out_f32 = out_f32;
+  p.nblk = d->Cin / CB;
+  // output channels per CTA: 64, or 32 for the transposed conv, whose four phase accumulators must stay in registers
+  const int nt = (d->Cout % 64 == 0 && d->mode == 0) ? 64 : (d->Cout % 32 == 0 ? 32 : 16);
+  const int nsplit = d->Cout / nt;
+  p.w_blk_bytes = 9u * (uint32_t)nt * 128u;
+  p.tiles_x = teco_ceil_div(d->W, TILE_COLS);
+  p.tiles_y = teco_ceil_div(d->H, TILE_ROWS);
+  const long long tiles = (long long)d->N * p.tiles_x * p.tiles_y;
+  TECO_CHECK_ARG(tiles < (1LL << 31), "teco_conv3x3_tc: too many tiles");
+  p.num_tiles = (int)tiles;
+  const size_t fixed = 1024 + 64 + (size_t)nt * sizeof(float);
+  p.resident = fixed + 2 * (size_t)HALO_STAGE + (size_t)p.nblk * p.w_blk_bytes <= SMEM_MAX ? 1 : 0;
+  p.stage_bytes = HALO_STAGE + (p.resident ? 0u : p.w_blk_bytes);
+  const size_t smem = fixed + 2 * (size_t)p.stage_bytes + (p.resident ? (size_t)p.nblk * p.w_blk_bytes : 0);
+  TECO_CHECK_ARG(smem <= SMEM_MAX, "teco_conv3x3_tc: shared memory budget exceeded (Cin=%d Cout=%d)", d->Cin, d->Cout);
+
+  CUtensorMap tmap;
+  const int rc = encode_halo_map(&tmap, x, d->N, d->H, d->W, d->Cin, "teco_conv3x3_tc");
+  if (rc != TECO_OK) return rc;
+  const KernelT kern = pick_kernel(d->mode, nt);
+  int per_sm = 0;
+  const int rc_occ = resident_ctas((const void*)kern, smem, &per_sm);
+  if (rc_occ != TECO_OK) return rc_occ;
+  // persistent: as many CTAs as are resident at once, spread over the Cout splits
+  const long long slots = ((long long)per_sm * teco_sm_count() + nsplit - 1) / nsplit;
+  const unsigned gx = (unsigned)(tiles < slots ? tiles : slots);
+  kern<<<dim3(gx, (unsigned)nsplit), NUM_THREADS, smem, stream>>>(tmap, p);
+  TECO_CUDA_LAUNCH_CHECK("teco_conv3x3_tc");
+  return TECO_OK;
+}
+
+}  // namespace
 
 extern "C" int64_t teco_packed_weight_bytes(int32_t cin_pad, int32_t cout_pad) {
   return 9LL * cin_pad * cout_pad * 2;
@@ -795,225 +482,44 @@ extern "C" int teco_conv3x3_tc(const teco_tc_desc* d, const void* x, const void*
   TECO_CHECK_ARG((((uintptr_t)x) & 15) == 0 && (((uintptr_t)wpk) & 15) == 0 && (((uintptr_t)y) & 15) == 0 &&
                      (((uintptr_t)res) & 15) == 0,
                  "teco_conv3x3_tc: tensors must be 16-byte aligned");
+  return launch_conv3x3(d, x, wpk, bias, res, y, res_f32, out_f32, (cudaStream_t)stream);
+}
 
-  TcParams p;
-  p.N = d->N; p.H = d->H; p.W = d->W; p.Cin = d->Cin; p.Cout = d->Cout;
-  p.mode = d->mode; p.act = d->act; p.out_f32_c = d->out_f32_c;
-  p.post_scale = d->post_scale; p.post_shift = d->post_shift;
-  p.wpk = (const uint8_t*)wpk; p.bias = bias; p.res = (const __nv_bfloat16*)res; p.y = (__nv_bfloat16*)y;
-  p.res_f32 = res_f32; p.out_f32 = out_f32; p.dbg = teco_g_dbg_timing;
-  p.nblk = d->Cin / CB;
-  const int sms = teco_sm_count();
-  const int nacc = d->mode == 1 ? 4 : 1;
-  const size_t budget = 208 * 1024;
-  // few spatial tiles but many output channels (FNet's 16x16 / 32x32 layers): split Cout over CTAs, 64 channels each
-  const long long tiles1 = (long long)d->N * teco_ceil_div(d->H, TILE_ROWS) * teco_ceil_div(d->W, 8);
-  p.nsplit = (d->Cout >= 128 && d->Cout % 64 == 0 && tiles1 * (d->Cout / 64) <= 2LL * sms) ? d->Cout / 64 : 1;
-  if (d->Cout / p.nsplit > 256) p.nsplit = d->Cout / 256;   // VGG's 512-channel layers: N <= 256 per UMMA / TMEM stage
-  p.Ncta = d->Cout / p.nsplit;
-  TECO_CHECK_ARG(nacc * p.Ncta <= 512, "teco_conv3x3_tc: Cout=%d too large for mode %d (TMEM has 512 columns)", d->Cout, d->mode);
-  const size_t tap_bytes = (size_t)p.Ncta * 128;
-  constexpr int H1 = 1;   // single halo box per block, horizontal taps as 128-byte descriptor offsets (the three-box variant lost the A/B and is gone)
-  // bytes of one J = 1 halo stage: one 10-pixel-wide box (23 KB, padded to the swizzle atom) or three 8-pixel boxes
-  const size_t stage1 = H1 ? (((size_t)HALO_ROWS * 10 * 128 + 1023) & ~(size_t)1023) : 3 * (size_t)HALO_ROWS * 8 * 128;
-  const bool single_wave = tiles1 * p.nsplit <= (long long)sms;
-  // Dispatch (same-box A/B, profiles/conv_tc_r01_notes.md): the one-tile-per-CTA kernel is faster for single-wave
-  // launches and for the epilogue-heavy transposed conv (two CTAs per SM); this persistent kernel wins multi-wave convs.
-  // ... except large transposed convs (many waves): persistent CTAs with one staging tile per output phase
-  constexpr int env_tma = 1;   // staged (TMA-store) epilogue wherever the layer qualifies
-  static const int env_tp = [] { const char* e = getenv("TECO_TC_TCONV_PERSIST"); return e ? atoi(e) : 1; }();
-  const bool tconv_persist = env_tp && env_tma && d->mode == 1 && tiles1 >= 4LL * sms && p.nsplit == 1 && p.Ncta == 64 && y && !out_f32 &&
-                             !res && d->H % TILE_ROWS == 0 && d->W % 8 == 0 && d->act < TECO_ACT_TANH24 && p.nblk == 1;
-  if (single_wave || (d->mode == 1 && !tconv_persist))
-    return teco_conv3x3_tc_one_tile(d, x, wpk, bias, res, y, res_f32, out_f32, stream);
+extern "C" int teco_conv3x3_lin_supported(int32_t N, int32_t H, int32_t W, int32_t num_layers) {
+  return (N > 0 && W == LIN_W && H >= LIN_ROWS && H % LIN_ROWS == 0 && H <= 4096 && num_layers >= 1 && num_layers <= LIN_MAX_LAYERS) ? 1 : 0;
+}
 
-  // ---- configuration: (J, HST, weight staging, K-split, accumulator stages, grid)
-  int J = 1;
-  p.mcast = 0; p.CS = 1; p.AS = 1;
-  if (single_wave) {
-    // One tile per CTA, one CTA per SM (e.g. the 128x128 trunk: 128 tiles).  Whole layer resident when it fits: fetched
-    // before the dependency wait and multicast over a 4-CTA cluster (measured 6.2 us vs 6.9 us for a ring, 64->64).
-    p.HST = p.nblk > 1 ? 2 : 1;
-    const size_t a_total1 = (size_t)p.HST * stage1;
-    if (p.nsplit == 1 && a_total1 + 9 * tap_bytes * p.nblk <= budget && 3 * p.nblk <= MAX_WST) {
-      p.mcast = 1; p.TPS = 3; p.WST = 3 * p.nblk;
-      p.CS = tiles1 >= 8 ? 4 : 1;
-    } else if (p.nsplit == 1 && a_total1 + 2 * 3 * tap_bytes <= budget) {
-      p.TPS = 3; p.WST = (int)((budget - a_total1) / (3 * tap_bytes));
-      if (p.WST > 3 * p.nblk) p.WST = 3 * p.nblk;
-      if (p.WST > MAX_WST) p.WST = MAX_WST;
-    } else {
-      p.TPS = 1;
-      int wst = (int)((budget - a_total1) / tap_bytes);
-      if (wst > 9 * p.nblk) wst = 9 * p.nblk;
-      if (wst > MAX_WST) wst = MAX_WST;
-      TECO_CHECK_ARG(wst >= 2, "teco_conv3x3_tc: shared memory budget too small (Cin=%d Cout=%d)", d->Cin, d->Cout);
-      p.WST = wst;
-    }
-  } else {
-    // Multi-wave problems: persistent CTAs (one per SM) walking tiles, double-buffered halo stages and -- when TMEM
-    // allows -- two accumulator stages, so TMA, MMA and epilogue overlap across tiles; the layer's weights stay resident
-    // in shared memory for the whole launch when they fit next to two halo stages.
-    p.HST = 2;
-    const size_t a_total1 = 2 * stage1;
-    if (a_total1 + 9 * tap_bytes * p.nblk <= budget && 3 * p.nblk <= MAX_WST) {
-      p.mcast = 1; p.TPS = 3; p.WST = 3 * p.nblk;             // resident, loaded once per CTA (no cluster: CS = 1)
-    } else if (a_total1 + 2 * 3 * tap_bytes <= budget) {
-      p.TPS = 3; p.WST = (int)((budget - a_total1) / (3 * tap_bytes));
-      if (p.WST > MAX_WST) p.WST = MAX_WST;
-    } else {
-      p.TPS = 1;
-      int wst = (int)((budget - a_total1) / tap_bytes);
-      if (wst > MAX_WST) wst = MAX_WST;
-      TECO_CHECK_ARG(wst >= 2, "teco_conv3x3_tc: shared memory budget too small (Cin=%d Cout=%d)", d->Cin, d->Cout);
-      p.WST = wst;
-    }
+extern "C" int teco_conv3x3_lin_tc(int32_t N, int32_t H, int32_t W, int32_t num_layers, const void* x_in, void* buf_a, void* buf_b,
+                                   const void* wpk_all, const float* bias_all, const int32_t* plan_host, void* stream) {
+  TECO_CHECK_ARG(teco_conv3x3_lin_supported(N, H, W, num_layers),
+                 "teco_conv3x3_lin_tc: needs W == 32, H a multiple of 4, 1..%d layers (got N=%d H=%d W=%d L=%d)", LIN_MAX_LAYERS, N, H, W, num_layers);
+  TECO_CHECK_ARG(x_in && buf_a && buf_b && wpk_all && bias_all && plan_host, "teco_conv3x3_lin_tc: NULL argument");
+  TECO_CHECK_ARG((((uintptr_t)x_in) & 15) == 0 && (((uintptr_t)buf_a) & 15) == 0 && (((uintptr_t)buf_b) & 15) == 0 &&
+                     (((uintptr_t)wpk_all) & 15) == 0,
+                 "teco_conv3x3_lin_tc: tensors must be 16-byte aligned");
+  ChainParams p = {};
+  p.N = N; p.H = H; p.L = num_layers; p.tiles_y = teco_ceil_div(H, TILE_ROWS);
+  for (int l = 0; l < num_layers; ++l) {
+    const int32_t* pl = plan_host + 4 * l;
+    TECO_CHECK_ARG(pl[0] >= 0 && pl[0] <= 2 && (pl[1] == 1 || pl[1] == 2) && pl[0] != pl[1] && pl[2] >= -1 && pl[2] <= 2 &&
+                       pl[3] >= 0 && pl[3] < TECO_ACT_TANH24,
+                   "teco_conv3x3_lin_tc: bad plan row %d {%d, %d, %d, %d}", l, pl[0], pl[1], pl[2], pl[3]);
+    for (int k = 0; k < 4; ++k) p.plan[l][k] = (int8_t)pl[k];
   }
-  // Multi-wave 3x3 convs with <= 64 output channels per CTA: two 16x8 sub-tiles per tile and two K-split chains each
-  // (4 independent accumulators) instead of one sub-tile with three -- a third less TMEM read traffic in the epilogue
-  // (the 64 B/clk tcgen05.ld path bounds it) and a 16+2 pixel wide halo row instead of two 8+2 ones.
-  static const int env_j2 = [] { const char* e = getenv("TECO_TC_J2"); return e ? atoi(e) : 1; }();
-  int ks_force = 0;
-  if (!single_wave && H1 && env_j2 && d->mode == 0 && p.TPS == 3 && p.mcast && p.Ncta <= 64 &&
-      tiles1 >= 4LL * sms) {
-    const size_t stage2 = ((size_t)HALO_ROWS * 18 * 128 + 1023) & ~(size_t)1023;
-    if (2 * stage2 + 9 * tap_bytes * p.nblk <= budget) { J = 2; ks_force = 2; }
+  p.bufs[0] = (__nv_bfloat16*)const_cast<void*>(x_in); p.bufs[1] = (__nv_bfloat16*)buf_a; p.bufs[2] = (__nv_bfloat16*)buf_b;
+  p.wpk = (const uint8_t*)wpk_all; p.bias = bias_all;
+  CUtensorMap maps[3];
+  for (int i = 0; i < 3; ++i) {
+    const int rc = encode_halo_map(&maps[i], p.bufs[i], N, H, LIN_W, 64, "teco_conv3x3_lin_tc");
+    if (rc != TECO_OK) return rc;
   }
-  // Narrow fp32 output stage (generator 64->3, fnet 32->2) on many tiles: the kx-fused kernel (MODE 2 above)
-  static const int env_kx = [] { const char* e = getenv("TECO_TC_KX"); return e ? atoi(e) : 1; }();
-  const bool kx = env_kx && H1 && !single_wave && d->mode == 0 && out_f32 && !y && !res && d->Cout == 16 && p.nsplit == 1 && p.nblk == 1 &&
-                  d->out_f32_c <= 4 && p.mcast && p.TPS == 3;
-  if (kx) {
-    double best = 0.0;
-    for (int jj = 2; jj <= 4; ++jj) {   // widest use of the 8*jj halo columns: W / (tiles * 8 jj)
-      const double eff = (double)d->W / ((double)teco_ceil_div(d->W, 8 * jj - 2) * 8 * jj);
-      if (eff > best + 1e-9) { best = eff; J = jj; }
-    }
-    ks_force = 1;
-  }
-  const int box_w = (H1 && !kx) ? 8 * J + 2 : 8 * J;
-  p.J = J;
-  p.tiles_x = kx ? teco_ceil_div(d->W, 8 * J - 2) : teco_ceil_div(d->W, 8 * J);
-  p.tiles_y = teco_ceil_div(d->H, TILE_ROWS);
-  p.num_tiles = (int)((long long)d->N * p.tiles_x * p.tiles_y);
-  p.copy_bytes = (uint32_t)(HALO_ROWS * box_w * 128);
-  p.halo_stage_bytes = H1 ? ((p.copy_bytes + 1023u) & ~1023u) : 3 * p.copy_bytes;
-  // Input larger than ~half of L2 streams from HBM: one tile of look-ahead (HST = 2) leaves the CTA waiting on DRAM
-  // latency (the 64->16 output stage at 296 x 128x128 ran 6300 clk per tile against ~2900 of work); use the shared memory
-  // the configuration leaves free for a deeper ring.
-  const bool tma_possible = tconv_persist || (env_tma && d->mode == 0 && y && !out_f32 && p.Ncta == 64 && d->act < TECO_ACT_TANH24);
-  const size_t staging_bytes = tconv_persist ? 1024 + (size_t)4 * 16384 : 1024 + (size_t)2 * J * 16384;
-  const double in_bytes = (double)d->N * d->H * d->W * d->Cin * 2.0;
-  if (!single_wave && p.nblk == 1 && in_bytes > 48e6) {
-    const size_t fixed = (size_t)p.WST * p.TPS * tap_bytes + (tma_possible ? staging_bytes : 0) + 8192;
-    while (p.HST < MAX_HST && fixed + (size_t)(p.HST + 1) * p.halo_stage_bytes <= 232448 - 2048) ++p.HST;
-  }
-  const size_t a_total = (size_t)p.HST * p.halo_stage_bytes;
-  p.w_slab_bytes = (uint32_t)(p.TPS * tap_bytes);
-  p.KS = ks_force ? ks_force : ((p.TPS == 3 && d->mode == 0 && J * 3 * p.Ncta <= 512) ? 3 : 1);
-  const uint32_t stage_cols = (uint32_t)(J * (kx ? 3 : nacc) * p.KS * p.Ncta);
-  if (!single_wave && 2 * stage_cols <= 512) p.AS = 2;
-  uint32_t cols = stage_cols * (uint32_t)p.AS, tc = 32;
-  while (tc < cols) tc <<= 1;
-  p.tmem_cols = tc;
-  if (single_wave) p.G = (p.num_tiles + p.CS - 1) / p.CS * p.CS;   // padded to the cluster size
-  else p.G = p.num_tiles < sms ? p.num_tiles : sms;
-  p.tma_out = tma_possible ? 1 : 0;
-  p.tma_res = (p.tma_out && res) ? 1 : 0;
-  size_t smem_bytes = 1024 + a_total + (size_t)p.WST * p.w_slab_bytes + (2 * MAX_HST + 2 * MAX_WST + 4 + 1) * 8 + 256 * sizeof(float) + 128 +
-                      (p.tma_out ? staging_bytes : 0);
-  if (smem_bytes > 232448 && p.tma_out) {       // 227 KB: the opt-in maximum of dynamic shared memory per block on sm_100
-    TECO_CHECK_ARG(!tconv_persist, "teco_conv3x3_tc: persistent transposed conv does not fit in shared memory");
-    smem_bytes -= staging_bytes;
-    p.tma_out = p.tma_res = 0;
-  }
-
-  PFN_encodeTiled enc = get_encode();
-  if (!enc) {
-    teco_set_error("teco_conv3x3_tc: cuTensorMapEncodeTiled is unavailable (no CUDA driver?)");
-    return TECO_E_CUDA;
-  }
-  CUtensorMap tmap;
-  const cuuint64_t gdim[4] = {(cuuint64_t)d->Cin, (cuuint64_t)d->W, (cuuint64_t)d->H, (cuuint64_t)d->N};
-  const cuuint64_t gstr[3] = {(cuuint64_t)d->Cin * 2, (cuuint64_t)d->W * d->Cin * 2, (cuuint64_t)d->H * d->W * d->Cin * 2};
-  const cuuint32_t box[4] = {(cuuint32_t)CB, (cuuint32_t)box_w, (cuuint32_t)HALO_ROWS, 1};
-  const cuuint32_t estr[4] = {1, 1, 1, 1};
-  CUresult cr = enc(&tmap, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(x), gdim, gstr, box, estr,
-                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (cr != CUDA_SUCCESS) {
-    teco_set_error("teco_conv3x3_tc: cuTensorMapEncodeTiled failed with CUresult %d (N=%d H=%d W=%d Cin=%d)", (int)cr, d->N,
-                   d->H, d->W, d->Cin);
-    return TECO_E_CUDA;
-  }
-  CUtensorMap tmap_y = tmap, tmap_r = tmap;   // placeholders when the staged epilogue is off
-  if (p.tma_out && d->mode == 1) {
-    // output [N, 2H, 2W, C] as {C, px, x, py, n*H + y}: one box = the 16x8 pixels of one sub-pixel phase (H % 16 == 0, so a
-    // box never runs from one image into the next)
-    const cuuint64_t odim[5] = {(cuuint64_t)d->Cout, 2, (cuuint64_t)d->W, 2, (cuuint64_t)d->N * d->H};
-    const cuuint64_t ostr[4] = {(cuuint64_t)d->Cout * 2, (cuuint64_t)d->Cout * 4, (cuuint64_t)d->W * d->Cout * 4,
-                                (cuuint64_t)d->W * d->Cout * 8};
-    const cuuint32_t obox[5] = {64, 1, 8, 1, (cuuint32_t)TILE_ROWS};
-    const cuuint32_t estr5[5] = {1, 1, 1, 1, 1};
-    cr = enc(&tmap_y, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, y, odim, ostr, obox, estr5, CU_TENSOR_MAP_INTERLEAVE_NONE,
-             CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (cr != CUDA_SUCCESS) {
-      teco_set_error("teco_conv3x3_tc: cuTensorMapEncodeTiled (transposed-conv output) failed with CUresult %d", (int)cr);
-      return TECO_E_CUDA;
-    }
-  } else if (p.tma_out) {
-    const cuuint64_t odim[4] = {(cuuint64_t)d->Cout, (cuuint64_t)d->W, (cuuint64_t)d->H, (cuuint64_t)d->N};
-    const cuuint64_t ostr[3] = {(cuuint64_t)d->Cout * 2, (cuuint64_t)d->W * d->Cout * 2, (cuuint64_t)d->H * d->W * d->Cout * 2};
-    const cuuint32_t obox[4] = {64, 8, (cuuint32_t)TILE_ROWS, 1};
-    cr = enc(&tmap_y, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, y, odim, ostr, obox, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-             CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (cr == CUDA_SUCCESS && p.tma_res)
-      cr = enc(&tmap_r, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(res), odim, ostr, obox, estr,
-               CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-               CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (cr != CUDA_SUCCESS) {
-      teco_set_error("teco_conv3x3_tc: cuTensorMapEncodeTiled (output tile) failed with CUresult %d", (int)cr);
-      return TECO_E_CUDA;
-    }
-  }
-  using KernelT = void (*)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const TcParams);
-  KernelT kern = nullptr;
-#define TECO_PICK(M, T, JJ, K)                                              \
-  if ((kx ? 2 : d->mode) == M && p.TPS == T && J == JJ && p.KS == K)        \
-    kern = conv3x3_tc_kernel<M, T, JJ, K, 1>;
-  TECO_PICK(0, 3, 2, 2) TECO_PICK(0, 3, 1, 3) TECO_PICK(0, 3, 2, 3) TECO_PICK(0, 3, 1, 1) TECO_PICK(0, 3, 2, 1) TECO_PICK(0, 1, 1, 1) TECO_PICK(0, 1, 2, 1)
-  TECO_PICK(1, 3, 1, 1) TECO_PICK(1, 3, 2, 1) TECO_PICK(1, 1, 1, 1) TECO_PICK(1, 1, 2, 1)
-  TECO_PICK(2, 3, 2, 1) TECO_PICK(2, 3, 3, 1) TECO_PICK(2, 3, 4, 1)
-#undef TECO_PICK
-  if (!kern) {
-    teco_set_error("teco_conv3x3_tc: no kernel instantiation for mode=%d TPS=%d J=%d KS=%d", d->mode, p.TPS, J, p.KS);
-    return TECO_E_UNSUPPORTED;
-  }
-  TECO_CUDA_CALL(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 232448));
-  const unsigned ctas = (unsigned)(p.G * p.nsplit);
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(ctas);
-  cfg.blockDim = dim3(NUM_THREADS);
-  cfg.dynamicSmemBytes = smem_bytes;
-  cfg.stream = (cudaStream_t)stream;
-  cudaLaunchAttribute attrs[2];
-  int na = 0;
-  attrs[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;   // PDL: prologue overlaps the previous kernel's tail
-  attrs[na].val.programmaticStreamSerializationAllowed = 1;
-  ++na;
-  if (p.CS > 1) {
-    attrs[na].id = cudaLaunchAttributeClusterDimension;
-    attrs[na].val.clusterDim.x = (unsigned)p.CS;
-    attrs[na].val.clusterDim.y = 1;
-    attrs[na].val.clusterDim.z = 1;
-    ++na;
-  }
-  cfg.attrs = attrs;
-  cfg.numAttrs = na;
-  cudaError_t le = cudaLaunchKernelEx(&cfg, kern, tmap, tmap_y, tmap_r, p);
-  if (le != cudaSuccess) {
-    teco_set_error("teco_conv3x3_tc: launch failed: %s (grid %u, cluster %d, smem %zu)", cudaGetErrorString(le), ctas, p.CS, smem_bytes);
-    return TECO_E_CUDA;
-  }
+  const size_t smem = 1024 + 2 * (size_t)HALO_STAGE + 2 * (size_t)LAYER_W_BYTES + 64;
+  int per_sm = 0;
+  const int rc = resident_ctas((const void*)conv3x3_chain_kernel, smem, &per_sm);
+  if (rc != TECO_OK) return rc;
+  const long long slots = (long long)per_sm * teco_sm_count();
+  const unsigned grid = (unsigned)(N < slots ? N : slots);
+  conv3x3_chain_kernel<<<grid, NUM_THREADS, smem, (cudaStream_t)stream>>>(maps[0], maps[1], maps[2], p);
+  TECO_CUDA_LAUNCH_CHECK("teco_conv3x3_lin_tc");
   return TECO_OK;
 }

@@ -1,4 +1,5 @@
-// PTX wrappers shared by the tcgen05 kernels (mbarrier, TMA, bulk copies, tcgen05.mma/ld/commit, UMMA descriptors).
+// PTX wrappers shared by the Hopper tensor-core kernels (mbarrier, TMA, bulk copies, wgmma and its shared-memory
+// descriptors).
 #pragma once
 #include <cuda.h>
 #include <stdint.h>
@@ -25,12 +26,15 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
         : "memory");
   } while (!done);
 }
-// Warp-collective wait: one lane polls the mbarrier, the rest park on the warp barrier (keeps 31 lanes per warp
-// from hammering the shared-memory pipe that the TMA engine is writing through).
+// Warp-collective wait: one lane polls the mbarrier, the rest park on the warp barrier.
 __device__ __forceinline__ void mbar_wait_warp(uint32_t bar, uint32_t parity) {
   if ((threadIdx.x & 31) == 0) mbar_wait(bar, parity);
   __syncwarp();
 }
+__device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+// generic-proxy global writes of this thread -> ordered before later async-proxy (TMA) reads
+__device__ __forceinline__ void fence_proxy_async_global() { asm volatile("fence.proxy.async.global;" ::: "memory"); }
+__device__ __forceinline__ void fence_mbar_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 __device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, int c2,
                                             int c3) {
   asm volatile(
@@ -43,142 +47,67 @@ __device__ __forceinline__ void bulk_load_1d(uint32_t dst, const void* src, uint
                "l"(src), "r"(bytes), "r"(bar)
                : "memory");
 }
-__device__ __forceinline__ void bulk_load_1d_mcast(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar, uint16_t mask) {
-  asm volatile(
-      "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1], %2, [%3], %4;" ::"r"(dst),
-      "l"(src), "r"(bytes), "r"(bar), "h"(mask)
-      : "memory");
-}
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// Programmatic dependent launch: let the next kernel in the stream start its prologue now; wait for the
-// previous kernel's results only where they are first needed.
-__device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
-__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-__device__ __forceinline__ void tcgen05_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tcgen05_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tcgen05_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void umma_bf16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accum) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accum)
-      : "memory");
-}
-// One elected lane of a fully converged warp (elect.sync): keeps the surrounding address arithmetic warp-uniform so
-// ptxas holds the UMMA descriptors in uniform registers instead of a per-MMA R2UR waterfall loop.
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile("{\n\t.reg .pred P;\n\telect.sync _|P, 0xffffffff;\n\tselp.u32 %0, 1, 0, P;\n\t}" : "=r"(pred));
-  return pred != 0;
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
-// UMMA shared-memory descriptor, K-major SWIZZLE_128B (cute::UMMA::SmemDescriptor bit layout):
-// [0,14) start>>4, [16,30) LBO>>4 (=1, unused for swizzled K-major), [32,46) SBO>>4, [46,48) version=1,
-// [61,64) layout type = 2 (SWIZZLE_128B).  Canonical layout ((8,n),2):((8,SBO),1) in 16-byte units.
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t saddr, uint32_t sbo) {
-  return (uint64_t)((saddr & 0x3FFFFu) >> 4) | (1ull << 16) | ((uint64_t)((sbo >> 4) & 0x3FFFu) << 32) | (1ull << 46) |
-         (2ull << 61);
-}
-// Instruction descriptor (cute::UMMA::InstrDescriptor): c_format F32 (1) @4, a/b format BF16 (1) @7/@10,
-// a/b major K (0) @15/@16, N>>3 @17, M>>4 @24.
-__device__ __forceinline__ uint32_t umma_idesc(int n) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(n >> 3) << 17) | ((128u >> 4) << 24);
+// wgmma shared-memory matrix descriptor (sm_90): [0,14) start >> 4, [16,30) LBO >> 4, [32,46) SBO >> 4,
+// [62,64) layout type (1 = SWIZZLE_128B); the base-offset field [49,52) is left 0.  The convolution kernels start A operands
+// at 128-byte row offsets that are not on 1024-byte swizzle-atom boundaries (halo rows of 1280 / 2304 B plus one pixel per
+// horizontal tap).  That relies on the hardware applying the 128-byte XOR swizzle to the final shared-memory address, as
+// the TMA writes it, rather than relative to the start address: observed H100 behaviour, not a documented guarantee; the
+// per-kernel tests against the oracle (every tap, ragged shapes) pin it.
+//   K-major SW128: 8 rows x 128 B atoms, SBO = stride between 8-row groups, LBO unused.
+//   MN-major SW128: 64 contiguous MN elements per 128-byte row, LBO = next 64 MN elements, SBO = next 8 K rows.
+__device__ __forceinline__ uint64_t gmma_desc_sw128(uint32_t saddr, uint32_t lbo, uint32_t sbo) {
+  return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)((lbo >> 4) & 0x3FFFu) << 16) |
+         ((uint64_t)((sbo >> 4) & 0x3FFFu) << 32) | (1ull << 62);
 }
 
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
 
+// D[64 x N] (+)= A[64 x 16] * B[16 x N], bf16 operands from shared memory, fp32 accumulators in registers (N / 2 per
+// thread).  TA / TB = 1: the operand is MN-major in shared memory.
+template <int N, int TA, int TB>
+struct Wgmma;
 
-// ---- additions for the staged (TMA-store) epilogues and the multi-layer kernels
-__device__ __forceinline__ void tma_store_4d(const CUtensorMap* map, uint32_t src, int c0, int c1, int c2, int c3) {
-  asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];" ::"l"(map), "r"(src),
-               "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-               : "memory");
-}
-__device__ __forceinline__ void tma_store_5d(const CUtensorMap* map, uint32_t src, int c0, int c1, int c2, int c3, int c4) {
-  asm volatile("cp.async.bulk.tensor.5d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5, %6}], [%1];" ::"l"(map), "r"(src),
-               "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_ld4(uint32_t taddr, uint32_t* r) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x4.b32 {%0, %1, %2, %3}, [%4];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
-               : "r"(taddr));
-}
-__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
-__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory"); }
-__device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void fence_proxy_async_global() { asm volatile("fence.proxy.async.global;" ::: "memory"); }
-__device__ __forceinline__ uint32_t ld_acquire_cta_smem(uint32_t addr) {
-  uint32_t v;
-  asm volatile("ld.acquire.cta.shared::cta.u32 %0, [%1];" : "=r"(v) : "r"(addr) : "memory");
-  return v;
-}
-__device__ __forceinline__ void st_release_cta_smem(uint32_t addr, uint32_t v) {
-  asm volatile("st.release.cta.shared::cta.u32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
-}
-// Wait with a suspend-time hint: the thread sleeps in hardware until the phase completes (or the hint expires) instead of
-// re-polling shared memory -- waiting warps must not compete with the tensor core's operand reads for the shared-memory pipe.
-__device__ __forceinline__ void mbar_wait_sleepy(uint32_t bar, uint32_t parity) {
-  uint32_t done;
-  do {
+template <int TA, int TB>
+struct Wgmma<16, TA, TB> {
+  __device__ __forceinline__ static void run(float* d, uint64_t da, uint64_t db, uint32_t accum) {
     asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2, %3;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(done)
-        : "r"(bar), "r"(parity), "r"(1000000u)
-        : "memory");
-  } while (!done);
-}
-__device__ __forceinline__ void mbar_wait_warp_sleepy(uint32_t bar, uint32_t parity) {
-  if ((threadIdx.x & 31) == 0) mbar_wait_sleepy(bar, parity);
-  __syncwarp();
-}
-// non-blocking test of an mbarrier phase (mbarrier.test_wait never suspends the thread)
-__device__ __forceinline__ bool mbar_test(uint32_t bar, uint32_t parity) {
-  uint32_t done;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "mbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(done)
-      : "r"(bar), "r"(parity)
-      : "memory");
-  return done != 0;
-}
-// instruction descriptor with an explicit M (128 per CTA; 256 for cta_group::2)
-__device__ __forceinline__ uint32_t umma_idesc_mn(int m, int n) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(m >> 4) << 24);
-}
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, %11, %12;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "l"(da), "l"(db), "r"(accum), "n"(TA), "n"(TB));
+  }
+};
+template <int TA, int TB>
+struct Wgmma<32, TA, TB> {
+  __device__ __forceinline__ static void run(float* d, uint64_t da, uint64_t db, uint32_t accum) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, "
+        "%14, %15}, %16, %17, p, 1, 1, %19, %20;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+          "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(da), "l"(db), "r"(accum), "n"(TA), "n"(TB));
+  }
+};
+template <int TA, int TB>
+struct Wgmma<64, TA, TB> {
+  __device__ __forceinline__ static void run(float* d, uint64_t da, uint64_t db, uint32_t accum) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, "
+        "%14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, "
+        "%35, %36;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+          "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+          "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+          "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(da), "l"(db), "r"(accum), "n"(TA), "n"(TB));
+  }
+};
+// The accumulator fragment of m64nN: register 4*j + 2*i + c of thread t holds row 16*(t/32 % 4) + (t%32)/4 + 8*i and
+// column 8*j + 2*(t%4) + c.
 
 }  // namespace tcptx

@@ -1,4 +1,4 @@
-// Shared helpers for libteco.so (sm_100a only).
+// Shared helpers for libteco.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>

@@ -3,9 +3,8 @@
 //   flow_lr -> symmetric pad, x4, upscale_four -> dense_image_warp(previous HR output) -> space_to_depth
 // (reference main.py:201,212-215; lib/ops.py:126-163 upscale_four; tf.contrib.image.dense_image_warp).  Same arithmetic,
 // formula for formula, as warp_s2d_fused_kernel in resample.cu (which keeps every other layout: fp32 destinations,
-// warped_out, unaligned channel offsets); what changes is the instruction count per HR pixel.  ncu of the first version
-// (profiles/r02_warp_s2d_32x1024_summary.txt): 195 thread instructions per HR pixel, issue slots 76 % busy, DRAM at 37 % --
-// issue-bound, not memory-bound.  Here:
+// warped_out, unaligned channel offsets); what changes is the instruction count per HR pixel (the first version is
+// issue-bound, not memory-bound).  Here:
 //   * CTA tile 4 x 32 LR pixels (16 x 128 HR): the per-tile work (flow bound, window set-up, barriers) is paid once per 2048
 //     HR pixels instead of 1024, and the staged source window carries 2 halo rows per 16 instead of per 8;
 //   * the 5 x 33 flow samples of the tile are parked in shared memory once (no thread repeats the symmetric-pad index
@@ -18,8 +17,7 @@
 //   * results go through a bf16 staging tile in shared memory in destination order and leave as 16-byte stores, six per LR
 //     pixel (was: three shuffles, eight selects and an 8-byte store per HR pixel with a quarter of the lanes idle);
 //   * rough motion (window larger than the 40 KB stage): the tile in two halves with their own windows, then an L1 gather.
-// Measured (profiles/r02_warp_versions_ab.txt, r02_warp_s2d_v2_32x1024_summary.txt): 239 -> 160 us on 32 x 1024x1024 HR frames
-// (0.39 -> 0.59 of the measured copy bandwidth), bit-identical output; 113 M instead of 204 M warp instructions.
+// The output is bit-identical to the first version's.
 #include "teco_common.cuh"
 #include "tc_ptx.cuh"
 

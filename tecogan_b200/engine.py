@@ -6,7 +6,7 @@ Per frame i:   i > 0:  flow = fnet(pre_inputs ++ LR_i);  pre_warp = warp(pre_gen
 frame 0 uses pre_warp = 0.
 
 bf16 mode keeps everything in pre-allocated device buffers and replays ONE CUDA graph per frame
-(~57 tcgen05 launches + warp/s2d + resample kernels); fp32 mode runs the differentiable mirror under no_grad.
+(~57 wgmma launches + warp/s2d + resample kernels); fp32 mode runs the differentiable mirror under no_grad.
 
 Look-ahead (bf16 mode, step(lr, next_lr=...) / run_sequence): the flow of frame i+1 depends only on LR_i and LR_{i+1}
 (main.py:211), not on any HR output, so fnet(LR_i ++ LR_{i+1}) is captured on a second stream of the frame graph and
@@ -66,7 +66,7 @@ class InferenceEngine:
             self.pre_gen = torch.zeros((batch, 4 * h, 4 * w, 3), device=self.device, dtype=f32)
             self.pre_warp = torch.zeros_like(self.pre_gen)
 
-    # ------------------------------------------------------------------ bf16 / tcgen05 path
+    # ------------------------------------------------------------------ bf16 / wgmma path
     def _frame_first(self):
         self.gen.x_in[..., S2D_OFF:S2D_OFF + 48].zero_()
         _f32_slice_to_bf16(self.lr_in, 0, 3, self.gen.x_in, LR_OFF)
@@ -277,7 +277,7 @@ class ClipEngine:
         if T < 1:
             raise ValueError("ClipEngine: a clip has at least one frame")
         if config.precision() != "bf16":
-            raise ValueError("ClipEngine runs the tcgen05 path; use InferenceEngine for the fp32 exact-parity mode")
+            raise ValueError("ClipEngine runs the wgmma path; use InferenceEngine for the fp32 exact-parity mode")
         self.h, self.w, self.T, self.B, self.nrb = h, w, T, batch, num_resblock
         self.device = torch.device(device)
         self.use_graph = use_graph

@@ -475,7 +475,7 @@ def adam_step(p, m, v, g, lr_t, b1, b2, eps, gscale=1.0):
 
 # ------------------------------------------------------------------------------------------ bf16 tensor-core path
 def packed_weight(w, cin_pad, cout_pad, transpose_layout=False, cin_perm=None):
-    """fp32 TF-layout weights -> UMMA-canonical bf16 slab [9][cin_pad/8][cout_pad][8] (device side)."""
+    """fp32 TF-layout weights -> K-major SWIZZLE_128B bf16 slab [cin_pad/64][9][cout_pad][64] (device side)."""
     w = _cc(w)
     if int(transpose_layout) & 1:
         cout, cin = w.shape[2], w.shape[3]
@@ -498,7 +498,7 @@ def pad_bias(b, cout_pad):
 
 
 def conv3x3_tc(x, wpk, bias, y=None, *, cout, act=ACT_NONE, res=None, mode=0, out_f32=None, res_f32=None, post=(1.0, 0.0)):
-    """One launch of the tcgen05 kernel.  x [N,H,W,Cin] bf16; y [N,H(,x2),W(,x2),cout] bf16 (allocated if None and
+    """One launch of the wgmma kernel.  x [N,H,W,Cin] bf16; y [N,H(,x2),W(,x2),cout] bf16 (allocated if None and
     out_f32 is None)."""
     N, H, W, Cin = x.shape
     s = 2 if mode == 1 else 1
@@ -569,7 +569,7 @@ def warp_s2d_fused(pre_gen, flow_lr, dst, ch_off, in_scale=1.0, in_shift=0.0, wa
 
 # ------------------------------------------------------------------------------------------ bf16 tensor-core TRAINING convs
 # bf16 compute, fp32 master weights / activations at the autograd boundary (north_star: "bf16 training").  Forward and the
-# input gradient run on the tcgen05 kernel (the input gradient of a 3x3 stride-1 SAME conv is the same conv with the taps
+# input gradient run on the wgmma kernel (the input gradient of a 3x3 stride-1 SAME conv is the same conv with the taps
 # flipped and Cin/Cout swapped: teco_pack_conv3x3_bf16 flag 3); the weight gradient stays on the fp32 kernel.
 _tc_wcache = {}
 
@@ -611,7 +611,7 @@ def _from_bf16_rows(yb, C, add=None):
 
 
 def conv3x3_wgrad_tc(xb, dzb, dw, cin, cout, accumulate=False):
-    """dw[3,3,cin,cout] fp32 (+)= sum_p xb[p+tap][ci] dzb[p][co] on tcgen05 (teco_conv3x3_wgrad_tc); xb / dzb: NHWC bf16 with
+    """dw[3,3,cin,cout] fp32 (+)= sum_p xb[p+tap][ci] dzb[p][co] on wgmma (teco_conv3x3_wgrad_tc); xb / dzb: NHWC bf16 with
     channel counts padded to multiples of 64."""
     N, H, W, cp = xb.shape
     call("teco_conv3x3_wgrad_tc", N, H, W, cp, dzb.shape[-1], cin, cout, ptr(xb, bf16), ptr(dzb, bf16), ptr(dw, f32),
@@ -671,7 +671,7 @@ class _Conv3x3TC(torch.autograd.Function):
         if ctx.needs_input_grad[1]:
             if Cout % 4 == 0:
                 dw = torch.empty_like(w)
-                conv3x3_wgrad_tc(xb, dzb, dw, Cin, Cout)          # tcgen05, pixels as the contraction dimension
+                conv3x3_wgrad_tc(xb, dzb, dw, Cin, Cout)          # wgmma, pixels as the contraction dimension
             else:   # 16-byte atomics need Cout % 4 == 0 (generator 64->3, fnet 32->2): dW with Cout rounded up to 4 --
                 c4 = (Cout + 3) // 4 * 4                          # the extra columns see the zero pad channels of dzb
                 dw4 = torch.empty(w.shape[:3] + (c4,), device=w.device, dtype=f32)
@@ -715,7 +715,7 @@ def _tconv_index(device):
 
 
 class _ConvTranspose2xTC(torch.autograd.Function):
-    """conv2_tran() 64 -> 64 on tcgen05: forward = the 4-phase kernel of the inference path (teco_conv3x3_tc mode 1), input and
+    """conv2_tran() 64 -> 64 on wgmma: forward = the 4-phase kernel of the inference path (teco_conv3x3_tc mode 1), input and
     weight gradients through the space-to-depth identities above.  Reference lib/ops.py:35-44 and its TF autodiff."""
 
     @staticmethod

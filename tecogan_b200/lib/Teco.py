@@ -50,7 +50,7 @@ def _vgg_raw(input_pm1):
                         b = get_variable('biases', (cout,), init='zeros')
                     from .. import config
                     if config.train_precision() == "bf16":
-                        x = K.conv3x3_train_tc(x, w, b, ACT_RELU)     # frozen weights: forward (+ input gradient) on tcgen05
+                        x = K.conv3x3_train_tc(x, w, b, ACT_RELU)     # frozen weights: forward (+ input gradient) on wgmma
                     else:
                         x = K.conv2d(x, w, b, 1, ACT_RELU)      # slim.conv2d default activation relu, SAME (lib/Teco.py:12)
                     out['vgg_19/conv%d/%s' % (blk, name)] = x

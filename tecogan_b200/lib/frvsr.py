@@ -2,7 +2,7 @@
 
 Two execution modes, chosen by tecogan_b200.config:
   * "fp32": every layer through the fp32 CUDA-core kernels, differentiable (training, exact parity);
-  * "bf16": NHWC bf16 activations through the tcgen05 tensor-core kernel (inference hot path).
+  * "bf16": NHWC bf16 activations through the wgmma tensor-core kernel (inference hot path).
 """
 import torch
 

@@ -42,7 +42,7 @@ def conv2_tran(batch_input, kernel=3, output_channel=64, stride=1, use_bias=True
         b = get_variable('biases', (output_channel,), init='zeros') if use_bias else None
     if (torch.is_grad_enabled() and config.train_precision() == "bf16" and config.train_tc_all() and cin == 64 and output_channel == 64
             and act in (ACT_NONE, ACT_RELU, ACT_LRELU02)):
-        return K.conv_transpose2x_train_tc(batch_input, w, b, act)   # tcgen05 forward, input and weight gradients
+        return K.conv_transpose2x_train_tc(batch_input, w, b, act)   # wgmma forward, input and weight gradients
     return K.conv2d_transpose(batch_input, w, b, act)
 
 
@@ -58,7 +58,7 @@ def conv2(batch_input, kernel=3, output_channel=64, stride=1, use_bias=True, sco
     if (kernel == 3 and stride == 1 and torch.is_grad_enabled() and config.train_precision() == "bf16"
             and (output_channel >= 16 or config.train_tc_all())
             and (act in (ACT_NONE, ACT_RELU, ACT_LRELU02) or (act == ACT_TANH24 and output_channel < 16 and res is None))):
-        return K.conv3x3_train_tc(batch_input, w, b, act, res)      # tcgen05 forward, input and weight gradients
+        return K.conv3x3_train_tc(batch_input, w, b, act, res)      # wgmma forward, input and weight gradients
     return K.conv2d(batch_input, w, b, stride, act, res)
 
 

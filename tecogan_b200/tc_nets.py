@@ -1,7 +1,7 @@
-"""bf16 tensor-core execution of generator_F / fnet (reference lib/frvsr.py) on the tcgen05 kernel.
+"""bf16 tensor-core execution of generator_F / fnet (reference lib/frvsr.py) on the wgmma kernel.
 
 Activations are NHWC bf16 with channel counts padded to multiples of 64 (one 128-byte swizzled row); weights are re-packed once per
-VariableStore version into the UMMA canonical layout (teco_pack_conv3x3_bf16).  The generator input uses an
+VariableStore version into the K-major SWIZZLE_128B layout (teco_pack_conv3x3_bf16).  The generator input uses an
 internal channel order  [0,48) = space-to-depth of the warped previous HR frame, [48,51) = LR RGB, [51,64) = 0
 so the fused warp kernel can store 16-byte vectors; the first layer's weights are permuted accordingly.
 """
@@ -26,7 +26,7 @@ def pad16(c):
 
 
 def pad64(c):
-    """bf16 activation tensors carry multiples of 64 channels: 64 ch = one 128-byte swizzled UMMA/TMA row."""
+    """bf16 activation tensors carry multiples of 64 channels: 64 ch = one 128-byte swizzled wgmma/TMA row."""
     return (c + 63) // 64 * 64
 
 
@@ -105,7 +105,7 @@ def _ensure_vars_fnet():
 
 
 class GeneratorPlan:
-    """Pre-allocated buffers + packed layers for one (B,h,w) generator shape; `run` issues 2N+5 tcgen05 launches
+    """Pre-allocated buffers + packed layers for one (B,h,w) generator shape; `run` issues 2N+5 wgmma launches
     and one bicubic kernel, with no allocation -- safe to capture in a CUDA graph."""
 
     def __init__(self, scope, B, h, w, num_resblock, device):
@@ -126,14 +126,16 @@ class GeneratorPlan:
         self.bic = torch.zeros((B, 4 * h, 4 * w, 3), device=device, dtype=f32)
         self.out = torch.zeros((B, 4 * h, 4 * w, 3), device=device, dtype=f32)
         self.launches = 2 * num_resblock + 5 + 1
-        # 32-pixel-wide frames in a batch: the whole trunk as one launch of the row-linearised kx-fused kernel
+        # 32-pixel-wide frames in a batch: the whole trunk can run as one launch of the multi-layer chain kernel (opt-in,
+        # config.set_lin_trunk; bench.py times it against the per-layer launches)
         self.lin = config.lin_trunk() and B >= 8 and K.conv3x3_lin_supported(B, h, w, 2 * num_resblock + 1)
-        if self.lin:
+        if K.conv3x3_lin_supported(B, h, w, 2 * num_resblock + 1):
             layers = [self.l_in] + [l for pair in self.l_res for l in pair]
             self.trunk_w = torch.cat([l.wpk for l in layers]).contiguous()
             self.trunk_b = torch.cat([l.bias for l in layers]).contiguous()
             # buffer ids: 0 = x_in, 1 = a, 2 = b.  input conv x_in -> a (ReLU); block: a -> b (ReLU), b -> a (+ a)
             self.trunk_plan = [(0, 1, -1, ACT_RELU)] + [(1, 2, -1, ACT_RELU), (2, 1, 1, ACT_NONE)] * num_resblock
+        if self.lin:
             self.launches = 1 + 4 + 1
 
     def run_bicubic(self, lr_f32, lr_cpitch=3):
@@ -162,7 +164,7 @@ class GeneratorPlan:
 
 
 class FNetPlan:
-    """Pre-allocated bf16 pipeline for fnet on [n,h,w] inputs: 14 tcgen05 launches + 3 max-pools + 3 resizes."""
+    """Pre-allocated bf16 pipeline for fnet on [n,h,w] inputs: 14 wgmma launches + 3 max-pools + 3 resizes."""
 
     def __init__(self, scope, n, h, w, device):
         self.n, self.h, self.w = n, h, w

@@ -1,7 +1,7 @@
-"""Generate tests/golden/*.npz by executing the REFERENCE's own Python (read from
-/root/reference, never copied) under tests/golden/tf_shim.py.  Run once in the build
-container:  python tests/golden/make_golden.py
-The GPU box has no /root/reference; tests only read the committed .npz files.
+"""Generate tests/golden/*.npz by executing the REFERENCE's own Python (read from a checkout of
+thunil/TecoGAN named by $TECOGAN_REFERENCE, never copied) under tests/golden/tf_shim.py:
+    TECOGAN_REFERENCE=/path/to/TecoGAN python tests/golden/make_golden.py
+The tests only read the committed .npz files; they never need the reference.
 
 What the vectors pin: the reference's graph wiring (see tf_shim.py docstring).  Parameters are
 regenerated at test time from the seeds stored in each file (oracle.init_*), so the fixtures
@@ -16,7 +16,7 @@ import torch
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 sys.path.insert(0, ROOT)
-REF = "/root/reference"
+REF = os.environ.get("TECOGAN_REFERENCE", "TecoGAN")
 
 from oracle import teco_oracle as O  # noqa: E402
 from tests.golden import tf_shim  # noqa: E402

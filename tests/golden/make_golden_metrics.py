@@ -1,11 +1,11 @@
 """Generate tests/golden/metrics.npz by executing the REFERENCE's own metric functions.
 
-/root/reference/metrics.py cannot be imported (module-level cv2 / skimage / LPIPS imports and a flag-driven main loop), so
+The reference's metrics.py cannot be imported (module-level cv2 / skimage / LPIPS imports and a flag-driven main loop), so
 its pure-numpy functions `_rgb2ycbcr`, `to_uint8`, `psnr` and `crop_8x8` (metrics.py:37-70, 77-92) are taken out of the
-file's syntax tree and executed unmodified with numpy (read from /root/reference, never copied into the repo).
+file's syntax tree and executed unmodified with numpy (read from the checkout named by $TECOGAN_REFERENCE, never copied into the repo).
 `ssim` (metrics.py:72-75) calls skimage.measure.compare_ssim, which is not installed: it is pinned in
 tests/test_oracle_golden.py by a second derivation (direct window sums) instead.
-Run once in the build container:  python tests/golden/make_golden_metrics.py
+Run once:  TECOGAN_REFERENCE=/path/to/TecoGAN python tests/golden/make_golden_metrics.py
 """
 import ast
 import os
@@ -13,7 +13,7 @@ import os
 import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-SRC = "/root/reference/metrics.py"
+SRC = os.path.join(os.environ.get("TECOGAN_REFERENCE", "TecoGAN"), "metrics.py")
 WANT = ("_rgb2ycbcr", "to_uint8", "psnr", "crop_8x8")
 
 

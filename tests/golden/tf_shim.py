@@ -1,6 +1,6 @@
 """A minimal *eager* stand-in for the TensorFlow-1.x API surface the reference touches on the
-hot path, so that the reference's own Python (lib/ops.py, lib/frvsr.py, lib/Teco.py under
-/root/reference) can be executed in this container to produce golden vectors.
+hot path, so that the reference's own Python (lib/ops.py, lib/frvsr.py, lib/Teco.py of a
+reference checkout) can be executed without TensorFlow to produce golden vectors.
 
 Scope and honesty: TensorFlow itself is not installable here, so the *primitive* semantics
 (SAME padding, conv2d_transpose alignment, legacy resize, dense_image_warp, fused BN) come

@@ -227,7 +227,7 @@ def test_adam_matches_tf_formulation():
     assert_close(dp, P["a"], 1e-7, what="adam")
 
 
-# ------------------------------------------------------------------------------------ tcgen05 kernel
+# ------------------------------------------------------------------------------------ wgmma kernel
 def _bf(t):
     return t.to(torch.bfloat16).to(torch.float32)
 
@@ -281,11 +281,11 @@ def _lin_chain_reference(x, layers, plan):
     (3, 32, [(0, 1, -1, 0)]),
     (5, 8, [(0, 1, 2, 2)]),                                                # external residual from buf_b, LeakyReLU
     (2, 32, [(0, 1, -1, 1), (1, 2, -1, 1), (2, 1, 1, 0)]),                  # input conv + one residual block (in-place residual)
-    (150, 32, [(0, 1, -1, 1), (1, 2, -1, 1), (2, 1, 1, 0), (1, 2, -1, 1), (2, 1, 1, 0)]),   # > 148 images: CTAs with 1 and 2 images
+    (150, 32, [(0, 1, -1, 1), (1, 2, -1, 1), (2, 1, 1, 0), (1, 2, -1, 1), (2, 1, 1, 0)]),   # > 132 images: more images than SMs
     (7, 12, [(0, 1, -1, 1)] + [(1, 2, -1, 1), (2, 1, 1, 0)] * 4),            # 9 layers: weight double buffer wraps
 ])
 def test_conv3x3_lin_chain_matches_oracle_on_bf16_operands(n, h, plan):
-    """teco_conv3x3_lin_tc: kx-fused N=192 MMAs on row-linearised 32-pixel-wide images, multi-layer in one launch."""
+    """teco_conv3x3_lin_tc: the multi-layer chain on 32-pixel-wide images in one launch (CTA-local images across layers)."""
     from tecogan_b200 import kernels as K
     L = len(plan)
     x = _bf(rnd(1, n, h, 32, 64))
@@ -335,7 +335,7 @@ def test_conv3x3_tc_fp32_output_stage():
 
 
 def test_conv3x3_tc_fp32_output_stage_streaming_from_hbm():
-    """The 64->3 output stage on an input larger than L2 (deep halo ring, many tiles per persistent CTA); checked against
+    """The 64->3 output stage on an input larger than L2 (many tiles per persistent CTA); checked against
     the oracle on a few sampled images."""
     from tecogan_b200 import kernels as K
     n, h, w = 48, 128, 128                      # 48 x 128 x 128 x 64 ch bf16 = 100 MB
@@ -354,7 +354,7 @@ def test_conv3x3_tc_fp32_output_stage_streaming_from_hbm():
 
 @pytest.mark.parametrize("n,h,w,c", [(3, 128, 128, 3), (2, 144, 180, 3), (1, 512, 512, 3), (40, 32, 32, 2), (7, 48, 22, 4)])
 def test_kx_fused_narrow_output_stage_matches_oracle(n, h, w, c):
-    """Many-tile fp32 output stages run the kx-fused kernel (one MMA per kernel row, shuffle-combined columns): every
+    """Many-tile fp32 output stages (Cout padded to 16, fp32 output straight from the accumulators): every
     width class (multiple of the tile width or not), with and without the bicubic residual."""
     from tecogan_b200 import kernels as K
     g = torch.Generator().manual_seed(11)
@@ -365,16 +365,16 @@ def test_kx_fused_narrow_output_stage_matches_oracle(n, h, w, c):
     out = torch.zeros(n, h, w, c, device="cuda")
     K.conv3x3_tc(x.cuda(), wpk, K.pad_bias(dev(b), 16), cout=16, out_f32=out, res_f32=bic.cuda(), post=(2.0, -1.0))
     ref = (O.conv2d(x[:2].float(), wt, b) + bic[:2]) * 2 - 1
-    assert_close(out[:2], ref, 1e-4, what="kx-fused output stage")
+    assert_close(out[:2], ref, 1e-4, what="narrow output stage")
     out2 = torch.zeros(n, h, w, c, device="cuda")
     K.conv3x3_tc(x.cuda(), wpk, K.pad_bias(dev(b), 16), cout=16, act=K.ACT_TANH24, out_f32=out2)
     ref2 = torch.tanh(O.conv2d(x[-1:].float(), wt, b)) * 24.0
-    assert_close(out2[-1:], ref2, 2e-4, what="kx-fused tanh head")
+    assert_close(out2[-1:], ref2, 2e-4, what="narrow tanh head")
 
 
 @pytest.mark.parametrize("n,h,w,cin,cout", [(1, 8, 16, 64, 64), (4, 32, 32, 64, 64), (2, 19, 21, 51, 64), (3, 16, 24, 128, 32), (2, 32, 32, 32, 256)])
 def test_conv3x3_wgrad_tc_matches_autograd_on_bf16_operands(n, h, w, cin, cout):
-    """tcgen05 weight gradient (pixels as the GEMM K dimension, MN-major operands, two taps per MMA) against torch autograd
+    """wgmma weight gradient (pixels as the GEMM K dimension, MN-major operands, one accumulator per tap) against torch autograd
     of the oracle convolution on the same bf16-rounded x and dz; ragged sizes exercise the zero-filled tile edges."""
     from tecogan_b200 import kernels as K
     x, dz = _bf(rnd(1, n, h, w, cin)), _bf(rnd(2, n, h, w, cout))

@@ -215,7 +215,7 @@ def _y_psnr_delta(frames_lr, ours01, ref01):
 @pytest.mark.parametrize("B", [6, 12])
 def test_metric_config_clip_engine_matches_oracle_and_streaming_engine(B):
     """bench.py headline path: B clips x 10 frames 32x32 in lock-step, one CUDA graph, fnet for all pairs first.
-    B = 12 takes the one-launch row-linearised trunk (teco_conv3x3_lin_tc, batches of >= 8 clips), B = 6 one launch per layer."""
+    B = 12 takes the one-launch trunk (teco_conv3x3_lin_tc, batches of >= 8 clips), B = 6 one launch per layer."""
     from tecogan_b200 import config
     from tecogan_b200.engine import ClipEngine, InferenceEngine
     T, N = 10, 16
@@ -223,6 +223,8 @@ def test_metric_config_clip_engine_matches_oracle_and_streaming_engine(B):
     clips = _smooth_clips(T, B, 32, 32, seed=3)
     _fresh_store({**pg, **pf})
     config.set_precision("bf16")
+    prev_lin = config.lin_trunk()
+    config.set_lin_trunk(True)                           # the one-launch chain at B >= 8; the per-layer kernels below
     eng = ClipEngine(32, 32, T, N, batch=B)
     assert eng.gen.lin == (B >= 8)
     u8 = eng.run(clips.cuda()).clone()
@@ -252,9 +254,10 @@ def test_metric_config_clip_engine_matches_oracle_and_streaming_engine(B):
             assert not per_layer.gen.lin
             u8_pl = per_layer.run(clips.cuda())
         finally:
-            config.set_lin_trunk(True)
+            config.set_lin_trunk(prev_lin)
         diff = (u8.float() - u8_pl.float()).abs()
         assert diff.max().item() <= 3 and diff.mean().item() < 0.05, (diff.max().item(), diff.mean().item())
+    config.set_lin_trunk(prev_lin)
 
 
 def test_configs1_128x128_lookahead_graph_32_frames_matches_oracle():

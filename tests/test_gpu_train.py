@@ -150,7 +150,7 @@ def test_gauss_down_loader_matches_oracle():
 
 
 def test_bf16_tensor_core_training_step_close_to_fp32_oracle():
-    """--precision bf16 for training: 3x3 convs run forward + input-gradient on tcgen05 (bf16 operands, fp32 accumulate,
+    """--precision bf16 for training: 3x3 convs run forward + input-gradient on wgmma (bf16 operands, fp32 accumulate,
     fp32 master weights).  Losses within 2e-2 relative of the fp32 oracle, gradient direction preserved (cosine > 0.99)."""
     from tecogan_b200 import config
     from tecogan_b200.lib.Teco import FRVSR
@@ -175,7 +175,7 @@ def test_bf16_tensor_core_training_step_close_to_fp32_oracle():
 
 
 def test_bf16_tensor_core_tecogan_step_with_vgg_close_to_fp32_oracle():
-    """Same for the full TecoGAN graph: VGG19 (frozen, up to 512 channels) also runs on tcgen05 in bf16 mode."""
+    """Same for the full TecoGAN graph: VGG19 (frozen, up to 512 channels) also runs on wgmma in bf16 mode."""
     from tecogan_b200 import config
     from tecogan_b200.lib.Teco import TecoGAN
     g, FL, P = _case("teco_pp")

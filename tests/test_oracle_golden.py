@@ -198,7 +198,7 @@ def test_tfext_legacy_resize_batchnorm_pool_s2d():
 
 
 # ---- evaluation metrics (SURVEY 8f-3): the oracle against the reference's own psnr / crop_8x8 / _rgb2ycbcr outputs
-# (tests/golden/make_golden_metrics.py executes those functions out of /root/reference/metrics.py) --------------------
+# (tests/golden/make_golden_metrics.py executes those functions out of the reference's metrics.py) --------------------
 def _metric_cases():
     g = _load("metrics")
     for i in range(int(g["n_cases"])):
