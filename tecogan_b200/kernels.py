@@ -636,12 +636,12 @@ class _Conv3x3TC(torch.autograd.Function):
         Cin, Cout = w.shape[2], w.shape[3]
         cip, cop = _pad64(Cin), _pad64(Cout)
         xb = _to_bf16_rows(x, cip)
-        if Cout < 16 and res is None:
-            # narrow output (generator 64 -> 3, fnet 32 -> 2): the fp32-output stage of the inference path -- the network's
-            # output is not rounded to bf16
+        if Cout < 16:
+            # narrow output (generator 64 -> 3 + fp32 bicubic residual, fnet 32 -> 2): the fp32-output stage of the
+            # inference path -- the network's output is not rounded to bf16, and the residual is added in fp32
             wpk, bp = _tc_packed(w, b, 0, cip, 16)
             y = torch.empty(x.shape[:3] + (Cout,), device=x.device, dtype=f32)
-            conv3x3_tc(xb, wpk, bp, None, cout=16, act=act, out_f32=y)
+            conv3x3_tc(xb, wpk, bp, None, cout=16, act=act, out_f32=y, res_f32=None if res is None else _cc(res))
         else:
             wpk, bp = _tc_packed(w, b, 0, cip, cop)
             yb = conv3x3_tc(xb, wpk, bp, cout=cop, act=act)

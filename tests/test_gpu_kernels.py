@@ -244,6 +244,83 @@ def _xpad(x):
     return out
 
 
+# Error model of the float64 references of the bf16 training convolutions.  The products of bf16 operands are exact in fp32;
+# each tensor-core K-step (16 products into the fp32 accumulator) and each later fp32 add (bias, residual, one atomicAdd of
+# a tile's partial dW) is off by at most one fp32 ulp of the running sum -- 2^-23 of sum|terms|, twice the round-to-nearest
+# bound, because the tensor cores' adder may truncate.  An fp32 result of S such steps is therefore within
+# S * 2^-23 * sum|terms| of the exact value, where sum|terms| is the same operation evaluated on |operands|.  A result
+# rounded to bf16 may in addition land on the neighbouring bf16 value: one bf16 ulp, at most 2^-7 of its magnitude.
+_STEP = 2.0 ** -23
+_BF_ULP = 2.0 ** -7
+
+
+def _act64(act, z):
+    return {0: lambda v: v, 1: torch.relu, 2: O.lrelu, 3: lambda v: torch.tanh(v) * 24}[act](z)
+
+
+def _act_grad64(act, y):
+    """act'(.) from the saved output y, as the backward pass computes it (LeakyReLU: y >= 0, like the forward's z >= 0)."""
+    if act == 1:
+        return (y > 0).double()
+    if act == 2:
+        return torch.where(y >= 0, torch.ones_like(y), torch.full_like(y, 0.2))
+    if act == 3:
+        return 24.0 * (1.0 - (y / 24.0) ** 2)
+    return torch.ones_like(y)
+
+
+def _bf_tie_ulp(v):
+    """One bf16 ulp where v (float64) lies within 2^-20 |v| of a bf16 rounding midpoint, else 0: there the fp32 arithmetic
+    of the kernel (a few fp32 roundings away from float64) may round v to either neighbour.  Zero for every element of a
+    bf16-valued dy times 1 or 0.2, so it only matters for tanh."""
+    ulp = torch.pow(2.0, torch.floor(torch.log2(v.abs().clamp_min(1e-30))) - 7)
+    near = ((v - _bf(v).double()).abs() - ulp / 2).abs() <= 2.0 ** -20 * v.abs()
+    return torch.where(near & (v != 0), ulp, torch.zeros_like(v))
+
+
+def _lin_grads(op, a, b, g):
+    """Gradients of <op(a, b), g> with respect to a and b, for op linear in each argument (float64 autograd)."""
+    a, b = a.detach().clone().requires_grad_(True), b.detach().clone().requires_grad_(True)
+    return torch.autograd.grad(op(a, b), (a, b), g)
+
+
+def _train_ref(op, x, w, b, act, dy, y_saved, round_y=True, res=None):
+    """float64 reference of one bf16 training convolution with the rounding points of kernels.py (_Conv3x3TC,
+    _ConvTranspose2xTC): operands rounded to bf16, y = bf16(act(op(x, w) + b)) (+ res in fp32) -- or, for the narrow fp32
+    output stage (round_y=False), act(op(x, w) + b) (+ res) unrounded -- dz = act'(y as saved) * dy, dzb = bf16(dz),
+    dx = bf16(input-grad(dzb, w)), dw = weight-grad(x, dzb), db = sum(dz).  Each value comes with its sum|terms|; the dz
+    ties of _bf_tie_ulp come with what they can move dx and dw by."""
+    xb, wb, b64 = _bf(x).double(), _bf(w).double(), b.double()
+    z = _act64(act, op(xb, wb) + b64)
+    s_z = op(xb.abs(), wb.abs()) + b64.abs()
+    y = _bf(z).double() if round_y else z
+    if res is not None:
+        y, s_z = y + res.double(), s_z + res.double().abs()
+    dz = _act_grad64(act, y_saved.detach().double().cpu()) * dy.double()
+    dzb, tie = _bf(dz).double(), _bf_tie_ulp(dz)
+    dx, dw = _lin_grads(op, xb, wb, dzb)
+    s_dx, s_dw = _lin_grads(op, xb.abs(), wb.abs(), dzb.abs())
+    t_dx, t_dw = _lin_grads(op, xb.abs(), wb.abs(), tie) if bool(tie.any()) else (torch.zeros_like(xb), torch.zeros_like(wb))
+    return dict(y=y, s_y=s_z, dx=_bf(dx).double(), s_dx=s_dx, t_dx=t_dx, dw=dw, s_dw=s_dw, t_dw=t_dw,
+                db=dz.sum(dim=(0, 1, 2)), s_db=dz.abs().sum(dim=(0, 1, 2)))
+
+
+def _wgrad_tiles(n, h, w):
+    """Tiles of the weight-gradient kernel (8 x 16 pixels); each adds its partial dW to every element with one atomic."""
+    return n * -(-h // 8) * -(-w // 16)
+
+
+def _assert_within(got, ref, bound, what):
+    assert got is not None, what + ": missing"
+    got = got.detach().double().cpu()
+    assert tuple(got.shape) == tuple(ref.shape), (what, tuple(got.shape), tuple(ref.shape))
+    err = (got - ref).abs()
+    bad = ~(err <= bound)
+    i = int(torch.argmax(err / bound.clamp_min(1e-30)))
+    assert not bad.any(), "%s: %d/%d elements outside the bound; max err %.3e; worst err/bound %.3e / %.3e" % (
+        what, int(bad.sum()), bad.numel(), err.max().item(), err.flatten()[i].item(), bound.flatten()[i].item())
+
+
 @pytest.mark.parametrize("n,h,w,cin,cout,act", [
     (1, 16, 8, 64, 64, 0), (1, 32, 32, 64, 64, 1), (2, 48, 40, 64, 64, 2), (1, 19, 21, 16, 32, 2), (1, 32, 32, 32, 64, 0),
     (1, 16, 16, 128, 256, 2), (1, 16, 24, 256, 128, 2), (1, 64, 64, 64, 16, 0), (1, 128, 128, 64, 64, 1), (3, 32, 32, 128, 128, 0),
@@ -372,24 +449,201 @@ def test_kx_fused_narrow_output_stage_matches_oracle(n, h, w, c):
     assert_close(out2[-1:], ref2, 2e-4, what="narrow tanh head")
 
 
-@pytest.mark.parametrize("n,h,w,cin,cout", [(1, 8, 16, 64, 64), (4, 32, 32, 64, 64), (2, 19, 21, 51, 64), (3, 16, 24, 128, 32), (2, 32, 32, 32, 256)])
+@pytest.mark.parametrize("n,h,w,cin,cout", [
+    (1, 8, 16, 64, 64), (4, 32, 32, 64, 64), (2, 19, 21, 51, 64), (3, 16, 24, 128, 32), (2, 32, 32, 32, 256),
+    (2, 9, 40, 256, 64),            # the transposed conv's space-to-depth shape: four 64-channel input blocks
+    (2, 13, 21, 64, 4),             # Cout rounded up to 4 (the narrow generator / FNet output layers)
+    (3, 5, 7, 32, 64),              # smaller than one 8 x 16 tile in both directions
+])
 def test_conv3x3_wgrad_tc_matches_autograd_on_bf16_operands(n, h, w, cin, cout):
-    """wgmma weight gradient (pixels as the GEMM K dimension, MN-major operands, one accumulator per tap) against torch autograd
-    of the oracle convolution on the same bf16-rounded x and dz; ragged sizes exercise the zero-filled tile edges."""
+    """wgmma weight gradient (pixels as the GEMM K dimension, MN-major operands, one accumulator per tap) against float64
+    autograd of the oracle convolution on the same bf16-rounded x and dz; ragged sizes exercise the zero-filled tile edges.
+    Bound per element (error model above): 8 K-steps per tile plus one atomicAdd per tile, (8 + tiles) * 2^-23 * sum|x dz|
+    -- with the initial |dw| added to sum|terms| when accumulating onto a non-zero dw.  db: fp32 sum over the pixels,
+    npix * 2^-23 * sum|dz|."""
     from tecogan_b200 import kernels as K
     x, dz = _bf(rnd(1, n, h, w, cin)), _bf(rnd(2, n, h, w, cout))
-    wt = torch.zeros(3, 3, cin, cout, requires_grad=True)
-    (O.conv2d(x, wt, None) * dz).sum().backward()
-    ref = wt.grad
+    ref, _ = _lin_grads(lambda c, a: O.conv2d(a, c), torch.zeros(3, 3, cin, cout, dtype=torch.float64), x.double(), dz.double())
+    s_ref, _ = _lin_grads(lambda c, a: O.conv2d(a, c), torch.zeros(3, 3, cin, cout, dtype=torch.float64), x.double().abs(),
+                          dz.double().abs())
+    gamma = (8 + _wgrad_tiles(n, h, w)) * _STEP
     dw = torch.full((3, 3, cin, cout), 7.0, device="cuda")
     K.conv3x3_wgrad_tc(_xpad(x), _xpad(dz), dw, cin, cout)
-    scale = ref.abs().max().item()
-    per_tap = [round((dw.cpu()[t // 3, t % 3] - ref[t // 3, t % 3]).abs().max().item() / scale, 4) for t in range(9)]
-    assert max(per_tap) < 2e-3, per_tap
+    _assert_within(dw, ref, gamma * s_ref, "wgrad")
+    dw0 = rnd(3, 3, 3, cin, cout, lo=-2.0, hi=2.0) * s_ref.max().item()
+    dw = dev(dw0)
     K.conv3x3_wgrad_tc(_xpad(x), _xpad(dz), dw, cin, cout, accumulate=True)
-    assert (dw.cpu() - 2 * ref).abs().max().item() < 4e-3 * scale
+    _assert_within(dw, dw0.double() + ref, gamma * (s_ref + dw0.double().abs()), "wgrad accumulate")
     db = K.bias_grad(dev(dz))
-    assert (db.cpu() - dz.sum(dim=(0, 1, 2))).abs().max().item() < 1e-3 * dz.abs().sum().item() ** 0.5
+    npix = n * h * w
+    _assert_within(db, dz.double().sum(dim=(0, 1, 2)), npix * _STEP * dz.double().abs().sum(dim=(0, 1, 2)), "bias grad")
+
+
+# ------------------------------------------------------------------------------------ bf16 training convolutions
+# The tests below call y.grad_fn.apply(dy): the autograd Function's backward itself, so they see every gradient it returns,
+# including the None it must return for an input that needs no gradient.
+_RELU, _LRELU, _TANH24 = 1, 2, 3
+
+
+@pytest.mark.parametrize("n,h,w,cin,cout,act,res,x_grad,w_grad", [
+    (2, 19, 13, 51, 64, _RELU, False, False, True),       # generator input stage (LR frame + warped s2d; no dx)
+    (1, 21, 30, 64, 64, _RELU, False, True, True),        # generator residual block, conv_1
+    (2, 17, 9, 64, 64, 0, True, True, True),              # generator residual block, conv_2 + residual
+    (2, 23, 18, 64, 3, 0, True, True, True),              # generator output conv + fp32 bicubic residual
+    (1, 5, 3, 64, 3, 0, True, True, True),                #   ... on an image smaller than one tile
+    (12, 67, 150, 64, 3, 0, True, True, True),            #   ... more tiles than the persistent grid has CTAs
+    (2, 18, 20, 6, 32, _LRELU, False, False, True),       # fnet input (two LR frames; no dx)
+    (1, 5, 3, 32, 32, _LRELU, False, True, True),
+    (1, 9, 11, 128, 256, _LRELU, False, True, True),
+    (1, 13, 7, 256, 128, _LRELU, False, True, True),
+    (2, 18, 20, 64, 32, _LRELU, False, True, True),
+    (2, 17, 25, 32, 2, _TANH24, False, True, True),       # fnet output: tanh * 24 (the flow), narrow fp32 output stage
+    (1, 12, 10, 3, 64, _RELU, False, True, False),        # VGG19 conv1_1: frozen weights, dx only
+    (1, 6, 5, 256, 512, _RELU, False, True, False),       # VGG19 conv4_1
+    (1, 5, 3, 512, 512, _RELU, False, True, False),       # VGG19 conv4_2 .. conv5_4
+    (2, 11, 14, 27, 64, _LRELU, False, True, True),       # discriminator input stage
+])
+def test_conv3x3_train_tc_matches_float64_reference(n, h, w, cin, cout, act, res, x_grad, w_grad):
+    """conv3x3_train_tc (the bf16 training convolution behind conv2() and the VGG trunk): forward, input, weight, bias and
+    residual gradients against _train_ref, per element.  Tolerances from the error model above:
+      y (Cout >= 16, bf16)       one bf16 ulp + (9 Cin_pad/16 + 3) * 2^-23 * sum|terms|   (K-steps, bias, act, residual)
+      y (Cout < 16, fp32)        L * (9 Cin_pad/16 + 3) * 2^-23 * sum|terms|, L = 24 for tanh * 24 (its slope bound), plus
+                                 4 fp32 ulps of |y| for tanhf and the * 24
+      dx (bf16)                  one bf16 ulp + (9 Cout_pad/16 + 1) * 2^-23 * sum|w dzb|
+      dw (fp32)                  (8 + weight-gradient tiles) * 2^-23 * sum|x dzb|
+      db (fp32)                  (npix + 8) * 2^-23 * sum|dz|
+    plus, for dx and dw, what the dz elements on a bf16 rounding tie (_bf_tie_ulp) can move them by.  The residual
+    gradient is dy itself."""
+    from tecogan_b200 import kernels as K
+    x = rnd(1, n, h, w, cin)
+    wt = rnd(2, 3, 3, cin, cout) * (3.0 / (9 * cin)) ** 0.5
+    b = rnd(3, cout) * 0.1
+    r = rnd(4, n, h, w, cout) if res else None
+    dy = _bf(rnd(5, n, h, w, cout))
+    K.tc_cache_clear()
+    xg, wg, bg = dev(x).requires_grad_(x_grad), dev(wt).requires_grad_(w_grad), dev(b).requires_grad_(w_grad)
+    y = K.conv3x3_train_tc(xg, wg, bg, act, None if r is None else dev(r))
+    dyg = dev(dy)
+    dx, dw, db, _, dres = y.grad_fn.apply(dyg)
+    torch.cuda.synchronize()
+    narrow = cout < 16
+    ref = _train_ref(O.conv2d, x, wt, b, act, dy, y, round_y=not narrow, res=r)
+
+    steps_f = 9 * _p64(cin) // 16 + 3
+    if narrow:
+        lip = 24.0 if act == _TANH24 else 1.0
+        bound_y = lip * steps_f * _STEP * ref["s_y"] + (4 * _STEP * ref["y"].abs() if act == _TANH24 else 0.0)
+    else:
+        bound_y = _BF_ULP * ref["y"].abs() + steps_f * _STEP * ref["s_y"]
+    _assert_within(y, ref["y"], bound_y, "y")
+    if x_grad:
+        steps_d = 9 * _p64(cout) // 16 + 1
+        _assert_within(dx, ref["dx"], _BF_ULP * ref["dx"].abs() + steps_d * _STEP * ref["s_dx"] + ref["t_dx"], "dx")
+    else:
+        assert dx is None, "dx computed for an input that needs no gradient"
+    if w_grad:
+        gamma_w = (8 + _wgrad_tiles(n, h, w)) * _STEP
+        _assert_within(dw, ref["dw"], gamma_w * ref["s_dw"] + ref["t_dw"], "dw")
+        _assert_within(db, ref["db"], (n * h * w + 8) * _STEP * ref["s_db"], "db")
+    else:
+        assert dw is None and db is None, "weight gradient computed for frozen weights"
+    if res:
+        assert dres is not None and torch.equal(dres, dyg), "the residual gradient is dy"
+    else:
+        assert dres is None
+
+
+@pytest.mark.parametrize("act", [0, _RELU, _LRELU])
+@pytest.mark.parametrize("n,h,w", [(1, 5, 7), (2, 9, 40), (3, 32, 32)])
+def test_conv_transpose2x_train_tc_matches_float64_reference(n, h, w, act):
+    """conv_transpose2x_train_tc (conv2_tran 64 -> 64, bf16 training): the 4-phase forward, and both gradients through the
+    space-to-depth rewrite -- a 256-channel dz feeding the weight-streaming path of teco_conv3x3_tc (dx) and the shifted
+    operand of teco_conv3x3_wgrad_tc (dw) -- against _train_ref with the float64 transposed convolution.  Tolerances from
+    the error model above:
+      y (bf16)    one bf16 ulp + (9 * 64/16 + 3) * 2^-23 * sum|terms|   (at most all nine taps per output phase)
+      dx (bf16)   one bf16 ulp + (9 * 256/16 + 1) * 2^-23 * sum|w dzb|
+      dw (fp32)   (8 + weight-gradient tiles of the LR grid) * 2^-23 * sum|x dzb|
+      db (fp32)   (npix + 8) * 2^-23 * sum|dz| over the 2x output."""
+    from tecogan_b200 import kernels as K
+    x = rnd(1, n, h, w, 64)
+    wt = rnd(2, 3, 3, 64, 64) * (3.0 / (4 * 64)) ** 0.5
+    b = rnd(3, 64) * 0.1
+    dy = _bf(rnd(5, n, 2 * h, 2 * w, 64))
+    K.tc_cache_clear()
+    xg, wg, bg = dev(x).requires_grad_(True), dev(wt).requires_grad_(True), dev(b).requires_grad_(True)
+    y = K.conv_transpose2x_train_tc(xg, wg, bg, act)
+    dx, dw, db, _ = y.grad_fn.apply(dev(dy))
+    torch.cuda.synchronize()
+    ref = _train_ref(O.conv2d_transpose, x, wt, b, act, dy, y)
+    _assert_within(y, ref["y"], _BF_ULP * ref["y"].abs() + (9 * 64 // 16 + 3) * _STEP * ref["s_y"], "y")
+    _assert_within(dx, ref["dx"], _BF_ULP * ref["dx"].abs() + (9 * 256 // 16 + 1) * _STEP * ref["s_dx"] + ref["t_dx"], "dx")
+    _assert_within(dw, ref["dw"], (8 + _wgrad_tiles(n, h, w)) * _STEP * ref["s_dw"] + ref["t_dw"], "dw")
+    _assert_within(db, ref["db"], (4 * n * h * w + 8) * _STEP * ref["s_db"], "db")
+
+
+def _pack_ref(w, cin_pad, cout_pad, flags, cin_perm=None):
+    """teco_pack_conv3x3_bf16 restated in numpy: w [3,3,cin,cout] ([3,3,cout,cin] with flag bit 0; taps flipped with bit 1)
+    -> bf16 bits [cin_pad/64][tap][cout_pad][16-byte chunk j ^ (co & 7)][8]; packed input channel k reads cin_perm[k]
+    (-1: zero).  bf16 rounding is torch's round-to-nearest-even."""
+    w = np.asarray(w, dtype=np.float32)
+    if flags & 1:
+        w = w.transpose(0, 1, 3, 2)
+    if flags & 2:
+        w = w[::-1, ::-1]
+    cin, cout = w.shape[2], w.shape[3]
+    w = w.reshape(9, cin, cout)
+    src = np.asarray(cin_perm if cin_perm is not None else [k if k < cin else -1 for k in range(cin_pad)])
+    full = np.zeros((9, cin_pad, cout_pad), dtype=np.float32)
+    ok = (src >= 0) & (src < cin)
+    full[:, ok, :cout] = w[:, src[ok], :]
+    bits = torch.from_numpy(full).to(torch.bfloat16).view(torch.int16).numpy()
+    blk = bits.reshape(9, cin_pad // 64, 8, 8, cout_pad).transpose(1, 0, 4, 2, 3)    # [blk][tap][co][j][e]
+    co = np.arange(cout_pad)[:, None]
+    return blk[:, :, co, np.arange(8)[None, :] ^ (co & 7), :].reshape(-1)
+
+
+@pytest.mark.parametrize("cin,cout,cin_pad,cout_pad,flags,perm", [
+    (64, 64, 64, 64, 0, False), (51, 64, 64, 64, 0, True), (64, 3, 64, 16, 0, False), (6, 32, 64, 32, 0, False),
+    (256, 512, 256, 512, 0, False), (64, 64, 64, 64, 1, False), (64, 64, 64, 64, 3, False), (2, 32, 64, 64, 3, False),
+    (3, 64, 64, 64, 3, False), (128, 256, 128, 256, 3, False), (64, 3, 64, 64, 3, False),
+])
+def test_packed_weight_layout_is_bit_exact(cin, cout, cin_pad, cout_pad, flags, perm):
+    """K.packed_weight bit for bit against the SWIZZLE_128B layout restated on the host: separates a packing error from a
+    kernel error.  cin / cout are the packed (GEMM) channel counts; with flag bit 0 the weights are stored [3,3,cout,cin].
+    Flag 3 is the input-gradient packing of _Conv3x3TC: the weights of a cout -> cin convolution with the taps flipped
+    (fnet 32 -> 2, generator 64 -> 3, fnet 256 -> 128, VGG 3 -> 64 above)."""
+    from tecogan_b200 import kernels as K
+    from tecogan_b200.tc_nets import GEN_CIN_PERM
+    shape = (3, 3, cout, cin) if flags & 1 else (3, 3, cin, cout)
+    wt = rnd(9, *shape) * 3.0
+    p = GEN_CIN_PERM if perm else None
+    got = K.packed_weight(dev(wt), cin_pad, cout_pad, flags, cin_perm=p).view(torch.int16).cpu().numpy()
+    ref = _pack_ref(wt.numpy(), cin_pad, cout_pad, flags, p)
+    assert got.shape == ref.shape and np.array_equal(got, ref), int((got != ref).sum())
+
+
+@pytest.mark.parametrize("c", [8, 64, 256])
+def test_fnet_bf16_glue_kernels_match_oracle(c):
+    """The bf16 glue of FNet inference, on bf16-valued inputs with odd sizes.  maxpool2_bf16 is a max, so bit-exact;
+    resize2x_bf16 is the oracle's legacy bilinear x2 (weights 0 and 1/2) in fp32 rounded once to bf16 -- at most one bf16
+    ulp apart if the association differs; f32_to_bf16_pad (round-to-nearest-even, a channel offset into a wider pitch, the
+    other channels untouched) and bf16_to_f32 (a source pitch wider than C) are exact."""
+    from tecogan_b200 import kernels as K
+    x = _bf(rnd(1, 2, 9, 7, c))
+    xb = dev(x).to(torch.bfloat16)
+    got = K.maxpool2_bf16(xb)
+    assert torch.equal(got.float().cpu(), O.maxpool(x)), "maxpool2_bf16"
+    got = K.resize2x_bf16(xb).float().cpu()
+    ref = _bf(O.resize_bilinear_legacy(x, 18, 14))
+    assert (got - ref).abs().le(_BF_ULP * ref.abs()).all(), "resize2x_bf16: max err %.3e" % (got - ref).abs().max().item()
+    src = rnd(2, 2, 5, 3, c) * 3.0
+    dst = torch.full((2, 5, 3, c + 24), 7.0, device="cuda", dtype=torch.bfloat16)
+    K.f32_to_bf16_pad(dev(src), dst, c, c_off=16, scale=0.5, shift=0.5)
+    want = torch.full((2, 5, 3, c + 24), 7.0, dtype=torch.bfloat16)
+    want[..., 16:16 + c] = (src * 0.5 + 0.5).to(torch.bfloat16)
+    assert torch.equal(dst.cpu().view(torch.int16), want.view(torch.int16)), "f32_to_bf16_pad"
+    back = K.bf16_to_f32(dst[..., 16:].contiguous(), c)
+    assert torch.equal(back.cpu(), want[..., 16:16 + c].float()), "bf16_to_f32"
 
 
 def test_abi_rejects_bad_arguments_with_valueerror():

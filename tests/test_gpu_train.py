@@ -194,6 +194,32 @@ def test_bf16_tensor_core_tecogan_step_with_vgg_close_to_fp32_oracle():
     assert out["with_d"] == ref["with_d"]
 
 
+def test_bf16_second_step_repacks_updated_weights():
+    """Step 2 of --precision bf16 training is a replay of the CUDA graph captured at step 1; the bf16 weight packing runs
+    inside that graph (after tc_cache_clear), so the replay must pack the weights Adam has just updated.  Step 2's losses
+    against the oracle's step 2 at the bf16 loss tolerance of the single-step TecoGAN test above -- in the oracle, two of
+    them move by more than that tolerance from step 1 to step 2, so a replay on stale packed weights fails here."""
+    from tecogan_b200 import config
+    from tecogan_b200.lib.Teco import TecoGAN
+    g, FL, P = _case("teco_pp")
+    ri, rt = torch.from_numpy(g["r_inputs"]), torch.from_numpy(g["r_targets"])
+    tr = O.Trainer(P, FL, True)
+    tr.step(ri, rt)
+    ref2 = tr.step(ri, rt)
+    _fresh_store(P)
+    config.set_train_precision("bf16")
+    try:
+        net = TecoGAN(ri.cuda(), rt.cuda(), FL)
+        net.train()
+        assert net.train.graph is not None, "step 1 did not capture the step graph"
+        out2 = net.train()
+    finally:
+        config.set_train_precision("fp32")
+    assert net.global_step() == 2
+    want = np.array([float(v) for v in ref2["update_list"]])
+    np.testing.assert_allclose(np.array(out2["update_list"]), want, rtol=4e-2, atol=2e-3)
+
+
 @pytest.mark.parametrize("fmt", ["tf", "pt"])
 def test_checkpoint_resume_restores_everything(tmp_path, fmt):
     """Saver semantics (reference main.py:307,346-349,418-421): save after two steps, restore weights + Adam moments +
