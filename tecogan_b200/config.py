@@ -36,8 +36,9 @@ def set_lin_trunk(on):
     """32-pixel-wide frames (the metric configuration's 32x32 LR clips): run the generator's input conv + all residual
     blocks as ONE launch of the multi-layer chain kernel (teco_conv3x3_lin_tc; every CTA keeps its own clips for all
     layers), for batches of at least 8 clips.  Off by default: on an H100 the 33 per-layer launches are faster at every
-    batch measured (8 to 264 clips: 1.4x to 7.6x) -- the chain has one CTA (two warpgroups) per SM in flight, the per-layer
-    kernel many -- so bench.py times the chain next to them instead."""
+    batch measured (8 to 264 clips: 1.4x to 7.6x) -- both have one CTA per SM in flight, but the chain's CTA owns whole
+    images through all 33 layers while the per-layer kernel spreads each layer's small tiles over every SM -- so bench.py
+    times the chain next to them instead."""
     _cfg["lin_trunk"] = bool(on)
 
 

@@ -20,7 +20,9 @@
 // sub-pixel phase accumulators (SURVEY.md A.3) and a 2x interleaving epilogue.
 //
 // Persistent CTAs walk tiles c, c + G, ...; the halo (and weight) ring has two stages, so the TMA of the next 64-channel
-// block or tile is in flight while the warpgroups run the MMAs and the epilogue of the current one.
+// block or tile is in flight while the warpgroups run the MMAs and the epilogue of the current one.  Layers with one
+// 64-channel input block and 64-channel bf16 output slices run on conv3x3_ws_kernel instead: the same MMAs and epilogue
+// arithmetic behind a producer warp, a deeper ring and TMA-staged residuals and stores.
 #include <cuda.h>
 #include "teco_common.cuh"
 #include "tc_ptx.cuh"
@@ -68,9 +70,9 @@ __device__ __forceinline__ void tap_route(int t, int& ry, int& rx, int& ph) {
 }
 
 // The nine taps x four K-steps of one 64-channel block for warpgroup wg: halo stage at halo_a, the block's packed
-// weights [tap][NT][64] at w_a.
+// weights [tap][NT][64] at w_a.  Issues and commits them; mma_block() also waits for them.
 template <int MODE, int NT, int NACC>
-__device__ __forceinline__ void mma_block(float (&acc)[NACC][NT / 2], uint32_t halo_a, uint32_t w_a, int wg) {
+__device__ __forceinline__ void mma_issue(float (&acc)[NACC][NT / 2], uint32_t halo_a, uint32_t w_a, int wg) {
   wgmma_fence();
 #pragma unroll
   for (int t = 0; t < 9; ++t) {
@@ -83,6 +85,11 @@ __device__ __forceinline__ void mma_block(float (&acc)[NACC][NT / 2], uint32_t h
       Wgmma<NT, 0, 0>::run(acc[ph], gmma_desc_sw128(a0 + 32u * k, 16u, HALO_COLS * 128u), gmma_desc_sw128(b0 + 32u * k, 16u, 1024u), 1u);
   }
   wgmma_commit();
+}
+
+template <int MODE, int NT, int NACC>
+__device__ __forceinline__ void mma_block(float (&acc)[NACC][NT / 2], uint32_t halo_a, uint32_t w_a, int wg) {
+  mma_issue<MODE, NT, NACC>(acc, halo_a, w_a, wg);
   wgmma_wait_all();
 }
 
@@ -320,6 +327,193 @@ conv3x3_chain_kernel(const __grid_constant__ CUtensorMap tmap0, const __grid_con
   }
 }
 
+// ------------------------------------------------------------------ warp-specialised 64 -> 64 layer (one K block)
+// Mode 0, Cin = 64, 64 output channels per CTA, bf16 output: the generator trunk, FNet's 64-channel layers and the
+// 64-input-channel training convolutions.  The CTA tile, the MMAs of each warpgroup and the epilogue arithmetic are those
+// of conv3x3_wgmma_kernel, so the results are bit-identical; what differs is the schedule:
+//   - one producer warp bulk-copies the weights once and TMA-loads the halo of each tile into a WS_STAGES-deep ring; a
+//     stage is refilled once all eight consumer warps have arrived on its `empty` barrier after their MMAs completed;
+//   - the two consumer warpgroups alternate in *issuing* MMAs (named barriers 1 and 2): warpgroup 1 may issue tile k once
+//     warpgroup 0 has issued (not completed) tile k, and warpgroup 0 may issue tile k + 1 once warpgroup 1 has issued
+//     tile k.  The barriers order only the issue; the tensor pipe then runs the two issue streams one after the other,
+//     so while it works on one warpgroup's MMAs the other, its own MMAs complete, runs its epilogue.  The epilogues
+//     themselves are not ordered against each other;
+//   - the epilogue does not wait on global loads or stores: each warpgroup has WS_OUT_BUFS SW128 staging tiles for its
+//     box of 8 rows x 8 pixels x 64 channels, used by tiles in turn.  The residual box of tile k + 1 is TMA-loaded into
+//     the next one while the MMAs of tile k run, once the store of tile k + 1 - WS_OUT_BUFS has read it (the store of
+//     tile k - 1 may still be reading its own: shared memory is busy with MMA operands then); the epilogue overwrites
+//     the residual with the bf16 result and one TMA tensor store writes it out (clipped at the image edges).  In-place
+//     residuals (res == y) are safe: each box is read and written by one warpgroup of one CTA only, the load completing
+//     before the store is issued.
+constexpr int WS_STAGES = 4;
+constexpr int WS_THREADS = NUM_THREADS + 32;          // two consumer warpgroups + the producer warp
+constexpr int WS_OUT_BUFS = 3;                        // staging tiles per warpgroup
+constexpr uint32_t WS_OUT_BYTES = 8 * 8 * 128;        // one warpgroup's output box: 8 rows x 8 pixels x 64 bf16
+constexpr size_t WS_SMEM = 1024 + WS_STAGES * (size_t)HALO_STAGE + LAYER_W_BYTES + 2 * WS_OUT_BUFS * WS_OUT_BYTES +
+                           (2 * WS_STAGES + 1 + 2 * WS_OUT_BUFS) * sizeof(uint64_t) + 64 * sizeof(float);
+
+// Epilogue of one warpgroup's box into its staging tile at out_a: bias -> activation -> (+ the residual already in the
+// staging tile) -> bf16, the same fp32 operations as epilogue().  The thread holds pixel (row 2 wq + i, column lane / 4)
+// of the box, channels 8 j + 2 (lane % 4) + {0, 1}: 16-byte chunk j of the pixel's 128-byte row, stored at chunk
+// j ^ (pixel & 7) = j ^ column (SWIZZLE_128B, conflict-free per instruction).
+template <int ACT>
+__device__ __forceinline__ void ws_epilogue(const float (&acc)[32], const float* s_bias, uint32_t out_a, bool res, int wq,
+                                            int lane) {
+  const int col = lane >> 2;
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    const uint32_t px = out_a + (uint32_t)(((2 * wq + i) * 8 + col) * 128 + 4 * (lane & 3));
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const int c = 8 * j + 2 * (lane & 3);
+      float v0 = teco_act(acc[4 * j + 2 * i] + s_bias[c], ACT);
+      float v1 = teco_act(acc[4 * j + 2 * i + 1] + s_bias[c + 1], ACT);
+      const uint32_t e = px + (uint32_t)((j ^ col) << 4);
+      if (res) {
+        uint32_t rb;
+        asm volatile("ld.shared.b32 %0, [%1];" : "=r"(rb) : "r"(e) : "memory");
+        const float2 r = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&rb));
+        v0 += r.x;
+        v1 += r.y;
+      }
+      const __nv_bfloat162 o = __floats2bfloat162_rn(v0, v1);
+      asm volatile("st.shared.b32 [%0], %1;" ::"r"(e), "r"(*reinterpret_cast<const uint32_t*>(&o)) : "memory");
+    }
+  }
+}
+
+__global__ void __launch_bounds__(WS_THREADS, 1)
+conv3x3_ws_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ CUtensorMap ymap,
+                  const __grid_constant__ CUtensorMap rmap, const TcParams p) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  uint8_t* ring = smem;                                              // WS_STAGES halo stages
+  uint8_t* w_s = ring + WS_STAGES * (size_t)HALO_STAGE;              // 9 taps x 64 x 64, resident
+  uint8_t* outs = w_s + LAYER_W_BYTES;                               // [2][WS_OUT_BUFS] staging tiles
+  uint64_t* full = reinterpret_cast<uint64_t*>(outs + 2 * WS_OUT_BUFS * WS_OUT_BYTES);   // [WS_STAGES]
+  uint64_t* empty = full + WS_STAGES;                                      // [WS_STAGES]
+  uint64_t* w_full = empty + WS_STAGES;
+  uint64_t* r_full = w_full + 1;                                           // [2][WS_OUT_BUFS] residual arrived
+  float* s_bias = reinterpret_cast<float*>(r_full + 2 * WS_OUT_BUFS);      // [64]
+
+  const int tid = threadIdx.x, wg = tid >> 7;
+  const int n0 = blockIdx.y * 64;
+  const int G = gridDim.x;
+  const int my_tiles = (int)blockIdx.x < p.num_tiles ? (p.num_tiles - (int)blockIdx.x + G - 1) / G : 0;
+
+  for (int c = tid; c < 64; c += WS_THREADS) s_bias[c] = p.bias ? p.bias[n0 + c] : 0.f;
+  if (tid == 0) {
+    for (int s = 0; s < WS_STAGES; ++s) {
+      mbar_init(smem_u32(&full[s]), 1);
+      mbar_init(smem_u32(&empty[s]), 8);     // one arrival per consumer warp
+    }
+    for (int i = 0; i < 1 + 2 * WS_OUT_BUFS; ++i) mbar_init(smem_u32(&w_full[i]), 1);   // w_full, r_full[]
+    fence_mbar_init();
+  }
+  __syncthreads();
+  if (my_tiles == 0) return;
+
+  auto tile_coords = [&](int it, int& n, int& y0, int& x0) {
+    int tile = (int)blockIdx.x + it * G;
+    const int tx = tile % p.tiles_x;
+    tile /= p.tiles_x;
+    const int ty = tile % p.tiles_y;
+    n = tile / p.tiles_y;
+    x0 = tx * TILE_COLS;
+    y0 = ty * TILE_ROWS;
+  };
+
+  if (wg == 2) {                              // producer warp: one lane issues every load of the ring
+    if (tid == NUM_THREADS) {
+      asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap) : "memory");
+      mbar_expect_tx(smem_u32(w_full), LAYER_W_BYTES);
+      for (int t = 0; t < 9; ++t)
+        bulk_load_1d(smem_u32(w_s + t * 8192u), p.wpk + ((size_t)t * p.Cout + n0) * 128, 8192u, smem_u32(w_full));
+      for (int k = 0; k < my_tiles; ++k) {
+        const int st = k % WS_STAGES;
+        if (k >= WS_STAGES) mbar_wait(smem_u32(&empty[st]), (uint32_t)((k / WS_STAGES - 1) & 1));
+        int n, y0, x0;
+        tile_coords(k, n, y0, x0);
+        const uint32_t bar = smem_u32(&full[st]);
+        mbar_expect_tx(bar, HALO_BYTES);
+        tma_load_4d(smem_u32(ring + (size_t)st * HALO_STAGE), &tmap, bar, 0, x0 - 1, y0 - 1, n);
+      }
+    }
+    return;
+  }
+
+  // consumer warpgroup wg: rows 8 wg .. 8 wg + 7 of every tile
+  const int wq = (tid >> 5) & 3, lane = tid & 31;
+  const bool leader = (tid & 127) == 0;       // issues this warpgroup's residual loads and output stores
+  const int my_turn = 1 + wg, other_turn = 2 - wg;   // named barrier 1 + g: warpgroup g may issue its MMAs
+  // staging tile b of this warpgroup <- the residual box of tile k, unless its rows are all below the image
+  auto load_res = [&](int k, int b) {
+    int n, y0, x0;
+    tile_coords(k, n, y0, x0);
+    if (y0 + 8 * wg >= p.H) return;
+    const uint32_t bar = smem_u32(&r_full[WS_OUT_BUFS * wg + b]);
+    mbar_expect_tx(bar, WS_OUT_BYTES);
+    tma_load_4d(smem_u32(outs + (WS_OUT_BUFS * wg + b) * WS_OUT_BYTES), &rmap, bar, n0, x0, y0 + 8 * wg, n);
+  };
+  // leader: before staging tile b is rewritten, every store from it has read it: all but the newest store, or all of
+  // them if the newest is from b
+  int last_store = -1;
+  auto wait_staging_free = [&](int b) {
+    if (last_store == b) bulk_wait_read<0>();
+    else bulk_wait_read<1>();
+  };
+  uint32_t r_phase = 0;                       // bit b: parity of r_full[WS_OUT_BUFS wg + b]
+  if (p.res && leader) load_res(0, 0);
+  mbar_wait(smem_u32(w_full), 0);
+  float acc[1][32];
+  for (int k = 0; k < my_tiles; ++k) {
+    const int st = k % WS_STAGES, sb = k % WS_OUT_BUFS, sb_next = sb + 1 == WS_OUT_BUFS ? 0 : sb + 1;
+    int n, y0, x0;
+    tile_coords(k, n, y0, x0);
+    const int oy0 = y0 + 8 * wg;
+    const bool live = oy0 < p.H;              // this warpgroup's rows are not all below the image
+    uint8_t* out_s = outs + (WS_OUT_BUFS * wg + sb) * WS_OUT_BYTES;
+#pragma unroll
+    for (int r = 0; r < 32; ++r) acc[0][r] = 0.f;
+    mbar_wait(smem_u32(&full[st]), (uint32_t)((k / WS_STAGES) & 1));
+    if (wg == 1 || k > 0) named_bar_sync(my_turn, 2 * 128);
+    mma_issue<0, 64, 1>(acc, smem_u32(ring + (size_t)st * HALO_STAGE), smem_u32(w_s), wg);
+    if (wg == 0 || k + 1 < my_tiles) named_bar_arrive(other_turn, 2 * 128);
+    if (p.res && leader && k + 1 < my_tiles) {
+      wait_staging_free(sb_next);
+      load_res(k + 1, sb_next);
+    }
+    wgmma_wait_all_fence(acc[0]);
+    if (lane == 0) mbar_arrive(smem_u32(&empty[st]));
+    if (!live) continue;
+
+    if (p.res) {
+      mbar_wait(smem_u32(&r_full[WS_OUT_BUFS * wg + sb]), (r_phase >> sb) & 1u);
+      r_phase ^= 1u << sb;
+    } else {
+      if (leader) wait_staging_free(sb);
+      named_bar_sync(3 + wg, 128);
+    }
+    const uint32_t out_a = smem_u32(out_s);
+    const bool res = p.res != nullptr;
+    switch (p.act) {                          // once per tile: the element loop is compiled per activation
+      case TECO_ACT_RELU: ws_epilogue<TECO_ACT_RELU>(acc[0], s_bias, out_a, res, wq, lane); break;
+      case TECO_ACT_LRELU02: ws_epilogue<TECO_ACT_LRELU02>(acc[0], s_bias, out_a, res, wq, lane); break;
+      case TECO_ACT_TANH24: ws_epilogue<TECO_ACT_TANH24>(acc[0], s_bias, out_a, res, wq, lane); break;
+      case TECO_ACT_SIGMOID: ws_epilogue<TECO_ACT_SIGMOID>(acc[0], s_bias, out_a, res, wq, lane); break;
+      default: ws_epilogue<TECO_ACT_NONE>(acc[0], s_bias, out_a, res, wq, lane); break;
+    }
+    fence_async_smem();                       // the staging writes -> visible to the TMA store
+    named_bar_sync(3 + wg, 128);
+    if (leader) {
+      tma_store_4d(&ymap, smem_u32(out_s), n0, x0, oy0, n);
+      bulk_commit();
+      last_store = sb;
+    }
+  }
+  if (leader) bulk_wait_all();
+}
+
 // ------------------------------------------------------------------ weight packing
 // out[blk][tap][cout_pad][64] bf16 in the SWIZZLE_128B image (16-byte chunk j of row r stored at chunk j ^ (r & 7))
 //   <- w[3,3,cin,cout] (or [3,3,cout,cin] when transpose_layout); packed input channel k reads cin_perm[k] (-1 = zero).
@@ -361,8 +555,10 @@ PFN_encodeTiled get_encode() {
   return fn;
 }
 
-// NHWC bf16 activations [N,H,W,C] as a 4-D map whose box is one tile's halo of 64 channels (SWIZZLE_128B, zero fill)
-int encode_halo_map(CUtensorMap* map, const void* x, int N, int H, int W, int C, const char* who) {
+// NHWC bf16 activations [N,H,W,C] as a 4-D map whose box is box_h rows x box_w pixels x 64 channels (SWIZZLE_128B, zero
+// fill): by default one tile's halo
+int encode_halo_map(CUtensorMap* map, const void* x, int N, int H, int W, int C, const char* who, int box_w = HALO_COLS,
+                    int box_h = HALO_ROWS) {
   PFN_encodeTiled enc = get_encode();
   if (!enc) {
     teco_set_error("%s: cuTensorMapEncodeTiled is unavailable (no CUDA driver?)", who);
@@ -370,7 +566,7 @@ int encode_halo_map(CUtensorMap* map, const void* x, int N, int H, int W, int C,
   }
   const cuuint64_t gdim[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)N};
   const cuuint64_t gstr[3] = {(cuuint64_t)C * 2, (cuuint64_t)W * C * 2, (cuuint64_t)H * W * C * 2};
-  const cuuint32_t box[4] = {(cuuint32_t)CB, (cuuint32_t)HALO_COLS, (cuuint32_t)HALO_ROWS, 1};
+  const cuuint32_t box[4] = {(cuuint32_t)CB, (cuuint32_t)box_w, (cuuint32_t)box_h, 1};
   const cuuint32_t estr[4] = {1, 1, 1, 1};
   const CUresult cr = enc(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(x), gdim, gstr, box, estr,
                           CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
@@ -393,7 +589,7 @@ KernelT pick_kernel(int mode, int nt) {
 
 // CTAs of `kern` resident per SM at `smem` bytes of dynamic shared memory; the opt-in shared-memory attribute is set on
 // first use and the answer cached per (kernel, size), so a launch costs no extra driver calls.
-int resident_ctas(const void* kern, size_t smem, int* per_sm) {
+int resident_ctas(const void* kern, size_t smem, int* per_sm, int threads = NUM_THREADS) {
   struct Entry { const void* kern; size_t smem; int per_sm; };
   static Entry cache[32];
   static int used = 0;
@@ -403,7 +599,7 @@ int resident_ctas(const void* kern, size_t smem, int* per_sm) {
   for (int i = 0; i < used; ++i) attr_set |= cache[i].kern == kern;
   if (!attr_set) TECO_CUDA_CALL(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_MAX));
   int n = 0;
-  TECO_CUDA_CALL(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, kern, NUM_THREADS, smem));
+  TECO_CUDA_CALL(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, kern, threads, smem));
   if (n < 1) n = 1;
   if (used < 32) cache[used++] = {kern, smem, n};
   *per_sm = n;
@@ -437,8 +633,26 @@ int launch_conv3x3(const teco_tc_desc* d, const void* x, const void* wpk, const 
   CUtensorMap tmap;
   const int rc = encode_halo_map(&tmap, x, d->N, d->H, d->W, d->Cin, "teco_conv3x3_tc");
   if (rc != TECO_OK) return rc;
-  const KernelT kern = pick_kernel(d->mode, nt);
   int per_sm = 0;
+  if (d->mode == 0 && nt == 64 && p.nblk == 1 && !out_f32) {
+    // output and residual: one warpgroup's box of 8 rows x 8 pixels x 64 channels
+    CUtensorMap ymap, rmap;
+    int rc_map = encode_halo_map(&ymap, y, d->N, d->H, d->W, d->Cout, "teco_conv3x3_tc", TILE_COLS, TILE_ROWS / 2);
+    if (rc_map != TECO_OK) return rc_map;
+    rmap = ymap;
+    if (res && res != y) {
+      rc_map = encode_halo_map(&rmap, res, d->N, d->H, d->W, d->Cout, "teco_conv3x3_tc", TILE_COLS, TILE_ROWS / 2);
+      if (rc_map != TECO_OK) return rc_map;
+    }
+    const int rc_occ = resident_ctas((const void*)conv3x3_ws_kernel, WS_SMEM, &per_sm, WS_THREADS);
+    if (rc_occ != TECO_OK) return rc_occ;
+    const long long slots = ((long long)per_sm * teco_sm_count() + nsplit - 1) / nsplit;
+    const unsigned gx = (unsigned)(tiles < slots ? tiles : slots);
+    conv3x3_ws_kernel<<<dim3(gx, (unsigned)nsplit), WS_THREADS, WS_SMEM, stream>>>(tmap, ymap, rmap, p);
+    TECO_CUDA_LAUNCH_CHECK("teco_conv3x3_tc");
+    return TECO_OK;
+  }
+  const KernelT kern = pick_kernel(d->mode, nt);
   const int rc_occ = resident_ctas((const void*)kern, smem, &per_sm);
   if (rc_occ != TECO_OK) return rc_occ;
   // persistent: as many CTAs as are resident at once, spread over the Cout splits

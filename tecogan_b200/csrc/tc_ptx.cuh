@@ -47,6 +47,29 @@ __device__ __forceinline__ void bulk_load_1d(uint32_t dst, const void* src, uint
                "l"(src), "r"(bytes), "r"(bar)
                : "memory");
 }
+__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
+}
+// shared -> global tensor store (out-of-bounds elements of the box are not written), tracked by bulk async-groups
+__device__ __forceinline__ void tma_store_4d(const CUtensorMap* map, uint32_t src, int c0, int c1, int c2, int c3) {
+  asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
+               ::"l"(map), "r"(src), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// all but the newest N of this thread's committed bulk stores have finished reading shared memory (their sources may
+// be overwritten)
+template <int N>
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+// ... and have completed their global writes
+__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+// named barriers 1..15: `count` threads (a multiple of 32) take part; arrive does not wait
+__device__ __forceinline__ void named_bar_sync(int id, int count) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
+__device__ __forceinline__ void named_bar_arrive(int id, int count) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
 
 // wgmma shared-memory matrix descriptor (sm_90): [0,14) start >> 4, [16,30) LBO >> 4, [32,46) SBO >> 4,
 // [62,64) layout type (1 = SWIZZLE_128B); the base-offset field [49,52) is left 0.  The convolution kernels start A operands
@@ -64,6 +87,13 @@ __device__ __forceinline__ uint64_t gmma_desc_sw128(uint32_t saddr, uint32_t lbo
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// wgmma_wait_all() for a register array the compiler must not move across the wait (the asm names it as read and written)
+template <int R>
+__device__ __forceinline__ void wgmma_wait_all_fence(float (&d)[R]) {
+  wgmma_wait_all();
+#pragma unroll
+  for (int r = 0; r < R; ++r) asm volatile("" : "+f"(d[r])::"memory");
+}
 
 // D[64 x N] (+)= A[64 x 16] * B[16 x N], bf16 operands from shared memory, fp32 accumulators in registers (N / 2 per
 // thread).  TA / TB = 1: the operand is MN-major in shared memory.
