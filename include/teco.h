@@ -240,6 +240,27 @@ int teco_metrics_psnr_y_u8(const uint8_t* tgt, int32_t tH, int32_t tW, const uin
 int teco_metrics_ssim_y_u8(const uint8_t* tgt, int32_t tH, int32_t tW, const uint8_t* out, int32_t oH, int32_t oW,
                            int32_t N, int32_t y0, int32_t x0, int32_t h, int32_t w, double* acc, void* stream);
 
+/* ---------------------------------------------------------------------------------------
+ * LPIPS-AlexNet v0.1 and tLP100 (reference metrics.py:183-202, LPIPSmodels/).  The five convolutions of
+ * torchvision alexnet().features[0:12] run through teco_conv2d_f32 with TECO_ACT_RELU; these three entry points
+ * are the rest of the network and the distance.  All fp32 except the head's float64 accumulation.
+ * ------------------------------------------------------------------------------------- */
+/* util.py:142-144 im2tensor + networks_basic.py:131-132 scaling layer, bit for bit: uint8 RGB [N,H,W,3] read
+ * through the window (y0,x0,h,w) -> x [N,h,w,3] fp32 = (float32(u8/127.5 - 1) - shift[c]) / scale[c] with the
+ * first part in float64, shift = (-.030,-.088,-.188), scale = (.458,.448,.450). */
+int teco_lpips_input_u8(const uint8_t* img, int32_t N, int32_t H, int32_t W, int32_t y0, int32_t x0, int32_t h,
+                        int32_t w, float* x, void* stream);
+/* torch MaxPool2d(3, stride 2), no padding, floor (alexnet().features[2] and [5], pretrained_networks.py:67-76):
+ * x [N,H,W,C] -> y [N,(H-3)/2+1,(W-3)/2+1,C].  H or W below 3 -> TECO_E_INVALID. */
+int teco_maxpool3s2_f32(const float* x, float* y, int32_t N, int32_t H, int32_t W, int32_t C, void* stream);
+/* PNetLin head of one layer (networks_basic.py:150-177, util.py:72-75).  For pair p, with a = fa[ia_host[p]] and
+ * b = fb[ib_host[p]] (feature maps [Na|Nb,H,W,C]) and f^ = f / (sqrt(sum_c f^2) + 1e-10):
+ *   out[p] += mean over the H*W pixels of sum_c lin[c] * (a^ - b^)^2     (float64 accumulation, double out[P])
+ * ia_host / ib_host: HOST arrays of P frame indices, 1 <= P <= 256; C <= 384. */
+int teco_lpips_head_f32(const float* fa, int32_t Na, const float* fb, int32_t Nb, const int32_t* ia_host,
+                        const int32_t* ib_host, int32_t P, int32_t H, int32_t W, int32_t C, const float* lin, double* out,
+                        void* stream);
+
 #ifdef __cplusplus
 }
 #endif

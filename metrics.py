@@ -1,12 +1,15 @@
 #!/usr/bin/env python
-"""Mirror of the reference's metrics.py command line (flags --output / --results / --targets, metrics.py:9-12) for the two
-metrics that are image arithmetic: PSNR and SSIM on the Y channel, computed on the GPU by tecogan_b200/metrics.py
-(teco_metrics_psnr_y_u8 / teco_metrics_ssim_y_u8).  Same frame selection (cutfr = 2, metrics.py:117,131), same cut of the
-result to the target size (:134-135), same crop_8x8 (:171-172), same per-frame / per-folder / total printout and
-metrics.csv layout (:205-242) restricted to keys = ["PSNR", "SSIM"].
-LPIPS / tLP (AlexNet weights) and tOF (cv2 Farneback on the CPU) are not part of this path: DESIGN.md section 6.
+"""Mirror of the reference's metrics.py command line (flags --output / --results / --targets, metrics.py:9-12), computed on
+the GPU: PSNR and SSIM on the Y channel (tecogan_b200/metrics.py: teco_metrics_psnr_y_u8 / teco_metrics_ssim_y_u8) and,
+with --lpips_alexnet and --lpips_lin, LPIPS and tLP100 (tecogan_b200/lpips.py: AlexNet and the LPIPS v0.1 head in CUDA).
+Same frame selection (cutfr = 2, metrics.py:117,131), same cut of the result to the target size (:134-135), same crop_8x8
+(:171-172), same per-frame / per-folder / total printout and metrics.csv layout (:205-242) restricted to
+keys = ["PSNR", "SSIM"], or ["PSNR", "SSIM", "LPIPS", "tLP100"] with the two LPIPS flags (the reference's order without
+tOF).  Each PNG is decoded and run through AlexNet once; tLP100 reuses the previous frame's features.
+tOF (cv2 Farneback on the CPU) is not part of this path: DESIGN.md section 6.
 
-  python metrics.py --output results/metric_log/ --results results/calendar --targets HR/calendar
+  python metrics.py --output results/metric_log/ --results results/calendar --targets HR/calendar \
+      [--lpips_alexnet ~/.cache/torch/hub/checkpoints/alexnet-owt-7be5be79.pth --lpips_lin LPIPSmodels/v0.1/alex.pth]
 """
 import argparse
 import os
@@ -18,6 +21,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
 
 KEYS = ["PSNR", "SSIM"]
+KEYS_LPIPS = ["PSNR", "SSIM", "LPIPS", "tLP100"]
 CUTFR = 2
 
 
@@ -37,22 +41,34 @@ def read_rgb(path):
         return np.ascontiguousarray(np.asarray(Image.open(path).convert("RGB")))
 
 
-def evaluate_folder(result_dir, target_dir, log=print):
-    """Per-frame PSNR / SSIM lists of one scene (frames cutfr .. n-cutfr-1), frames grouped by size into batched launches."""
+def evaluate_folder(result_dir, target_dir, log=print, lpips=None):
+    """Per-frame lists of one scene (frames cutfr .. n-cutfr-1): PSNR / SSIM, and LPIPS / tLP100 when `lpips` (a
+    tecogan_b200.lpips.LPIPS model) is given.  The previous frame's target and result features are kept for tLP100."""
     import torch
     from tecogan_b200 import metrics as M
     result, target = listPNGinDir(result_dir), listPNGinDir(target_dir)
-    lists = {k: [] for k in KEYS}
+    lists = {k: [] for k in (KEYS if lpips is None else KEYS_LPIPS)}
+    prev = None
     for i in range(CUTFR, len(target) - CUTFR):
         out, tar = read_rgb(result[i]), read_rgb(target[i])
         msg = "frame %d, tar %s, out %s, " % (i, str(tar.shape), str(out.shape))
         t, o = torch.from_numpy(tar).cuda(), torch.from_numpy(out).cuda()
         ps, ss = M.frame_metrics(t, o)            # window = crop_8x8 of the common area; no cropped copies
-        y, x, _, _ = M.crop_window(min(tar.shape[0], out.shape[0]), min(tar.shape[1], out.shape[1]))
+        win = M.crop_window(min(tar.shape[0], out.shape[0]), min(tar.shape[1], out.shape[1]))
         lists["PSNR"].append(ps[0])
         lists["SSIM"].append(ss[0])
         log(result[i])
-        log(msg + "psnr %02.2f, ssim %02.2f, crop (%d, %d)" % (ps[0], ss[0], y, x))
+        msg += "psnr %02.2f, ssim %02.2f" % (ps[0], ss[0])
+        if lpips is not None:                     # metrics.py:183-202
+            feats = lpips.features([t, o], win)   # target at 0, result at 1
+            lists["LPIPS"].append(lpips.distances(feats, feats, [(0, 1)])[0])
+            msg += ", lpips %02.2f" % lists["LPIPS"][-1]
+            if prev is not None:
+                d_tar, d_out = lpips.distances(prev, feats, [(0, 0), (1, 1)])
+                lists["tLP100"].append(100.0 * abs(d_tar - d_out))
+                msg += ", tLPx100 %02.2f" % lists["tLP100"][-1]
+            prev = feats
+        log(msg + ", crop (%d, %d)" % win[:2])
     return lists
 
 
@@ -61,7 +77,16 @@ def main(argv=None):
     ap.add_argument("--output", required=True, help="the path of output directory")
     ap.add_argument("--results", required=True, help="the list of paths of result directory")
     ap.add_argument("--targets", required=True, help="the list of paths of target directory")
+    ap.add_argument("--lpips_alexnet", default=None,
+                    help="torchvision ImageNet AlexNet state dict (alexnet-owt-*.pth); with --lpips_lin adds LPIPS and tLP100")
+    ap.add_argument("--lpips_lin", default=None, help="LPIPS v0.1 linear weights (LPIPSmodels/v0.1/alex.pth)")
     F = ap.parse_args(argv)
+    if (F.lpips_alexnet is None) != (F.lpips_lin is None):
+        ap.error("--lpips_alexnet and --lpips_lin go together: give both for LPIPS / tLP100, or neither")
+    keys, lpips = KEYS, None
+    if F.lpips_alexnet is not None:
+        from tecogan_b200.lpips import LPIPS
+        keys, lpips = KEYS_LPIPS, LPIPS(F.lpips_alexnet, F.lpips_lin)
     import pandas as pd
     os.makedirs(F.output, exist_ok=True)
     logf = open(os.path.join(F.output, "metricsfile.txt"), "a")
@@ -71,15 +96,15 @@ def main(argv=None):
         logf.write(m + "\n")
     result_list, target_list = F.results.split(','), F.targets.split(',')
     folder_n = len(result_list)
-    sum_d = {"FrameAvg_" + k: 0.0 for k in KEYS}
-    len_d = {k: 0 for k in KEYS}
-    avg_d = {"Avg_" + k: [] for k in KEYS}
-    folder_d = {"FolderAvg_" + k: 0.0 for k in KEYS}
+    sum_d = {"FrameAvg_" + k: 0.0 for k in keys}
+    len_d = {k: 0 for k in keys}
+    avg_d = {"Avg_" + k: [] for k in keys}
+    folder_d = {"FolderAvg_" + k: 0.0 for k in keys}
     csv = os.path.join(F.output, "metrics.csv")
     for fi in range(folder_n):
-        lists = evaluate_folder(result_list[fi], target_list[fi], log)
+        lists = evaluate_folder(result_list[fi], target_list[fi], log, lpips)
         pd_dict = {}
-        for k in KEYS:
+        for k in keys:
             cur = np.float32(lists[k])
             pd_dict["%s_%02d" % (k, fi)] = pd.Series(cur)
             mean = cur.sum() / cur.shape[0]
@@ -89,7 +114,7 @@ def main(argv=None):
             len_d[k] += cur.shape[0]
             folder_d["FolderAvg_" + k] += mean
         pd.DataFrame(pd_dict).to_csv(csv, mode='w' if fi == 0 else 'a')
-    for k in KEYS:
+    for k in keys:
         sum_d["FrameAvg_" + k] = pd.Series([sum_d["FrameAvg_" + k] / len_d[k]])
         folder_d["FolderAvg_" + k] = pd.Series([folder_d["FolderAvg_" + k] / folder_n])
         avg_d["Avg_" + k] = pd.Series(np.float32(avg_d["Avg_" + k]))
@@ -98,7 +123,7 @@ def main(argv=None):
         pd.DataFrame(d).to_csv(csv, mode='a')
     log("Finished.")
     logf.close()
-    return {k: float(sum_d["FrameAvg_" + k][0]) for k in KEYS}
+    return {k: float(sum_d["FrameAvg_" + k][0]) for k in keys}
 
 
 if __name__ == "__main__":

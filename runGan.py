@@ -4,8 +4,9 @@ Mirror of the reference's runGan.py launcher (run cases, reference runGan.py:1-1
 python3 runGan.py 1   # inference on LR/calendar with the flags of record (reference runGan.py:67-90)
 python3 runGan.py 3   # train TecoGAN  (reference runGan.py:107-244)
 python3 runGan.py 4   # train FRVSR    (reference runGan.py:247-296)
-python3 runGan.py 2   # PSNR / SSIM of ./results/<scene> against ./HR/<scene> on the GPU (reference runGan.py:92-105; the
-                      # LPIPS / tLP / tOF columns of the reference's metrics.py are outside the hot path, DESIGN.md section 6)
+python3 runGan.py 2   # PSNR / SSIM, and LPIPS / tLP100 when the AlexNet and LPIPS v0.1 weights are found, of ./results/<scene>
+                      # against ./HR/<scene> on the GPU (reference runGan.py:92-105; the reference's tOF column is outside
+                      # the hot path, DESIGN.md section 6)
 Case 0 (download, needs network) is outside the hot path and prints why it is not run.
 Extra arguments after the case number are appended to the main.py command line (e.g. --max_iter 100).
 '''
@@ -63,6 +64,20 @@ elif runcase == 2:
     dirstr, tarstr = './results/', './HR/'
     cmd1 = [sys.executable, os.path.join(HERE, "metrics.py"), "--output", dirstr + "metric_log/",
             "--results", ",".join(dirstr + _ for _ in testpre), "--targets", ",".join(tarstr + _ for _ in testpre)] + extra
+    # LPIPS / tLP100 need two weight files: LPIPS v0.1's linear layers where the reference keeps them, and torchvision's
+    # ImageNet AlexNet, which the reference downloads into the torch hub cache on its first metrics run.
+    lin = './LPIPSmodels/v0.1/alex.pth'
+    alex = os.environ.get("TECO_LPIPS_ALEXNET")
+    if not alex:
+        import glob
+        import torch
+        found = sorted(glob.glob(os.path.join(torch.hub.get_dir(), "checkpoints", "alexnet-owt-*.pth")))
+        alex = found[0] if found else None
+    if alex and os.path.exists(alex) and os.path.exists(lin):
+        cmd1 += ["--lpips_alexnet", alex, "--lpips_lin", lin]
+    else:
+        print("LPIPS and tLP100 are skipped: they need %s and the torchvision AlexNet weights ($TECO_LPIPS_ALEXNET, or "
+              "alexnet-owt-*.pth under torch.hub.get_dir()/checkpoints)" % lin)
     mycall(cmd1).communicate()
 elif runcase == 3:   # Train TecoGAN -- flags of record reference runGan.py:142-234
     now_str = datetime.datetime.now().strftime("%m-%d-%H")

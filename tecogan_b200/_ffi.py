@@ -78,6 +78,9 @@ SIGNATURES = {
     "teco_adam_f32": [_P, _P, _P, _P, _I64, _F, _F, _F, _F, _F, _P],
     "teco_metrics_psnr_y_u8": [_P, _I32, _I32, _P, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _P, _P],
     "teco_metrics_ssim_y_u8": [_P, _I32, _I32, _P, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _P, _P],
+    "teco_lpips_input_u8": [_P, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _P, _P],
+    "teco_maxpool3s2_f32": [_P, _P, _I32, _I32, _I32, _I32, _P],
+    "teco_lpips_head_f32": [_P, _I32, _P, _I32, _P, _P, _I32, _I32, _I32, _I32, _P, _P, _P],
 }
 _RESTYPES = {"teco_packed_weight_bytes": C.c_int64, "teco_crc32c": C.c_int64}
 
