@@ -21,8 +21,9 @@
 //
 // Persistent CTAs walk tiles c, c + G, ...; the halo (and weight) ring has two stages, so the TMA of the next 64-channel
 // block or tile is in flight while the warpgroups run the MMAs and the epilogue of the current one.  Layers with one
-// 64-channel input block and 64-channel bf16 output slices run on conv3x3_ws_kernel instead: the same MMAs and epilogue
-// arithmetic behind a producer warp, a deeper ring and TMA-staged residuals and stores.
+// 64-channel input block and 64-channel bf16 output slices (mode 0, or mode 1 without a residual) run on
+// conv3x3_ws_kernel instead: the same MMAs and epilogue arithmetic behind a producer warp, a deeper ring and TMA-staged
+// residuals and stores.
 #include <cuda.h>
 #include "teco_common.cuh"
 #include "tc_ptx.cuh"
@@ -70,19 +71,29 @@ __device__ __forceinline__ void tap_route(int t, int& ry, int& rx, int& ph) {
 }
 
 // The nine taps x four K-steps of one 64-channel block for warpgroup wg: halo stage at halo_a, the block's packed
-// weights [tap][NT][64] at w_a.  Issues and commits them; mma_block() also waits for them.
-template <int MODE, int NT, int NACC>
+// weights [tap][NT][64] at w_a.  Issues and commits them; mma_block() also waits for them.  ZERO_INIT: the first MMA
+// into each accumulator ignores its old contents (scale-d = 0) instead of the caller zeroing the registers.  Zeroing four
+// accumulators in registers made ptxas interleave the zeroing moves with the MMAs and serialise every wgmma.
+template <int MODE, int NT, int NACC, bool ZERO_INIT = false>
 __device__ __forceinline__ void mma_issue(float (&acc)[NACC][NT / 2], uint32_t halo_a, uint32_t w_a, int wg) {
   wgmma_fence();
 #pragma unroll
   for (int t = 0; t < 9; ++t) {
     int ry, rx, ph;
     tap_route<MODE>(t, ry, rx, ph);
+    bool first = true;                        // no earlier tap feeds accumulator ph
+#pragma unroll
+    for (int u = 0; u < t; ++u) {
+      int uy, ux, uph;
+      tap_route<MODE>(u, uy, ux, uph);
+      first &= uph != ph;
+    }
     const uint32_t a0 = halo_a + (uint32_t)(((8 * wg + ry) * HALO_COLS + rx) * 128);
     const uint32_t b0 = w_a + (uint32_t)t * (uint32_t)NT * 128u;
 #pragma unroll
     for (int k = 0; k < CB / 16; ++k)
-      Wgmma<NT, 0, 0>::run(acc[ph], gmma_desc_sw128(a0 + 32u * k, 16u, HALO_COLS * 128u), gmma_desc_sw128(b0 + 32u * k, 16u, 1024u), 1u);
+      Wgmma<NT, 0, 0>::run(acc[ph], gmma_desc_sw128(a0 + 32u * k, 16u, HALO_COLS * 128u), gmma_desc_sw128(b0 + 32u * k, 16u, 1024u),
+                           ZERO_INIT && first && k == 0 ? 0u : 1u);
   }
   wgmma_commit();
 }
@@ -345,56 +356,79 @@ conv3x3_chain_kernel(const __grid_constant__ CUtensorMap tmap0, const __grid_con
 //     the residual with the bf16 result and one TMA tensor store writes it out (clipped at the image edges).  In-place
 //     residuals (res == y) are safe: each box is read and written by one warpgroup of one CTA only, the load completing
 //     before the store is issued.
-constexpr int WS_STAGES = 4;
+// MODE 1 (the transposed convolution) runs the same schedule with the four phase accumulators of mma_issue<1, 64, 4>: a
+// warpgroup's 8 x 8 input pixels are a 16 x 16 pixel box of the interleaved 2H x 2W output, 32 KB, staged in one SW128
+// tile per warpgroup and written by one TMA store.  The 72 KB of resident weights, 3 halo stages and the two 32 KB boxes
+// fill 209 KB of the 227 KB; there is no residual.
 constexpr int WS_THREADS = NUM_THREADS + 32;          // two consumer warpgroups + the producer warp
-constexpr int WS_OUT_BUFS = 3;                        // staging tiles per warpgroup
-constexpr uint32_t WS_OUT_BYTES = 8 * 8 * 128;        // one warpgroup's output box: 8 rows x 8 pixels x 64 bf16
-constexpr size_t WS_SMEM = 1024 + WS_STAGES * (size_t)HALO_STAGE + LAYER_W_BYTES + 2 * WS_OUT_BUFS * WS_OUT_BYTES +
-                           (2 * WS_STAGES + 1 + 2 * WS_OUT_BUFS) * sizeof(uint64_t) + 64 * sizeof(float);
+
+template <int MODE>
+struct WsCfg {
+  static constexpr int S = MODE == 1 ? 2 : 1;                    // output pixels per input pixel, per axis
+  static constexpr int NACC = S * S;                             // phase accumulators
+  static constexpr int STAGES = MODE == 1 ? 3 : 4;               // halo ring depth
+  static constexpr int OUT_BUFS = MODE == 1 ? 1 : 3;             // staging tiles per warpgroup
+  static constexpr uint32_t OUT_BYTES = S * S * 8 * 8 * 128;     // one warpgroup's output box: 8S rows x 8S pixels x 64 bf16
+  static constexpr size_t SMEM = 1024 + STAGES * (size_t)HALO_STAGE + LAYER_W_BYTES + 2 * OUT_BUFS * (size_t)OUT_BYTES +
+                                 (2 * STAGES + 1 + 2 * OUT_BUFS) * sizeof(uint64_t) + 64 * sizeof(float);
+  static_assert(SMEM <= SMEM_MAX, "conv3x3_ws_kernel: shared memory budget");
+};
 
 // Epilogue of one warpgroup's box into its staging tile at out_a: bias -> activation -> (+ the residual already in the
-// staging tile) -> bf16, the same fp32 operations as epilogue().  The thread holds pixel (row 2 wq + i, column lane / 4)
-// of the box, channels 8 j + 2 (lane % 4) + {0, 1}: 16-byte chunk j of the pixel's 128-byte row, stored at chunk
-// j ^ (pixel & 7) = j ^ column (SWIZZLE_128B, conflict-free per instruction).
-template <int ACT>
-__device__ __forceinline__ void ws_epilogue(const float (&acc)[32], const float* s_bias, uint32_t out_a, bool res, int wq,
+// staging tile) -> bf16, the same fp32 operations as epilogue().  The thread holds input pixel (row 2 wq + i, column
+// lane / 4) of the box, channels 8 j + 2 (lane % 4) + {0, 1}; accumulator ph goes to box pixel (oy, ox) =
+// (S (2 wq + i) + ph / 2, S col + ph % 2).  Channel chunk j of that pixel's 128-byte row is stored at chunk j ^ (ox & 7)
+// (SWIZZLE_128B: the box is 8 S pixels wide, so ox & 7 is the pixel's row index within its 1024-byte atom).  A store
+// instruction is conflict-free in MODE 0; in MODE 1 its eight columns hit four chunks, two lanes per bank.
+template <int ACT, int MODE, int NACC>
+__device__ __forceinline__ void ws_epilogue(const float (&acc)[NACC][32], const float* s_bias, uint32_t out_a, bool res, int wq,
                                             int lane) {
+  constexpr int S = WsCfg<MODE>::S;
   const int col = lane >> 2;
 #pragma unroll
   for (int i = 0; i < 2; ++i) {
-    const uint32_t px = out_a + (uint32_t)(((2 * wq + i) * 8 + col) * 128 + 4 * (lane & 3));
 #pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const int c = 8 * j + 2 * (lane & 3);
-      float v0 = teco_act(acc[4 * j + 2 * i] + s_bias[c], ACT);
-      float v1 = teco_act(acc[4 * j + 2 * i + 1] + s_bias[c + 1], ACT);
-      const uint32_t e = px + (uint32_t)((j ^ col) << 4);
-      if (res) {
-        uint32_t rb;
-        asm volatile("ld.shared.b32 %0, [%1];" : "=r"(rb) : "r"(e) : "memory");
-        const float2 r = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&rb));
-        v0 += r.x;
-        v1 += r.y;
+    for (int ph = 0; ph < NACC; ++ph) {
+      const int oy = S * (2 * wq + i) + (ph >> 1), ox = S * col + (ph & 1);
+      const uint32_t px = out_a + (uint32_t)((oy * 8 * S + ox) * 128 + 4 * (lane & 3));
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const int c = 8 * j + 2 * (lane & 3);
+        float v0 = teco_act(acc[ph][4 * j + 2 * i] + s_bias[c], ACT);
+        float v1 = teco_act(acc[ph][4 * j + 2 * i + 1] + s_bias[c + 1], ACT);
+        const uint32_t e = px + (uint32_t)((j ^ (ox & 7)) << 4);
+        if (res) {
+          uint32_t rb;
+          asm volatile("ld.shared.b32 %0, [%1];" : "=r"(rb) : "r"(e) : "memory");
+          const float2 r = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&rb));
+          v0 += r.x;
+          v1 += r.y;
+        }
+        const __nv_bfloat162 o = __floats2bfloat162_rn(v0, v1);
+        asm volatile("st.shared.b32 [%0], %1;" ::"r"(e), "r"(*reinterpret_cast<const uint32_t*>(&o)) : "memory");
       }
-      const __nv_bfloat162 o = __floats2bfloat162_rn(v0, v1);
-      asm volatile("st.shared.b32 [%0], %1;" ::"r"(e), "r"(*reinterpret_cast<const uint32_t*>(&o)) : "memory");
     }
   }
 }
 
+template <int MODE>
 __global__ void __launch_bounds__(WS_THREADS, 1)
 conv3x3_ws_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ CUtensorMap ymap,
                   const __grid_constant__ CUtensorMap rmap, const TcParams p) {
+  using Cfg = WsCfg<MODE>;
+  constexpr int WS_STAGES = Cfg::STAGES, WS_OUT_BUFS = Cfg::OUT_BUFS, NACC = Cfg::NACC, S = Cfg::S;
+  constexpr uint32_t WS_OUT_BYTES = Cfg::OUT_BYTES;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint8_t* ring = smem;                                              // WS_STAGES halo stages
   uint8_t* w_s = ring + WS_STAGES * (size_t)HALO_STAGE;              // 9 taps x 64 x 64, resident
   uint8_t* outs = w_s + LAYER_W_BYTES;                               // [2][WS_OUT_BUFS] staging tiles
-  uint64_t* full = reinterpret_cast<uint64_t*>(outs + 2 * WS_OUT_BUFS * WS_OUT_BYTES);   // [WS_STAGES]
+  uint64_t* full = reinterpret_cast<uint64_t*>(outs + 2 * WS_OUT_BUFS * (size_t)WS_OUT_BYTES);   // [WS_STAGES]
   uint64_t* empty = full + WS_STAGES;                                      // [WS_STAGES]
   uint64_t* w_full = empty + WS_STAGES;
   uint64_t* r_full = w_full + 1;                                           // [2][WS_OUT_BUFS] residual arrived
   float* s_bias = reinterpret_cast<float*>(r_full + 2 * WS_OUT_BUFS);      // [64]
+  const bool has_res = MODE == 0 && p.res != nullptr;                      // the dispatch sends no mode-1 residual here
 
   const int tid = threadIdx.x, wg = tid >> 7;
   const int n0 = blockIdx.y * 64;
@@ -463,31 +497,29 @@ conv3x3_ws_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constan
     else bulk_wait_read<1>();
   };
   uint32_t r_phase = 0;                       // bit b: parity of r_full[WS_OUT_BUFS wg + b]
-  if (p.res && leader) load_res(0, 0);
+  if (has_res && leader) load_res(0, 0);
   mbar_wait(smem_u32(w_full), 0);
-  float acc[1][32];
+  float acc[NACC][32];
   for (int k = 0; k < my_tiles; ++k) {
     const int st = k % WS_STAGES, sb = k % WS_OUT_BUFS, sb_next = sb + 1 == WS_OUT_BUFS ? 0 : sb + 1;
     int n, y0, x0;
     tile_coords(k, n, y0, x0);
     const int oy0 = y0 + 8 * wg;
     const bool live = oy0 < p.H;              // this warpgroup's rows are not all below the image
-    uint8_t* out_s = outs + (WS_OUT_BUFS * wg + sb) * WS_OUT_BYTES;
-#pragma unroll
-    for (int r = 0; r < 32; ++r) acc[0][r] = 0.f;
+    uint8_t* out_s = outs + (WS_OUT_BUFS * wg + sb) * (size_t)WS_OUT_BYTES;
     mbar_wait(smem_u32(&full[st]), (uint32_t)((k / WS_STAGES) & 1));
     if (wg == 1 || k > 0) named_bar_sync(my_turn, 2 * 128);
-    mma_issue<0, 64, 1>(acc, smem_u32(ring + (size_t)st * HALO_STAGE), smem_u32(w_s), wg);
+    mma_issue<MODE, 64, NACC, true>(acc, smem_u32(ring + (size_t)st * HALO_STAGE), smem_u32(w_s), wg);
     if (wg == 0 || k + 1 < my_tiles) named_bar_arrive(other_turn, 2 * 128);
-    if (p.res && leader && k + 1 < my_tiles) {
+    if (has_res && leader && k + 1 < my_tiles) {
       wait_staging_free(sb_next);
       load_res(k + 1, sb_next);
     }
-    wgmma_wait_all_fence(acc[0]);
+    wgmma_wait_all_fence(acc);
     if (lane == 0) mbar_arrive(smem_u32(&empty[st]));
     if (!live) continue;
 
-    if (p.res) {
+    if (has_res) {
       mbar_wait(smem_u32(&r_full[WS_OUT_BUFS * wg + sb]), (r_phase >> sb) & 1u);
       r_phase ^= 1u << sb;
     } else {
@@ -495,18 +527,17 @@ conv3x3_ws_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constan
       named_bar_sync(3 + wg, 128);
     }
     const uint32_t out_a = smem_u32(out_s);
-    const bool res = p.res != nullptr;
     switch (p.act) {                          // once per tile: the element loop is compiled per activation
-      case TECO_ACT_RELU: ws_epilogue<TECO_ACT_RELU>(acc[0], s_bias, out_a, res, wq, lane); break;
-      case TECO_ACT_LRELU02: ws_epilogue<TECO_ACT_LRELU02>(acc[0], s_bias, out_a, res, wq, lane); break;
-      case TECO_ACT_TANH24: ws_epilogue<TECO_ACT_TANH24>(acc[0], s_bias, out_a, res, wq, lane); break;
-      case TECO_ACT_SIGMOID: ws_epilogue<TECO_ACT_SIGMOID>(acc[0], s_bias, out_a, res, wq, lane); break;
-      default: ws_epilogue<TECO_ACT_NONE>(acc[0], s_bias, out_a, res, wq, lane); break;
+      case TECO_ACT_RELU: ws_epilogue<TECO_ACT_RELU, MODE>(acc, s_bias, out_a, has_res, wq, lane); break;
+      case TECO_ACT_LRELU02: ws_epilogue<TECO_ACT_LRELU02, MODE>(acc, s_bias, out_a, has_res, wq, lane); break;
+      case TECO_ACT_TANH24: ws_epilogue<TECO_ACT_TANH24, MODE>(acc, s_bias, out_a, has_res, wq, lane); break;
+      case TECO_ACT_SIGMOID: ws_epilogue<TECO_ACT_SIGMOID, MODE>(acc, s_bias, out_a, has_res, wq, lane); break;
+      default: ws_epilogue<TECO_ACT_NONE, MODE>(acc, s_bias, out_a, has_res, wq, lane); break;
     }
     fence_async_smem();                       // the staging writes -> visible to the TMA store
     named_bar_sync(3 + wg, 128);
     if (leader) {
-      tma_store_4d(&ymap, smem_u32(out_s), n0, x0, oy0, n);
+      tma_store_4d(&ymap, smem_u32(out_s), n0, S * x0, S * oy0, n);
       bulk_commit();
       last_store = sb;
     }
@@ -580,6 +611,8 @@ int encode_halo_map(CUtensorMap* map, const void* x, int N, int H, int W, int C,
 
 using KernelT = void (*)(const CUtensorMap, const TcParams);
 
+// Mode 1 reaches these instances only with Cin > 64, Cout not a multiple of 64, a residual or an fp32 output; the
+// generator and the bf16 training transposed convolutions (64 -> 64, bf16, no residual) run on conv3x3_ws_kernel<1>.
 KernelT pick_kernel(int mode, int nt) {
   if (mode == 1) return nt == 32 ? conv3x3_wgmma_kernel<1, 32> : conv3x3_wgmma_kernel<1, 16>;
   if (nt == 64) return conv3x3_wgmma_kernel<0, 64>;
@@ -634,21 +667,29 @@ int launch_conv3x3(const teco_tc_desc* d, const void* x, const void* wpk, const 
   const int rc = encode_halo_map(&tmap, x, d->N, d->H, d->W, d->Cin, "teco_conv3x3_tc");
   if (rc != TECO_OK) return rc;
   int per_sm = 0;
-  if (d->mode == 0 && nt == 64 && p.nblk == 1 && !out_f32) {
-    // output and residual: one warpgroup's box of 8 rows x 8 pixels x 64 channels
+  // one K block, 64-channel bf16 output slices, and no residual in mode 1: the warp-specialised kernel
+  if (p.nblk == 1 && d->Cout % 64 == 0 && !out_f32 && (d->mode == 0 || !res)) {
+    // output and residual: one warpgroup's box of 8 rows x 8 pixels (16 x 16 of the 2H x 2W output in mode 1) x 64 channels
+    const int s = d->mode == 1 ? 2 : 1;
     CUtensorMap ymap, rmap;
-    int rc_map = encode_halo_map(&ymap, y, d->N, d->H, d->W, d->Cout, "teco_conv3x3_tc", TILE_COLS, TILE_ROWS / 2);
+    int rc_map = encode_halo_map(&ymap, y, d->N, s * d->H, s * d->W, d->Cout, "teco_conv3x3_tc", s * TILE_COLS, s * TILE_ROWS / 2);
     if (rc_map != TECO_OK) return rc_map;
     rmap = ymap;
     if (res && res != y) {
       rc_map = encode_halo_map(&rmap, res, d->N, d->H, d->W, d->Cout, "teco_conv3x3_tc", TILE_COLS, TILE_ROWS / 2);
       if (rc_map != TECO_OK) return rc_map;
     }
-    const int rc_occ = resident_ctas((const void*)conv3x3_ws_kernel, WS_SMEM, &per_sm, WS_THREADS);
+    const void* kern = d->mode == 1 ? (const void*)conv3x3_ws_kernel<1> : (const void*)conv3x3_ws_kernel<0>;
+    const size_t ws_smem = d->mode == 1 ? WsCfg<1>::SMEM : WsCfg<0>::SMEM;
+    const int rc_occ = resident_ctas(kern, ws_smem, &per_sm, WS_THREADS);
     if (rc_occ != TECO_OK) return rc_occ;
-    const long long slots = ((long long)per_sm * teco_sm_count() + nsplit - 1) / nsplit;
+    const int nsplit_ws = d->Cout / 64;
+    const long long slots = ((long long)per_sm * teco_sm_count() + nsplit_ws - 1) / nsplit_ws;
     const unsigned gx = (unsigned)(tiles < slots ? tiles : slots);
-    conv3x3_ws_kernel<<<dim3(gx, (unsigned)nsplit), WS_THREADS, WS_SMEM, stream>>>(tmap, ymap, rmap, p);
+    if (d->mode == 1)
+      conv3x3_ws_kernel<1><<<dim3(gx, (unsigned)nsplit_ws), WS_THREADS, ws_smem, stream>>>(tmap, ymap, rmap, p);
+    else
+      conv3x3_ws_kernel<0><<<dim3(gx, (unsigned)nsplit_ws), WS_THREADS, ws_smem, stream>>>(tmap, ymap, rmap, p);
     TECO_CUDA_LAUNCH_CHECK("teco_conv3x3_tc");
     return TECO_OK;
   }

@@ -94,6 +94,15 @@ __device__ __forceinline__ void wgmma_wait_all_fence(float (&d)[R]) {
 #pragma unroll
   for (int r = 0; r < R; ++r) asm volatile("" : "+f"(d[r])::"memory");
 }
+// ... for A accumulators of R registers each
+template <int A, int R>
+__device__ __forceinline__ void wgmma_wait_all_fence(float (&d)[A][R]) {
+  wgmma_wait_all();
+#pragma unroll
+  for (int a = 0; a < A; ++a)
+#pragma unroll
+    for (int r = 0; r < R; ++r) asm volatile("" : "+f"(d[a][r])::"memory");
+}
 
 // D[64 x N] (+)= A[64 x 16] * B[16 x N], bf16 operands from shared memory, fp32 accumulators in registers (N / 2 per
 // thread).  TA / TB = 1: the operand is MN-major in shared memory.
