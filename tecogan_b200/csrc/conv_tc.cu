@@ -340,72 +340,118 @@ conv3x3_chain_kernel(const __grid_constant__ CUtensorMap tmap0, const __grid_con
 
 // ------------------------------------------------------------------ warp-specialised 64 -> 64 layer (one K block)
 // Mode 0, Cin = 64, 64 output channels per CTA, bf16 output: the generator trunk, FNet's 64-channel layers and the
-// 64-input-channel training convolutions.  The CTA tile, the MMAs of each warpgroup and the epilogue arithmetic are those
-// of conv3x3_wgmma_kernel, so the results are bit-identical; what differs is the schedule:
+// 64-input-channel training convolutions.  The CTA tile (16 rows x 8 pixels), the products with their tap and K order,
+// and the epilogue arithmetic are those of conv3x3_wgmma_kernel; what differs:
+//   - the MMA operands are swapped, D[cout][pixel] = W_tap[cout][cin] X[cin][pixel] (mma_issue_tile): M = the 64 output
+//     channels, A = the resident weight tap; N = the tile's 128 pixels, B = the halo at the tap's offset.  One
+//     m64n128k16 reads 6 KB of shared-memory operands for 131072 MACs, where two m64n64k16 with the pixels as A read
+//     8 KB, and at the tensor rate those reads alone would take all of the SM's shared-memory bandwidth;
+//   - one consumer warpgroup owns a whole tile (64 accumulator registers per thread); the two take alternate tiles of the
+//     CTA's walk;
 //   - one producer warp bulk-copies the weights once and TMA-loads the halo of each tile into a WS_STAGES-deep ring; a
-//     stage is refilled once all eight consumer warps have arrived on its `empty` barrier after their MMAs completed;
-//   - the two consumer warpgroups alternate in *issuing* MMAs (named barriers 1 and 2): warpgroup 1 may issue tile k once
-//     warpgroup 0 has issued (not completed) tile k, and warpgroup 0 may issue tile k + 1 once warpgroup 1 has issued
-//     tile k.  The barriers order only the issue; the tensor pipe then runs the two issue streams one after the other,
-//     so while it works on one warpgroup's MMAs the other, its own MMAs complete, runs its epilogue.  The epilogues
-//     themselves are not ordered against each other;
+//     stage is refilled once the warps that read it have arrived on its `empty` barrier after their MMAs completed;
+//   - the two consumer warpgroups alternate in *issuing* MMAs (named barriers 1 and 2): the warpgroup of tile k + 1 may
+//     issue once the warpgroup of tile k has issued (not completed) its MMAs.  The barriers order only the issue; the
+//     tensor pipe runs the two issue streams one after the other, so while it works on one warpgroup's MMAs the other,
+//     its own MMAs complete, runs its epilogue.  The epilogues themselves are not ordered against each other;
 //   - the epilogue does not wait on global loads or stores: each warpgroup has WS_OUT_BUFS SW128 staging tiles for its
-//     box of 8 rows x 8 pixels x 64 channels, used by tiles in turn.  The residual box of tile k + 1 is TMA-loaded into
-//     the next one while the MMAs of tile k run, once the store of tile k + 1 - WS_OUT_BUFS has read it (the store of
-//     tile k - 1 may still be reading its own: shared memory is busy with MMA operands then); the epilogue overwrites
-//     the residual with the bf16 result and one TMA tensor store writes it out (clipped at the image edges).  In-place
-//     residuals (res == y) are safe: each box is read and written by one warpgroup of one CTA only, the load completing
-//     before the store is issued.
-// MODE 1 (the transposed convolution) runs the same schedule with the four phase accumulators of mma_issue<1, 64, 4>: a
-// warpgroup's 8 x 8 input pixels are a 16 x 16 pixel box of the interleaved 2H x 2W output, 32 KB, staged in one SW128
-// tile per warpgroup and written by one TMA store.  The 72 KB of resident weights, 3 halo stages and the two 32 KB boxes
-// fill 209 KB of the 227 KB; there is no residual.
+//     output box (one tile, 16 rows x 8 pixels x 64 channels), used by its tiles in turn.  The residual box of its next
+//     tile is TMA-loaded into the next staging tile while the MMAs of this one run, once the store of its previous tile
+//     has read that staging tile; the epilogue overwrites the residual with the bf16 result and one TMA tensor store
+//     writes it out (clipped at the image edges).  In-place residuals (res == y) are safe: each box is read and written
+//     by one warpgroup of one CTA only, the load completing before the store is issued.
+// MODE 1 (the transposed convolution) runs the same producer, ring, turn-taking and stores with the unswapped MMAs:
+// both warpgroups work on every tile, warpgroup g on input rows 8g .. 8g + 7 with the four phase accumulators of
+// mma_issue<1, 64, 4>.  Its 8 x 8 input pixels are a 16 x 16 pixel box of the interleaved 2H x 2W output, 32 KB, staged
+// in one SW128 tile per warpgroup and written by one TMA store; there is no residual.
 constexpr int WS_THREADS = NUM_THREADS + 32;          // two consumer warpgroups + the producer warp
 
 template <int MODE>
 struct WsCfg {
   static constexpr int S = MODE == 1 ? 2 : 1;                    // output pixels per input pixel, per axis
   static constexpr int NACC = S * S;                             // phase accumulators
-  static constexpr int STAGES = MODE == 1 ? 3 : 4;               // halo ring depth
-  static constexpr int OUT_BUFS = MODE == 1 ? 1 : 3;             // staging tiles per warpgroup
-  static constexpr uint32_t OUT_BYTES = S * S * 8 * 8 * 128;     // one warpgroup's output box: 8S rows x 8S pixels x 64 bf16
+  static constexpr int NR = MODE == 1 ? 32 : 64;                 // registers per accumulator and thread
+  static constexpr int WARPS_PER_STAGE = MODE == 1 ? 8 : 4;      // consumer warps that read each halo stage
+  static constexpr int STAGES = 3;                               // halo ring depth
+  static constexpr int OUT_BUFS = MODE == 1 ? 1 : 2;             // staging tiles per warpgroup
+  static constexpr int BOX_ROWS = TILE_ROWS, BOX_COLS = S * TILE_COLS;   // one warpgroup's output box
+  static constexpr uint32_t OUT_BYTES = BOX_ROWS * BOX_COLS * 128;
   static constexpr size_t SMEM = 1024 + STAGES * (size_t)HALO_STAGE + LAYER_W_BYTES + 2 * OUT_BUFS * (size_t)OUT_BYTES +
                                  (2 * STAGES + 1 + 2 * OUT_BUFS) * sizeof(uint64_t) + 64 * sizeof(float);
   static_assert(SMEM <= SMEM_MAX, "conv3x3_ws_kernel: shared memory budget");
 };
 
+// MODE 0, one warpgroup per tile: the nine taps x four K-steps of mma_issue<0, …> with the operands swapped, A = weight
+// tap t ([64 cout][64 cin], SBO = 8 rows of 128 B), B = the halo from (ky, kx) (8-pixel groups one halo row apart).  The
+// first MMA runs with scale-d = 0.  Issues and commits them.
+__device__ __forceinline__ void mma_issue_tile(float (&acc)[64], uint32_t halo_a, uint32_t w_a) {
+  wgmma_fence();
+#pragma unroll
+  for (int t = 0; t < 9; ++t) {
+    const uint32_t a0 = w_a + (uint32_t)t * 64u * 128u;
+    const uint32_t b0 = halo_a + (uint32_t)(((t / 3) * HALO_COLS + t % 3) * 128);
+#pragma unroll
+    for (int k = 0; k < CB / 16; ++k)
+      Wgmma<128, 0, 0>::run(acc, gmma_desc_sw128(a0 + 32u * k, 16u, 1024u), gmma_desc_sw128(b0 + 32u * k, 16u, HALO_COLS * 128u),
+                            t == 0 && k == 0 ? 0u : 1u);
+  }
+  wgmma_commit();
+}
+
 // Epilogue of one warpgroup's box into its staging tile at out_a: bias -> activation -> (+ the residual already in the
-// staging tile) -> bf16, the same fp32 operations as epilogue().  The thread holds input pixel (row 2 wq + i, column
-// lane / 4) of the box, channels 8 j + 2 (lane % 4) + {0, 1}; accumulator ph goes to box pixel (oy, ox) =
-// (S (2 wq + i) + ph / 2, S col + ph % 2).  Channel chunk j of that pixel's 128-byte row is stored at chunk j ^ (ox & 7)
-// (SWIZZLE_128B: the box is 8 S pixels wide, so ox & 7 is the pixel's row index within its 1024-byte atom).  A store
-// instruction is conflict-free in MODE 0; in MODE 1 its eight columns hit four chunks, two lanes per bank.
-template <int ACT, int MODE, int NACC>
-__device__ __forceinline__ void ws_epilogue(const float (&acc)[NACC][32], const float* s_bias, uint32_t out_a, bool res, int wq,
-                                            int lane) {
-  constexpr int S = WsCfg<MODE>::S;
-  const int col = lane >> 2;
+// staging tile) -> bf16, the same fp32 operations as epilogue().  The box's pixel p (row p / 8 S, column p % 8 S) is the
+// 128-byte row p of the tile; channel chunk q of it is stored at chunk q ^ (p & 7) (SWIZZLE_128B: the box is 8 S pixels
+// wide, so p & 7 is the column's row index within its 1024-byte atom).
+//   MODE 0: the thread holds channels 16 wq + lane / 4 + 8 i (bias b[i]) of pixels 8 j + 2 (lane % 4) + {0, 1}, i.e. of
+//     tile row j.  Matrix (j, i), pixels 8 j .. 8 j + 7 by chunk 2 wq + i, is one 8 x 8 matrix of the transposed
+//     ldmatrix / stmatrix; one x4 moves rows j, j + 1 of both chunks, each matrix conflict-free.
+//   MODE 1: the thread holds input pixel (row 2 wq + i, column lane / 4) of the box, channels 8 j + 2 (lane % 4) + {0, 1};
+//     accumulator ph goes to box pixel (S (2 wq + i) + ph / 2, S col + ph % 2).  A 4-byte store instruction's eight
+//     columns hit four chunks, two lanes per bank.  There is no residual.
+template <int ACT, int MODE, int NACC, int NR>
+__device__ __forceinline__ void ws_epilogue(const float (&acc)[NACC][NR], const float* s_bias, const float (&b)[2],
+                                            uint32_t out_a, bool res, int wq, int lane) {
+  if constexpr (MODE == 0) {
+    const int q = 2 * wq + ((lane >> 3) & 1);                        // lane supplies row lane % 8 of matrix lane / 8
+    const uint32_t row_a = out_a + (uint32_t)((8 * (lane >> 4) + (lane & 7)) * 128 + ((q ^ (lane & 7)) << 4));
 #pragma unroll
-  for (int i = 0; i < 2; ++i) {
+    for (int jj = 0; jj < TILE_ROWS / 2; ++jj) {
+      const uint32_t a = row_a + (uint32_t)jj * 2u * TILE_COLS * 128u;
+      uint32_t r[4];
+      if (res) ldmatrix_x4_trans(r, a);
 #pragma unroll
-    for (int ph = 0; ph < NACC; ++ph) {
-      const int oy = S * (2 * wq + i) + (ph >> 1), ox = S * col + (ph & 1);
-      const uint32_t px = out_a + (uint32_t)((oy * 8 * S + ox) * 128 + 4 * (lane & 3));
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const int c = 8 * j + 2 * (lane & 3);
-        float v0 = teco_act(acc[ph][4 * j + 2 * i] + s_bias[c], ACT);
-        float v1 = teco_act(acc[ph][4 * j + 2 * i + 1] + s_bias[c + 1], ACT);
-        const uint32_t e = px + (uint32_t)((j ^ (ox & 7)) << 4);
+      for (int m = 0; m < 4; ++m) {                                  // matrix m = (row 2 jj + m / 2, chunk 2 wq + m % 2)
+        const int j = 2 * jj + (m >> 1), i = m & 1;
+        float v0 = teco_act(acc[0][4 * j + 2 * i] + b[i], ACT);
+        float v1 = teco_act(acc[0][4 * j + 2 * i + 1] + b[i], ACT);
         if (res) {
-          uint32_t rb;
-          asm volatile("ld.shared.b32 %0, [%1];" : "=r"(rb) : "r"(e) : "memory");
-          const float2 r = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&rb));
-          v0 += r.x;
-          v1 += r.y;
+          const float2 rf = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&r[m]));
+          v0 += rf.x;
+          v1 += rf.y;
         }
         const __nv_bfloat162 o = __floats2bfloat162_rn(v0, v1);
-        asm volatile("st.shared.b32 [%0], %1;" ::"r"(e), "r"(*reinterpret_cast<const uint32_t*>(&o)) : "memory");
+        r[m] = *reinterpret_cast<const uint32_t*>(&o);
+      }
+      stmatrix_x4_trans(a, r);
+    }
+  } else {
+    constexpr int S = WsCfg<MODE>::S;
+    const int col = lane >> 2;
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+#pragma unroll
+      for (int ph = 0; ph < NACC; ++ph) {
+        const int oy = S * (2 * wq + i) + (ph >> 1), ox = S * col + (ph & 1);
+        const uint32_t px = out_a + (uint32_t)((oy * 8 * S + ox) * 128 + 4 * (lane & 3));
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const int c = 8 * j + 2 * (lane & 3);
+          const float v0 = teco_act(acc[ph][4 * j + 2 * i] + s_bias[c], ACT);
+          const float v1 = teco_act(acc[ph][4 * j + 2 * i + 1] + s_bias[c + 1], ACT);
+          const __nv_bfloat162 o = __floats2bfloat162_rn(v0, v1);
+          const uint32_t e = px + (uint32_t)((j ^ (ox & 7)) << 4);
+          asm volatile("st.shared.b32 [%0], %1;" ::"r"(e), "r"(*reinterpret_cast<const uint32_t*>(&o)) : "memory");
+        }
       }
     }
   }
@@ -439,7 +485,7 @@ conv3x3_ws_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constan
   if (tid == 0) {
     for (int s = 0; s < WS_STAGES; ++s) {
       mbar_init(smem_u32(&full[s]), 1);
-      mbar_init(smem_u32(&empty[s]), 8);     // one arrival per consumer warp
+      mbar_init(smem_u32(&empty[s]), Cfg::WARPS_PER_STAGE);   // one arrival per consumer warp reading the stage
     }
     for (int i = 0; i < 1 + 2 * WS_OUT_BUFS; ++i) mbar_init(smem_u32(&w_full[i]), 1);   // w_full, r_full[]
     fence_mbar_init();
@@ -476,70 +522,68 @@ conv3x3_ws_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constan
     return;
   }
 
-  // consumer warpgroup wg: rows 8 wg .. 8 wg + 7 of every tile
+  // consumer warpgroup wg.  MODE 0: tiles wg, wg + 2, ... of the walk, whole.  MODE 1: rows 8 wg .. 8 wg + 7 of every
+  // tile.  The MMAs are issued in turns over both warpgroups: MODE 0 issues tile k in turn k, MODE 1 warpgroup g's part
+  // of tile k in turn 2 k + g.
   const int wq = (tid >> 5) & 3, lane = tid & 31;
   const bool leader = (tid & 127) == 0;       // issues this warpgroup's residual loads and output stores
   const int my_turn = 1 + wg, other_turn = 2 - wg;   // named barrier 1 + g: warpgroup g may issue its MMAs
-  // staging tile b of this warpgroup <- the residual box of tile k, unless its rows are all below the image
-  auto load_res = [&](int k, int b) {
+  const int k_first = MODE == 0 ? wg : 0, k_step = MODE == 0 ? 2 : 1, turns = MODE == 0 ? my_tiles : 2 * my_tiles;
+  auto load_res = [&](int k, int b) {         // staging tile b of this warpgroup <- the residual box of tile k
     int n, y0, x0;
     tile_coords(k, n, y0, x0);
-    if (y0 + 8 * wg >= p.H) return;
     const uint32_t bar = smem_u32(&r_full[WS_OUT_BUFS * wg + b]);
     mbar_expect_tx(bar, WS_OUT_BYTES);
-    tma_load_4d(smem_u32(outs + (WS_OUT_BUFS * wg + b) * WS_OUT_BYTES), &rmap, bar, n0, x0, y0 + 8 * wg, n);
+    tma_load_4d(smem_u32(outs + (WS_OUT_BUFS * wg + b) * WS_OUT_BYTES), &rmap, bar, n0, x0, y0, n);
   };
-  // leader: before staging tile b is rewritten, every store from it has read it: all but the newest store, or all of
-  // them if the newest is from b
-  int last_store = -1;
-  auto wait_staging_free = [&](int b) {
-    if (last_store == b) bulk_wait_read<0>();
-    else bulk_wait_read<1>();
-  };
+  const float bias_r[2] = {s_bias[16 * wq + (lane >> 2)], s_bias[16 * wq + 8 + (lane >> 2)]};   // MODE 0's channels
   uint32_t r_phase = 0;                       // bit b: parity of r_full[WS_OUT_BUFS wg + b]
-  if (has_res && leader) load_res(0, 0);
+  if (has_res && leader && k_first < my_tiles) load_res(k_first, 0);
   mbar_wait(smem_u32(w_full), 0);
-  float acc[NACC][32];
-  for (int k = 0; k < my_tiles; ++k) {
-    const int st = k % WS_STAGES, sb = k % WS_OUT_BUFS, sb_next = sb + 1 == WS_OUT_BUFS ? 0 : sb + 1;
+  float acc[NACC][Cfg::NR];
+  for (int k = k_first, m = 0; k < my_tiles; k += k_step, ++m) {
+    const int st = k % WS_STAGES, sb = m % WS_OUT_BUFS, sb_next = sb + 1 == WS_OUT_BUFS ? 0 : sb + 1;
+    const int turn = MODE == 0 ? k : 2 * k + wg;
     int n, y0, x0;
     tile_coords(k, n, y0, x0);
-    const int oy0 = y0 + 8 * wg;
-    const bool live = oy0 < p.H;              // this warpgroup's rows are not all below the image
+    const int oy0 = MODE == 0 ? y0 : y0 + 8 * wg;   // first input row of this warpgroup's box
     uint8_t* out_s = outs + (WS_OUT_BUFS * wg + sb) * (size_t)WS_OUT_BYTES;
     mbar_wait(smem_u32(&full[st]), (uint32_t)((k / WS_STAGES) & 1));
-    if (wg == 1 || k > 0) named_bar_sync(my_turn, 2 * 128);
-    mma_issue<MODE, 64, NACC, true>(acc, smem_u32(ring + (size_t)st * HALO_STAGE), smem_u32(w_s), wg);
-    if (wg == 0 || k + 1 < my_tiles) named_bar_arrive(other_turn, 2 * 128);
-    if (has_res && leader && k + 1 < my_tiles) {
-      wait_staging_free(sb_next);
-      load_res(k + 1, sb_next);
+    if (turn > 0) named_bar_sync(my_turn, 2 * 128);
+    const uint32_t halo_a = smem_u32(ring + (size_t)st * HALO_STAGE);
+    if constexpr (MODE == 0) mma_issue_tile(acc[0], halo_a, smem_u32(w_s));
+    else mma_issue<MODE, 64, NACC, true>(acc, halo_a, smem_u32(w_s), wg);
+    if (turn + 1 < turns) named_bar_arrive(other_turn, 2 * 128);
+    if (has_res && leader && k + k_step < my_tiles) {
+      // staging tile sb_next was last used by this warpgroup's tile m + 1 - WS_OUT_BUFS; all of its later stores may still
+      // be reading their own
+      bulk_wait_read<(WS_OUT_BUFS >= 2 ? WS_OUT_BUFS - 2 : 0)>();
+      load_res(k + k_step, sb_next);
     }
     wgmma_wait_all_fence(acc);
     if (lane == 0) mbar_arrive(smem_u32(&empty[st]));
-    if (!live) continue;
+    if (MODE == 1 && oy0 >= p.H) continue;    // MODE 1: this warpgroup's rows are all below the image
 
     if (has_res) {
       mbar_wait(smem_u32(&r_full[WS_OUT_BUFS * wg + sb]), (r_phase >> sb) & 1u);
       r_phase ^= 1u << sb;
     } else {
-      if (leader) wait_staging_free(sb);
+      if (leader) bulk_wait_read<WS_OUT_BUFS - 1>();   // the store that last used staging tile sb has read it
       named_bar_sync(3 + wg, 128);
     }
     const uint32_t out_a = smem_u32(out_s);
     switch (p.act) {                          // once per tile: the element loop is compiled per activation
-      case TECO_ACT_RELU: ws_epilogue<TECO_ACT_RELU, MODE>(acc, s_bias, out_a, has_res, wq, lane); break;
-      case TECO_ACT_LRELU02: ws_epilogue<TECO_ACT_LRELU02, MODE>(acc, s_bias, out_a, has_res, wq, lane); break;
-      case TECO_ACT_TANH24: ws_epilogue<TECO_ACT_TANH24, MODE>(acc, s_bias, out_a, has_res, wq, lane); break;
-      case TECO_ACT_SIGMOID: ws_epilogue<TECO_ACT_SIGMOID, MODE>(acc, s_bias, out_a, has_res, wq, lane); break;
-      default: ws_epilogue<TECO_ACT_NONE, MODE>(acc, s_bias, out_a, has_res, wq, lane); break;
+      case TECO_ACT_RELU: ws_epilogue<TECO_ACT_RELU, MODE>(acc, s_bias, bias_r, out_a, has_res, wq, lane); break;
+      case TECO_ACT_LRELU02: ws_epilogue<TECO_ACT_LRELU02, MODE>(acc, s_bias, bias_r, out_a, has_res, wq, lane); break;
+      case TECO_ACT_TANH24: ws_epilogue<TECO_ACT_TANH24, MODE>(acc, s_bias, bias_r, out_a, has_res, wq, lane); break;
+      case TECO_ACT_SIGMOID: ws_epilogue<TECO_ACT_SIGMOID, MODE>(acc, s_bias, bias_r, out_a, has_res, wq, lane); break;
+      default: ws_epilogue<TECO_ACT_NONE, MODE>(acc, s_bias, bias_r, out_a, has_res, wq, lane); break;
     }
     fence_async_smem();                       // the staging writes -> visible to the TMA store
     named_bar_sync(3 + wg, 128);
     if (leader) {
-      tma_store_4d(&ymap, smem_u32(out_s), n0, S * x0, S * oy0, n);
+      tma_store_4d(&ymap, out_a, n0, S * x0, S * oy0, n);
       bulk_commit();
-      last_store = sb;
     }
   }
   if (leader) bulk_wait_all();
@@ -669,14 +713,15 @@ int launch_conv3x3(const teco_tc_desc* d, const void* x, const void* wpk, const 
   int per_sm = 0;
   // one K block, 64-channel bf16 output slices, and no residual in mode 1: the warp-specialised kernel
   if (p.nblk == 1 && d->Cout % 64 == 0 && !out_f32 && (d->mode == 0 || !res)) {
-    // output and residual: one warpgroup's box of 8 rows x 8 pixels (16 x 16 of the 2H x 2W output in mode 1) x 64 channels
+    // output and residual: one warpgroup's box of 16 rows x 8 pixels (a whole tile; 16 x 16 of the 2H x 2W output in
+    // mode 1) x 64 channels
     const int s = d->mode == 1 ? 2 : 1;
     CUtensorMap ymap, rmap;
-    int rc_map = encode_halo_map(&ymap, y, d->N, s * d->H, s * d->W, d->Cout, "teco_conv3x3_tc", s * TILE_COLS, s * TILE_ROWS / 2);
+    int rc_map = encode_halo_map(&ymap, y, d->N, s * d->H, s * d->W, d->Cout, "teco_conv3x3_tc", s * TILE_COLS, TILE_ROWS);
     if (rc_map != TECO_OK) return rc_map;
     rmap = ymap;
     if (res && res != y) {
-      rc_map = encode_halo_map(&rmap, res, d->N, d->H, d->W, d->Cout, "teco_conv3x3_tc", TILE_COLS, TILE_ROWS / 2);
+      rc_map = encode_halo_map(&rmap, res, d->N, d->H, d->W, d->Cout, "teco_conv3x3_tc", TILE_COLS, TILE_ROWS);
       if (rc_map != TECO_OK) return rc_map;
     }
     const void* kern = d->mode == 1 ? (const void*)conv3x3_ws_kernel<1> : (const void*)conv3x3_ws_kernel<0>;

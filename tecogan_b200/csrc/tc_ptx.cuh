@@ -72,9 +72,9 @@ __device__ __forceinline__ void named_bar_arrive(int id, int count) {
 }
 
 // wgmma shared-memory matrix descriptor (sm_90): [0,14) start >> 4, [16,30) LBO >> 4, [32,46) SBO >> 4,
-// [62,64) layout type (1 = SWIZZLE_128B); the base-offset field [49,52) is left 0.  The convolution kernels start A operands
-// at 128-byte row offsets that are not on 1024-byte swizzle-atom boundaries (halo rows of 1280 / 2304 B plus one pixel per
-// horizontal tap).  That relies on the hardware applying the 128-byte XOR swizzle to the final shared-memory address, as
+// [62,64) layout type (1 = SWIZZLE_128B); the base-offset field [49,52) is left 0.  The convolution kernels start halo
+// operands (A operands, and the B operands of the 64-channel layer's swapped MMAs) at 128-byte row offsets that are not on
+// 1024-byte swizzle-atom boundaries (halo rows of 1280 / 2304 B plus one pixel per horizontal tap).  That relies on the hardware applying the 128-byte XOR swizzle to the final shared-memory address, as
 // the TMA writes it, rather than relative to the start address: observed H100 behaviour, not a documented guarantee; the
 // per-kernel tests against the oracle (every tap, ragged shapes) pin it.
 //   K-major SW128: 8 rows x 128 B atoms, SBO = stride between 8-row groups, LBO unused.
@@ -146,7 +146,42 @@ struct Wgmma<64, TA, TB> {
         : "l"(da), "l"(db), "r"(accum), "n"(TA), "n"(TB));
   }
 };
+template <int TA, int TB>
+struct Wgmma<128, TA, TB> {
+  __device__ __forceinline__ static void run(float* d, uint64_t da, uint64_t db, uint32_t accum) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, "
+        "%14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, "
+        "%37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, "
+        "%60, %61, %62, %63}, %64, %65, p, 1, 1, %67, %68;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+          "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+          "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+          "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]),
+          "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]),
+          "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]),
+          "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]),
+          "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(da), "l"(db), "r"(accum), "n"(TA), "n"(TB));
+  }
+};
 // The accumulator fragment of m64nN: register 4*j + 2*i + c of thread t holds row 16*(t/32 % 4) + (t%32)/4 + 8*i and
 // column 8*j + 2*(t%4) + c.
+
+// Four 8 x 8 b16 matrices between shared memory and registers, transposed: lanes 8m .. 8m + 7 give the addresses of the
+// eight 16-byte rows of matrix m, and register m of lane t holds the elements (rows 2*(t%4) and 2*(t%4) + 1, column t/4)
+// of matrix m in its low and high halves.  That is the accumulator fragment above with the 16-byte rows on its columns.
+__device__ __forceinline__ void ldmatrix_x4_trans(uint32_t (&r)[4], uint32_t addr) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
+               : "r"(addr)
+               : "memory");
+}
+__device__ __forceinline__ void stmatrix_x4_trans(uint32_t addr, const uint32_t (&r)[4]) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.trans.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r[0]), "r"(r[1]),
+               "r"(r[2]), "r"(r[3])
+               : "memory");
+}
 
 }  // namespace tcptx
