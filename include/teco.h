@@ -261,6 +261,39 @@ int teco_lpips_head_f32(const float* fa, int32_t Na, const float* fb, int32_t Nb
                         const int32_t* ib_host, int32_t P, int32_t H, int32_t W, int32_t C, const float* lin, double* out,
                         void* stream);
 
+/* ---------------------------------------------------------------------------------------
+ * tOF (reference metrics.py:143-169): cv2.cvtColor(RGB2GRAY) and cv2.calcOpticalFlowFarneback(prev, next, None,
+ * 0.5, 3, 15, 3, 5, 1.2, 0) in stages, each batched over frames or frame pairs, then the per-pair tOF.  Only these
+ * parameters exist.  Level k of an H x W frame is round_half_even(H / 2^k) x round_half_even(W / 2^k); levels
+ * whose sides would fall below 32 are dropped (tecogan_b200/tof.py: pyramid_sizes).  DESIGN.md section 4.4.
+ * ------------------------------------------------------------------------------------- */
+/* uint8 RGB [N,H,W,3] read through the window (y0,x0,h,w) -> grey [N,h,w] uint8,
+ * (9798 R + 19235 G + 3735 B + 16384) >> 15 (cv2's COLOR_RGB2GRAY on uint8, bit for bit). */
+int teco_tof_grey_u8(const uint8_t* img, int32_t N, int32_t H, int32_t W, int32_t y0, int32_t x0, int32_t h, int32_t w,
+                     uint8_t* grey, void* stream);
+/* Pyramid level 0..3 of full-resolution grey frames [N,H,W] -> out [N,lh,lw] fp32: Gaussian blur (reflect-101;
+ * sigma (2^level - 1) / 2, ksize max(cvRound(5 sigma) | 1, 3); level 0: the fixed 1/4 1/2 1/4) of the FULL frame,
+ * then INTER_LINEAR to lh x lw (an exact halving is the 2x2 mean).  (lh, lw) must be the level's size. */
+int teco_farneback_pyramid_u8(const uint8_t* grey, int32_t N, int32_t H, int32_t W, int32_t level, int32_t lh, int32_t lw,
+                              float* out, void* stream);
+/* Polynomial expansion (poly_n 5, sigma 1.2) of fp32 images [N,h,w] -> R [N,h,w,5] fp32, channels = coefficients
+ * of (y, x, yy, xx, xy); borders replicated.  One R per frame and level serves every pair that uses the frame. */
+int teco_farneback_polyexp_f32(const float* img, int32_t N, int32_t h, int32_t w, float* R, void* stream);
+/* One update iteration of P pairs: pair p = (R[i0_host[p]], R[i1_host[p]]) of R [Nf,h,w,5], flow_in [P,h,w,2]
+ * (NULL: zero flow) -> flow_out [P,h,w,2] (must not alias flow_in).  Per-pixel field from R0, R1 sampled at
+ * x + flow and the border weights, 15x15 box mean (float64), (g11 g22 - g12^2 + 1e-3)-regularised solve.
+ * i0_host / i1_host: HOST arrays, 1 <= P <= 256. */
+int teco_farneback_iterate_f32(const float* R, int32_t Nf, int32_t h, int32_t w, const int32_t* i0_host,
+                               const int32_t* i1_host, int32_t P, const float* flow_in, float* flow_out, void* stream);
+/* Flow of the coarser level [P,sh,sw,2] -> INTER_LINEAR to [P,h,w,2], times 2 (1 / pyr_scale). */
+int teco_farneback_flow_up_f32(const float* flow_in, int32_t P, int32_t sh, int32_t sw, float* flow_out, int32_t h,
+                               int32_t w, void* stream);
+/* tOF of P flow pairs [P,H,W,2] over the window (y0,x0,h,w) (crop_8x8): out[p] = mean of
+ * sqrt(|a-b|_x^2 + |a-b|_y^2) (fp32 per pixel as numpy, float64 sum; no atomics: deterministic).
+ * partial: scratch of P * 32 doubles. */
+int teco_tof_reduce_f32(const float* flow_a, const float* flow_b, int32_t P, int32_t H, int32_t W, int32_t y0, int32_t x0,
+                        int32_t h, int32_t w, double* partial, double* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

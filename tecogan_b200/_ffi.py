@@ -81,6 +81,12 @@ SIGNATURES = {
     "teco_lpips_input_u8": [_P, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _P, _P],
     "teco_maxpool3s2_f32": [_P, _P, _I32, _I32, _I32, _I32, _P],
     "teco_lpips_head_f32": [_P, _I32, _P, _I32, _P, _P, _I32, _I32, _I32, _I32, _P, _P, _P],
+    "teco_tof_grey_u8": [_P, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _P, _P],
+    "teco_farneback_pyramid_u8": [_P, _I32, _I32, _I32, _I32, _I32, _I32, _P, _P],
+    "teco_farneback_polyexp_f32": [_P, _I32, _I32, _I32, _P, _P],
+    "teco_farneback_iterate_f32": [_P, _I32, _I32, _I32, _P, _P, _I32, _P, _P, _P],
+    "teco_farneback_flow_up_f32": [_P, _I32, _I32, _I32, _P, _I32, _I32, _P],
+    "teco_tof_reduce_f32": [_P, _P, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _P, _P, _P],
 }
 _RESTYPES = {"teco_packed_weight_bytes": C.c_int64, "teco_crc32c": C.c_int64}
 

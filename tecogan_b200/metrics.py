@@ -1,10 +1,9 @@
 """Evaluation metrics of the reference's `metrics.py` computed on the device (SURVEY.md 8f-3): PSNR and SSIM on the Y channel
-of the uint8 result / target frames here, and -- given an `lpips.LPIPS` model -- LPIPS and tLP100 (tecogan_b200/lpips.py).
+of the uint8 result / target frames here, given an `lpips.LPIPS` model LPIPS and tLP100 (tecogan_b200/lpips.py), and with
+tof=True the Farneback-flow tOF (tecogan_b200/tof.py).
 Same function names and argument order as the reference (`psnr(img_true, img_pred)`, `ssim(img_true, img_pred)`,
 `crop_8x8(img)`, metrics.py:63-92); frames are uint8 RGB CUDA tensors `[H,W,3]` (or `[N,H,W,3]` for the batched calls),
 i.e. exactly what `main.py` inference writes through `save_img`.
-
-Not here, on purpose: tOF (cv2's Farneback optical flow, a CPU library routine) -- DESIGN.md section 6.
 """
 import math
 
@@ -98,10 +97,10 @@ def frame_metrics(targets, results, crop=True):
     return _finish(acc, win, True)
 
 
-def evaluate_sequence(targets, results, cutfr=2, lpips=None):
-    """The reference's per-folder loop (metrics.py:124-202) without tOF: frames cutfr .. N-cutfr-1, crop_8x8, per-frame
-    lists and their means (the 'FolderAvg' numbers).  PSNR and SSIM always; with `lpips` (an lpips.LPIPS model) also
-    LPIPS and tLP100, whose list starts at frame cutfr+1 and so is one shorter."""
+def evaluate_sequence(targets, results, cutfr=2, lpips=None, tof=False):
+    """The reference's per-folder loop (metrics.py:124-202): frames cutfr .. N-cutfr-1, crop_8x8, per-frame lists and
+    their means (the 'FolderAvg' numbers).  PSNR and SSIM always; with `lpips` (an lpips.LPIPS model) also LPIPS and
+    tLP100, and with tof=True also tOF; the temporal lists start at frame cutfr+1 and so are one shorter."""
     t, p = _as_batch(targets, "targets"), _as_batch(results, "results")
     n = t.shape[0]
     if n - 2 * cutfr <= 0:
@@ -113,4 +112,8 @@ def evaluate_sequence(targets, results, cutfr=2, lpips=None):
         lp, tlp = lpips.sequence(t[cutfr:n - cutfr], p[cutfr:n - cutfr], win)
         r.update({"LPIPS": lp, "tLP100": tlp, "FolderAvg_LPIPS": sum(lp) / len(lp),
                   "FolderAvg_tLP100": sum(tlp) / len(tlp) if tlp else float("nan")})
+    if tof:
+        from .tof import tof_sequence
+        of = tof_sequence(t[cutfr:n - cutfr], p[cutfr:n - cutfr])
+        r.update({"tOF": of, "FolderAvg_tOF": sum(of) / len(of) if of else float("nan")})
     return r
