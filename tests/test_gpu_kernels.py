@@ -108,30 +108,6 @@ def test_warp_and_gradients_match_oracle():
     assert_close(g_got[1], g_ref[1], 1e-4, what="warp dflow")
 
 
-@pytest.mark.parametrize("h,w,fh,fw,B", [(16, 16, 16, 16, 1), (18, 22, 16, 16, 2), (36, 45, 32, 40, 1)])
-def test_fused_feedback_kernel_matches_oracle_composition(h, w, fh, fw, B):
-    """upscale_four(4*pad_sym(flow_lr)) -> dense_image_warp(pre_gen) -> space_to_depth, main.py:201,212-215."""
-    from tecogan_b200 import kernels as K
-    pre_gen, flow_lr = rnd(1, B, 4 * h, 4 * w, 3, lo=0, hi=1), rnd(2, B, fh, fw, 2, lo=-6, hi=6)
-    fl = O.upscale_four(O.pad_symmetric_br(flow_lr, h - fh, w - fw) * 4.0)
-    warped = O.dense_image_warp(pre_gen, fl)
-    ref = O.space_to_depth4(warped)
-    dst = torch.zeros(B, h, w, 48, device="cuda")
-    wout = torch.zeros(B, 4 * h, 4 * w, 3, device="cuda")
-    K.warp_s2d_fused(dev(pre_gen), dev(flow_lr), dst, 0, warped_out=wout)
-    assert_close(wout, warped, 2e-5, what="fused warp")
-    assert_close(dst, ref, 2e-5, what="fused s2d")
-    # bf16 destination inside a 64-channel packed buffer, reading [-1,1] data with the deprocess folded in
-    dst16 = torch.zeros(B, h, w, 64, device="cuda", dtype=torch.bfloat16)
-    K.warp_s2d_fused(dev(pre_gen * 2 - 1), dev(flow_lr), dst16, 0, in_scale=0.5, in_shift=0.5)
-    assert_close(dst16[..., :48], ref, 5e-3, what="fused s2d bf16")
-    assert float(dst16[..., 48:].abs().max()) == 0.0
-    # unaligned channel offset (reference channel order: LR first) takes the scalar store path
-    dst51 = torch.zeros(B, h, w, 51, device="cuda")
-    K.warp_s2d_fused(dev(pre_gen), dev(flow_lr), dst51, 3)
-    assert_close(dst51[..., 3:], ref, 2e-5, what="fused s2d @3")
-
-
 def test_in_tree_resamplers_match_golden_and_oracle():
     import os
     from tecogan_b200 import kernels as K

@@ -190,14 +190,15 @@ def test_metrics_cli_lists_png_like_the_reference(tmp_path):
 
 
 def test_warp_v2_source_window_holds_every_query_of_its_tile():
-    """Host restatement of the window construction of warp_s2d_v2_kernel (csrc/warp_s2d_v2.cu::v2_window): from the min / max of
+    """The host restatement (tests/warp_tiles.py::window) of the window construction of warp_s2d_v2_kernel
+    (csrc/warp_s2d_v2.cu::v2_window), which test_gpu_warp_feedback.py uses to classify its cases: from the min / max of
     the 4 x flow_lr samples around a 4 x 32 LR tile it derives the rows / columns of the previous HR frame that the tile's
     bilinear queries can touch.  Property: for random flows (smooth, rough, far out of range) and ragged frame sizes, every
     query of every HR pixel of the tile -- floor clamped to [0, size-2] plus its +1 neighbour, as dense_image_warp does --
     lies inside the window, and the 'interior' flags are only set when no clamp can trigger."""
     import numpy as np
+    from tests.warp_tiles import V2_TLH as TLH, V2_TLW as TLW, tile_bounds, window
     rng = np.random.RandomState(0)
-    TLH, TLW = 4, 32
 
     def upscale4(f):                                   # upscale_four: legacy bilinear x4, edge-replicated (lib/ops.py:126-163)
         h, w, _ = f.shape
@@ -212,20 +213,8 @@ def test_warp_v2_source_window_holds_every_query_of_its_tile():
         fl = upscale4(flow4.astype(np.float64))
         for ly0 in range(0, h, TLH):
             for lx0 in range(0, w, TLW):
-                ii = np.minimum(np.arange(ly0, ly0 + TLH + 1), h - 1)
-                jj = np.minimum(np.arange(lx0, lx0 + TLW + 1), w - 1)
-                s = flow4[np.ix_(ii, jj)]
-                mny, mxy, mnx, mxx = s[..., 0].min(), s[..., 0].max(), s[..., 1].min(), s[..., 1].max()
                 Y0, X0 = 4 * ly0, 4 * lx0
-                qy_lo, qy_hi = Y0 - mxy, Y0 + 4 * TLH - 1 - mny
-                qx_lo, qx_hi = X0 - mxx, X0 + 4 * TLW - 1 - mnx
-                clampf = lambda v, hi: min(max(v, 0.0), hi)
-                y_lo = int(clampf(np.floor(qy_lo) - 1, H - 2))
-                y_hi = int(clampf(np.floor(qy_hi) + 1, H - 2)) + 1
-                x_lo = int(clampf(np.floor(qx_lo) - 1, W - 2)) & ~3
-                x_hi = min((int(clampf(np.floor(qx_hi) + 1, W - 2)) + 1) | 3, W - 1)
-                int_y = qy_lo >= 1 and qy_hi <= H - 3
-                int_x = qx_lo >= 1 and qx_hi <= W - 3
+                y_lo, y_hi, x_lo, x_hi, int_y, int_x = window(*tile_bounds(flow4, ly0, lx0, TLH, h, w), Y0, 4 * TLH, X0, H, W)[:6]
                 assert (x_hi - x_lo + 1) % 4 == 0 and x_lo % 4 == 0          # 16-byte aligned bulk copies of fp32 RGB rows
                 ys = np.arange(Y0, min(Y0 + 4 * TLH, H))
                 xs = np.arange(X0, min(X0 + 4 * TLW, W))
