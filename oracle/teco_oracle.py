@@ -97,7 +97,10 @@ def resize_bilinear_legacy(x, oh, ow):
 def dense_image_warp(image, flow):
     """tf.contrib.image.dense_image_warp.  [TF-ext] SURVEY A.7.
     out[b,y,x] = bilinear(image[b], (y - flow[b,y,x,0], x - flow[b,y,x,1])), floor clamped to
-    [0,size-2], alpha clamped to [0,1].  lib/Teco.py:120,140,224,254; main.py:215."""
+    [0,size-2], alpha clamped to [0,1].  lib/Teco.py:120,140,224,254; main.py:215.
+    Gradient to the query only where 0 < alpha_raw <= 1: TF clamps with minimum(maximum(0, a), 1), and at a tie
+    Maximum's gradient goes to its first argument (the constant 0) and Minimum's to its first argument (a).
+    torch.clamp would pass it at both ends, so at every integer query."""
     n, h, w, c = image.shape
     gy = torch.arange(h, dtype=image.dtype).view(1, h, 1)
     gx = torch.arange(w, dtype=image.dtype).view(1, 1, w)
@@ -106,7 +109,9 @@ def dense_image_warp(image, flow):
 
     def split(q, size):
         fl = torch.clamp(torch.floor(q), 0, size - 2)
-        al = torch.clamp(q - fl, 0.0, 1.0)
+        a = q - fl
+        al = torch.clamp(a, 0.0, 1.0)
+        al = torch.where((a > 0) & (a <= 1), al, al.detach())
         return fl.long(), al
 
     y0, ay = split(qy, h)

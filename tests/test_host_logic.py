@@ -230,6 +230,18 @@ def test_warp_v2_source_window_holds_every_query_of_its_tile():
                 assert x_lo <= ix.min() and ix.max() + 1 <= x_hi, (case, ly0, lx0, x_lo, x_hi, ix.min(), ix.max())
 
 
+def test_resample_case_tables_reach_every_edge():
+    """tests/resample_cases.py classifies each case of test_gpu_resample_exact.py from its own seeded inputs: alpha_raw
+    classes per warp axis, max-pool ties, odd sizes, bf16 rounding midpoints, the bicubic kernel dispatched to, and
+    launches above one grid-stride pass at 132 SMs.  Together the cases of each family reach every required key."""
+    from tests import resample_cases as R
+    for family, (table, _) in R.FAMILIES.items():
+        seen = set()
+        for name in table:
+            seen |= R.keys(family, name)
+        assert R.REQUIRED[family] <= seen, (family, sorted(R.REQUIRED[family] - seen))
+
+
 def test_conv_transpose_gradients_through_the_space_to_depth_identity():
     """kernels._ConvTranspose2xTC computes both gradients of conv2_tran as ordinary 3x3 stride-1 problems on the space-to-depth
     form of dz (W' = zero-scattered weights, rows kernels._tconv_rows()).  The identity itself, in fp32 on the CPU with the

@@ -122,6 +122,44 @@ def test_warp_identity_and_integer_shift_and_clamp():
     assert torch.allclose(out[0, 3, 2], im[0, 2, 4]) and torch.allclose(out[0, 0, 7], im[0, 0, 7])
 
 
+def _warp_clamp_only(image, flow):
+    """dense_image_warp's forward value as the oracle computed it before the TF gradient rule: clamp alone."""
+    n, h, w, c = image.shape
+    qy = torch.arange(h, dtype=image.dtype).view(1, h, 1) - flow[..., 0]
+    qx = torch.arange(w, dtype=image.dtype).view(1, 1, w) - flow[..., 1]
+    fy, fx = torch.clamp(torch.floor(qy), 0, h - 2), torch.clamp(torch.floor(qx), 0, w - 2)
+    ay, ax = torch.clamp(qy - fy, 0.0, 1.0).unsqueeze(-1), torch.clamp(qx - fx, 0.0, 1.0).unsqueeze(-1)
+    b, y0, x0 = torch.arange(n).view(n, 1, 1), fy.long(), fx.long()
+    tl, tr, bl, br = image[b, y0, x0], image[b, y0, x0 + 1], image[b, y0 + 1, x0], image[b, y0 + 1, x0 + 1]
+    top, bot = ax * (tr - tl) + tl, ax * (br - bl) + bl
+    return ay * (bot - top) + top
+
+
+def test_warp_gradient_to_the_flow_follows_tf_at_integer_queries():
+    """At zero flow every query is an integer: alpha_raw is 0 everywhere but in row H-1 (y) and column W-1 (x), where
+    the floor is clamped to size-2 and alpha_raw is 1.  TF passes the query gradient only where 0 < alpha_raw <= 1, so
+    dflow is zero except row H-1 of component 0 and column W-1 of component 1 -- and non-zero there."""
+    img, r = _rnd(11, 2, 6, 7, 3), _rnd(12, 2, 6, 7, 3)
+    flow = torch.zeros(2, 6, 7, 2, requires_grad=True)
+    (d,) = torch.autograd.grad((O.dense_image_warp(img, flow) * r).sum(), flow)
+    assert (d[:, :-1, :, 0] == 0).all() and (d[:, :, :-1, 1] == 0).all()
+    assert (d[:, -1, :, 0] != 0).all() and (d[:, :, -1, 1] != 0).all()
+    # a fractional query keeps its gradient; integer shifts inside the frame have none on that axis
+    flow = torch.zeros(2, 6, 7, 2)
+    flow[..., 0], flow[..., 1] = 0.25, -1.0
+    flow.requires_grad_(True)
+    (d,) = torch.autograd.grad((O.dense_image_warp(img, flow) * r).sum(), flow)
+    assert (d[:, 1:, :, 0] != 0).all() and (d[:, :, :-2, 1] == 0).all()
+
+
+def test_warp_forward_value_is_unchanged_by_the_gradient_rule():
+    img = _rnd(13, 3, 9, 11, 3)
+    for flow in (torch.zeros(3, 9, 11, 2), torch.round(_rnd(14, 3, 9, 11, 2) * 6), _rnd(15, 3, 9, 11, 2) * 4,
+                 torch.round(_rnd(16, 3, 9, 11, 2) * 64) / 16, _rnd(17, 3, 9, 11, 2) * 30):
+        assert torch.equal(O.dense_image_warp(img, flow), _warp_clamp_only(img, flow))
+        assert torch.equal(O.dense_image_warp(img.double(), flow.double()), _warp_clamp_only(img.double(), flow.double()))
+
+
 def test_inference_sequence_shapes_nonmultiple_of_8():
     pg, pf = O.init_generator(num_resblock=2), O.init_fnet()
     g = _load("calendar_lr")
