@@ -14,7 +14,11 @@ Differences forced by the environment, stated once:
     down-sampling, crops) is the same either way;
   * --precision {bf16,fp32} selects wgmma tensor-core or fp32 CUDA-core convolutions for inference;
     --train_precision {fp32,bf16} does the same for training (default fp32, the reference's arithmetic);
-  * under `torchrun` each rank trains on its own clip shard with one NCCL all-reduce per step.
+  * under `torchrun` each rank trains on its own clip shard with one NCCL all-reduce per step;
+  * monitoring (--summary_dir: TensorBoard scalars, logfile.txt, validation scalars, test-sequence frames at every
+    checkpoint) runs on rank 0 only, in process: the held-out scenes end_dir+1..end_dir_val are optional (validation is
+    skipped with a message when they are absent) and the test sequence is super-resolved synchronously instead of by an
+    un-awaited subprocess.
 """
 import argparse
 import math
@@ -176,12 +180,9 @@ def restore_train_state(train_state, spec):
 
 
 def inference(FLAGS):
-    import numpy as np
-    import torch
     from tecogan_b200 import config, variables as V
     from tecogan_b200.engine import InferenceEngine
     from tecogan_b200.lib.dataloader import inference_data_loader
-    from tecogan_b200.lib.ops import save_img
     if FLAGS.checkpoint is None:
         raise ValueError('The checkpoint file is needed to performing the test.')
     inference_data = inference_data_loader(FLAGS)
@@ -195,6 +196,15 @@ def inference(FLAGS):
     print('Finish building the network')
     image_dir = FLAGS.output_dir if FLAGS.output_pre == "" else os.path.join(FLAGS.output_dir, FLAGS.output_pre)
     os.makedirs(image_dir, exist_ok=True)
+    super_resolve_frames(eng, inference_data, image_dir, FLAGS.output_name, FLAGS.output_ext)
+
+
+def super_resolve_frames(eng, inference_data, image_dir, output_name, output_ext):
+    """The per-frame loop of reference main.py:253-268: every frame through `eng`, the 5 warm-up frames discarded, the
+    rest saved as <output_name>_<frame name>.<output_ext>."""
+    import numpy as np
+    import torch
+    from tecogan_b200.lib.ops import save_img
     max_iter = len(inference_data.inputs)
     srtime = 0
     print('Frame evaluation starts!!')
@@ -208,18 +218,23 @@ def inference(FLAGS):
         srtime += time.time() - t0
         if i >= 5:
             name, _ = os.path.splitext(os.path.basename(str(inference_data.paths_LR[i])))
-            filename = FLAGS.output_name + '_' + name
+            filename = output_name + '_' + name
             print('saving image %s' % filename)
-            save_img(os.path.join(image_dir, "%s.%s" % (filename, FLAGS.output_ext)), out[0])
+            save_img(os.path.join(image_dir, "%s.%s" % (filename, output_ext)), out[0])
         else:   # First 5 is a hard-coded symmetric frame padding, ignored but time added!
             print("Warming up %d" % (5 - i))
     print("total time " + str(srtime) + ", frame number " + str(max_iter))
 
 
-def synthetic_hr_batch(FLAGS, step, rank, device):
-    """Seeded smooth-noise HR clips [B,RNN_N,4crop+8,4crop+8,3] in [0,1] moving by a constant sub-pixel velocity."""
+TEST_SEQUENCE_DIR = './LR/calendar/'      # reference main.py:164, hard-coded there as well
+
+
+def synthetic_hr_batch(FLAGS, step, rank, device, validation=False):
+    """Seeded smooth-noise HR clips [B,RNN_N,4crop+8,4crop+8,3] in [0,1] moving by a constant sub-pixel velocity.
+    Training batch `step` of `rank` uses seed 1000003 * rank + step; validation batch `step` counts down from the top of
+    the generator's 32-bit seed range, which no training batch reaches (fewer than 4000 ranks, 4e9 steps)."""
     import torch
-    g = torch.Generator().manual_seed(1000003 * rank + step)
+    g = torch.Generator().manual_seed(0xFFFFFFFF - step if validation else 1000003 * rank + step)
     B, T, S = FLAGS.batch_size, FLAGS.RNN_N, FLAGS.crop_size * 4 + 8
     base = torch.rand(B, 3, S // 8 + 8, S // 8 + 8, generator=g)
     big = torch.nn.functional.interpolate(base, scale_factor=8, mode='bicubic', align_corners=False).clamp(0, 1)
@@ -228,6 +243,50 @@ def synthetic_hr_batch(FLAGS, step, rank, device):
         oy, ox = 8 + 2 * t, 8 + t
         out[:, t] = big[:, :, oy:oy + S, ox:ox + S].permute(0, 2, 3, 1)
     return out.to(device)
+
+
+def test_while_train(FLAGS, step):
+    """reference main.py:151-174 (testWhileTrain), in process and synchronous: the first 10 frames of ./LR/calendar/
+    super-resolved with the current weights at the --precision inference arithmetic into <output_dir>/train/ as
+    <%09d step>_<frame>.<output_ext> -- the files `main.py --mode inference --input_dir_len 10 --output_name %09d
+    --output_pre ""` writes.  The global precision is restored and the engine (its CUDA graph, buffers and packed weights)
+    is released before training continues; the training step keeps its own buffers and repacks its weights."""
+    import argparse
+    import torch
+    from tecogan_b200 import config
+    from tecogan_b200.engine import InferenceEngine
+    from tecogan_b200.lib.dataloader import inference_data_loader
+    print('[testWhileTrain] step %d:' % step)
+    if not os.path.isdir(TEST_SEQUENCE_DIR):
+        print('[testWhileTrain] %s not found, no test-sequence frames' % TEST_SEQUENCE_DIR)
+        return
+    tflags = argparse.Namespace(input_dir_LR=TEST_SEQUENCE_DIR, input_dir_HR=None, input_dir_len=10)
+    data = inference_data_loader(tflags)
+    h, w = data.inputs[0].shape[:2]
+    image_dir = os.path.join(FLAGS.output_dir, 'train')
+    os.makedirs(image_dir, exist_ok=True)
+    prev_precision = config.precision()
+    try:
+        config.set_precision(FLAGS.precision)
+        eng = InferenceEngine(h, w, FLAGS.num_resblock)
+        super_resolve_frames(eng, data, image_dir, '%09d' % step, FLAGS.output_ext)
+        del eng
+        torch.cuda.synchronize()
+    finally:
+        config.set_precision(prev_precision)
+
+
+def validation_source(FLAGS, dev):
+    """k -> HR validation batch k (reference lib/dataloader.py:287-297), or None when there is no validation data.
+    Batch k depends on k only, so a resumed run sees the same validation batches."""
+    if FLAGS.input_video_dir:
+        from tecogan_b200.lib.dataloader import validation_loader
+        loader, why = validation_loader(FLAGS)
+        if loader is None:
+            print('[main] validation skipped: %s' % why)
+            return None
+        return lambda k: loader.batch(k).to(dev)
+    return lambda k: synthetic_hr_batch(FLAGS, k, 0, dev, validation=True)
 
 
 def train(FLAGS):
@@ -279,6 +338,13 @@ def train(FLAGS):
         print('Loading everything from the checkpoint to continue the training...')
         restore_train_state(Net.train, FLAGS.checkpoint)
     start_step = Net.global_step()
+    monitor = bool(FLAGS.summary_dir) and rank == 0      # summaries, validation, test sequence: rank 0, no collective
+    if monitor:
+        from tecogan_b200.summary import EventWriter
+        writer = EventWriter(FLAGS.summary_dir)
+        val_hr = validation_source(FLAGS, dev)
+        test_while_train(FLAGS, start_step)
+    tested = {start_step}
     if loader is not None:
         clip_iter = loader.batches(start_step=start_step)
         next_hr = lambda gstep: next(clip_iter).to(dev, non_blocking=True)
@@ -293,6 +359,15 @@ def train(FLAGS):
             run_step = Net.global_step()
             if step == 0 and rank == 0:
                 print('Optimization starts!!!(Ctrl+C to stop, will try saving the last model...)')
+            if monitor and (run_step % FLAGS.summary_freq) == 0:     # reference main.py:384-402
+                print('Run and Recording summary!!')
+                writer.add_scalars(run_step, [('learning_rate', res["lr"])] + list(zip(Net.update_list_name, Net.update_list_avg())))
+                if val_hr is not None:
+                    val = Net.train.evaluate(*frvsr_gpu_data_loader(val_hr(run_step // FLAGS.summary_freq), FLAGS))
+                    writer.add_scalars(run_step, [('val_' + name, v) for name, v in val.items()])
+                    print('-----------Validation data scalars-----------')
+                    for name, v in val.items():
+                        print('val_' + name, v)
             if (run_step % FLAGS.display_freq) == 0 and rank == 0:
                 rate = (step + 1) * FLAGS.batch_size * world / (time.time() - start)
                 remaining = (max_iter - start_step - step) * FLAGS.batch_size * world / rate
@@ -305,14 +380,23 @@ def train(FLAGS):
             if (run_step % FLAGS.save_freq) == 0 and rank == 0:
                 print('Save the checkpoint')
                 save_checkpoint(store, FLAGS.output_dir, run_step, Net.train)
+                if monitor:
+                    test_while_train(FLAGS, run_step)
+                    tested.add(run_step)
     except KeyboardInterrupt:
         if rank == 0:
             print('main.py: KeyboardInterrupt->saving the checkpoint')
             save_checkpoint(store, FLAGS.output_dir, Net.global_step(), Net.train)
+            if monitor:
+                test_while_train(FLAGS, Net.global_step())
         print('main.py: quit')
         sys.exit(0)
     if rank == 0:
         save_checkpoint(store, FLAGS.output_dir, Net.global_step(), Net.train)
+        if monitor and Net.global_step() not in tested:
+            test_while_train(FLAGS, Net.global_step())
+    if monitor:
+        writer.close()
     print('Optimization done!!!!!!!!!!!!')
     if world > 1:
         dist.destroy_process_group()
@@ -325,14 +409,23 @@ def main(argv=None):
     if FLAGS.output_dir is None:
         raise ValueError('The output directory is needed')
     os.makedirs(FLAGS.output_dir, exist_ok=True)
+    tee = None
     if FLAGS.summary_dir:
         os.makedirs(FLAGS.summary_dir, exist_ok=True)
-    if FLAGS.mode == 'inference':
-        inference(FLAGS)
-    elif FLAGS.mode == 'train':
-        train(FLAGS)
-    else:
-        raise ValueError("mode must be 'inference' or 'train'")
+        if os.environ.get('RANK', '0') == '0':          # reference main.py:126-136: stdout also goes to logfile.txt
+            from tecogan_b200.summary import Tee
+            tee = sys.stdout = Tee(os.path.join(FLAGS.summary_dir, 'logfile.txt'))
+    try:
+        if FLAGS.mode == 'inference':
+            inference(FLAGS)
+        elif FLAGS.mode == 'train':
+            train(FLAGS)
+        else:
+            raise ValueError("mode must be 'inference' or 'train'")
+    finally:
+        if tee is not None:
+            sys.stdout = tee.terminal
+            tee.close()
 
 
 if __name__ == '__main__':

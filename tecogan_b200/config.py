@@ -1,8 +1,9 @@
 """Run-time configuration of the compute path (not part of the reference interface)."""
+import contextlib as _contextlib
 import os as _os
 
 _cfg = {"precision": "bf16", "train_precision": "fp32", "lin_trunk": _os.environ.get("TECO_LIN_TRUNK", "0") == "1",
-        "train_tc_all": _os.environ.get("TECO_TRAIN_TC_ALL", "1") == "1"}
+        "train_tc_all": _os.environ.get("TECO_TRAIN_TC_ALL", "1") == "1", "train_forward": False}
 
 
 def set_precision(p):
@@ -30,6 +31,24 @@ def set_train_precision(p):
 
 def train_precision():
     return _cfg["train_precision"]
+
+
+@_contextlib.contextmanager
+def train_forward():
+    """Inside this block the training graph picks its convolution kernels as under autograd even when gradients are off:
+    the trainer's forward-only evaluation (Network.train.evaluate) runs under torch.no_grad() on the kernels a training
+    step runs, so its losses are the ones training would report for the same batch."""
+    prev = _cfg["train_forward"]
+    _cfg["train_forward"] = True
+    try:
+        yield
+    finally:
+        _cfg["train_forward"] = prev
+
+
+def training_kernels(grad_enabled):
+    """Convolution dispatch of the training graph: its kernels run under autograd and inside train_forward()."""
+    return grad_enabled or _cfg["train_forward"]
 
 
 def set_lin_trunk(on):

@@ -282,6 +282,11 @@ class _FlatAdam:
         K.adam_step(self.flat, self.m, self.v, flat_grad, lr_t, self.b1, self.b2, self.eps, gscale)
 
 
+def _stack_scalars(vals, device):
+    """Loss scalars (0-d tensors or Python numbers) as one fp32 device vector."""
+    return torch.stack([v.detach().float() if torch.is_tensor(v) else torch.full((), float(v), device=device) for v in vals])
+
+
 Network = collections.namedtuple('Network', 'gen_output, train, learning_rate, update_list, '
                                  'update_list_name, update_list_avg, image_summary, global_step')
 
@@ -303,6 +308,7 @@ class _TrainState:
         self.loss_ema = None
         self.counter1 = self.counter2 = 0
         self.last = None
+        self.eval_in = self.eval_tg = self.eval_graph = None   # evaluate(): buffers and graph of its own
         from .. import config
         K.tc_cache_clear()                         # packed bf16 weights of a previous trainer are not ours
         prev_precision = config.precision()
@@ -365,8 +371,7 @@ class _TrainState:
             else:
                 b[o:o + n].copy_(gr.reshape(-1))
             o += n
-        scal = [g.t_balance if self.GAN else torch.zeros((), device=b.device)] + list(g.update_list)
-        scal = torch.stack([s_.detach().float() if torch.is_tensor(s_) else torch.full((), float(s_), device=b.device) for s_ in scal])
+        scal = _stack_scalars([g.t_balance if self.GAN else torch.zeros((), device=b.device)] + list(g.update_list), b.device)
         b[o:o + scal.numel()].copy_(scal)
         self._scal_off, self._n_scal = o, scal.numel()
         self._names_now = g.update_list_name
@@ -417,6 +422,49 @@ class _TrainState:
         self.last = {"update_list": vals, "update_list_name": self._names_now, "with_d": with_d, "lr": lr,
                      "gen_outputs": self._gen_outputs, "t_balance": scal_host[0], "tb_ema": self.tb_ema}
         return self.last
+
+    # ---- forward-only evaluation (reference main.py:299-304,391-402: the validation fetch of Net.update_list) -------
+    def _evaluate_compute(self):
+        """The training graph's forward on eval_in / eval_tg with the current weights: the kernels, precision and packed-weight
+        discipline of _compute, no autograd tape, and nothing written but the tensors this pass allocates."""
+        from .. import config
+        K.tc_cache_clear()            # pack the current weights in this pass (inside this graph when captured)
+        prev_precision = config.precision()
+        try:
+            config.set_precision("fp32")
+            with torch.no_grad(), config.train_forward():
+                g = _Graph(self.eval_in, self.eval_tg, self.FLAGS, self.GAN, self.global_step)
+        finally:
+            config.set_precision(prev_precision)
+        self._eval_scal = _stack_scalars(g.update_list, self.eval_in.device)
+        self._eval_names = list(g.update_list_name)
+
+    def evaluate(self, r_inputs, r_targets):
+        """Losses of the training graph on another batch, without training: {name: float} for every entry of
+        Network.update_list (the reference's `uplen` names -- t_balance, Dst_ratio and the D counters are running state,
+        not losses of a batch).  Runs at the current global_step (the Dst ratio of the last step) on the kernels of
+        training, from input buffers and a CUDA graph of its own, captured under the rule of the training step.  Weights,
+        Adam moments, the step counters, the EMAs, the with-D decision and the training step's buffers are only read."""
+        if self.eval_in is None:
+            self.eval_in = torch.empty_like(self.static_in)
+            self.eval_tg = torch.empty_like(self.static_tg)
+        self.eval_in.copy_(r_inputs)
+        self.eval_tg.copy_(r_targets)
+        if self.use_graph and self.FLAGS.Dt_ratio_add == 0.0:
+            if self.eval_graph is None:
+                side = torch.cuda.Stream()
+                side.wait_stream(torch.cuda.current_stream())
+                with torch.cuda.stream(side):
+                    self._evaluate_compute()
+                torch.cuda.current_stream().wait_stream(side)
+                torch.cuda.synchronize()
+                self.eval_graph = torch.cuda.CUDAGraph()
+                with torch.cuda.graph(self.eval_graph):
+                    self._evaluate_compute()
+            self.eval_graph.replay()
+        else:
+            self._evaluate_compute()
+        return dict(zip(self._eval_names, self._eval_scal.tolist()))
 
     # ---- checkpoint / resume (reference: tf.train.Saver over GLOBAL_VARIABLES, main.py:307,346-349) -------------------
     def state_tensors(self):

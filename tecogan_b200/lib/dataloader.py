@@ -2,7 +2,8 @@
 frvsr_gpu_data_loader (lib/dataloader.py:306-332) and -- as the caller side of the training path -- a host loader for
 HR training clips (`HRClipLoader`) that follows `loadHR` + `tf.train.shuffle_batch` (lib/dataloader.py:147-273): same
 directory layout, frame windows, moving-first-frame / random-crop / flip augmentation, a thread pool instead of TF queue
-runners.  The validation split (lib/dataloader.py:287-296) only feeds TensorBoard summaries and is not loaded."""
+runners.  The validation split (lib/dataloader.py:287-296) is a second `HRClipLoader` over the held-out scenes
+(`validation_loader`); it feeds the val_* summaries of main.py --mode train --summary_dir."""
 import collections
 import concurrent.futures
 import os
@@ -61,6 +62,10 @@ def frvsr_gpu_data_loader(HR_frames, FLAGS):
     return lr, tgt
 
 
+class EmptyClipSet(ValueError):
+    """The scene range holds no usable clip, or fewer samples than one batch."""
+
+
 class HRClipLoader:
     """Host half of the training input (reference lib/dataloader.py:147-273, `loadHR`; main.py flags :60-78).
 
@@ -78,18 +83,26 @@ class HRClipLoader:
     every world-th clip of the permutation.  Decoding runs on `queue_thread` worker threads, `prefetch` batches ahead;
     every sample's augmentation is a function of (rand_seed, epoch, sample index) only, so a run is reproducible whatever
     the thread timing.  Output: float32 [B, RNN_N, tar_size, tar_size, 3] in [0, 1] (pinned when CUDA is available) for
-    `frvsr_gpu_data_loader`."""
+    `frvsr_gpu_data_loader`.
 
-    def __init__(self, FLAGS, tar_size=None, rank=0, world=1, prefetch=4):
+    `dirs` = (first, last) overrides str_dir..end_dir and `salt` != 0 moves every permutation and augmentation draw to a
+    stream of its own: the validation loader (`validation_loader`, reference lib/dataloader.py:287-297) reads the held-out
+    scenes end_dir+1..end_dir_val with the same augmentation, and its draws never repeat the training loader's.  With the
+    defaults the training batches are those of a loader without these arguments, byte for byte."""
+
+    def __init__(self, FLAGS, tar_size=None, rank=0, world=1, prefetch=4, dirs=None, salt=0, queue_thread=None):
         self.F = FLAGS
         self.tar_size = tar_size if tar_size is not None else FLAGS.crop_size * 4 + int(1.5 * 3.0) * 2
         self.rank, self.world, self.prefetch = rank, world, max(1, prefetch)
+        self.salt = [int(salt)] if salt else []       # last seed word; salt 0 leaves the training seeds as they were
+        self.queue_thread = int(FLAGS.queue_thread if queue_thread is None else queue_thread)
+        first, last = dirs if dirs is not None else (FLAGS.str_dir, FLAGS.end_dir)
         if FLAGS.input_video_dir == '':
             raise ValueError('Video input directory input_video_dir is not provided')
         if not os.path.exists(FLAGS.input_video_dir):
             raise ValueError('Video input directory not found')
         self.clips = []
-        for dir_i in range(FLAGS.str_dir, FLAGS.end_dir + 1):
+        for dir_i in range(first, last + 1):
             d = os.path.join(FLAGS.input_video_dir, '%s_%04d' % (FLAGS.input_video_pre, dir_i))
             if not os.path.exists(d):
                 continue
@@ -99,11 +112,11 @@ class HRClipLoader:
             self.clips.append(d)
         self.windows = FLAGS.max_frm - FLAGS.RNN_N + 1
         if not self.clips or self.windows <= 0:
-            raise Exception('No frame files in the video input directory')
+            raise EmptyClipSet('No frame files in the video input directory')
         self.image_count = len(self.clips) * self.windows
         self.steps_per_epoch = self.image_count // (FLAGS.batch_size * world)
         if self.steps_per_epoch == 0:
-            raise ValueError('HRClipLoader: %d samples cannot fill one batch of %d x %d ranks'
+            raise EmptyClipSet('HRClipLoader: %d samples cannot fill one batch of %d x %d ranks'
                              % (self.image_count, FLAGS.batch_size, world))
         print('Sequenced batches: {}, sequence length: {}'.format(self.image_count, FLAGS.RNN_N))
 
@@ -122,7 +135,7 @@ class HRClipLoader:
         """One augmented clip [RNN_N, tar, tar, 3]; deterministic in (rand_seed, epoch, index)."""
         F, T, tar = self.F, self.F.RNN_N, self.tar_size
         clip, start = self.clips[index // self.windows], index % self.windows
-        rng = np.random.default_rng([int(F.rand_seed) & 0x7FFFFFFF, int(epoch), int(index)])
+        rng = np.random.default_rng([int(F.rand_seed) & 0x7FFFFFFF, int(epoch), int(index)] + self.salt)
         moving = False
         if F.movingFirstFrame:
             step = np.floor(rng.uniform(-3.5, 4.5, size=(T, 2))).astype(np.int64)
@@ -149,21 +162,33 @@ class HRClipLoader:
         return np.ascontiguousarray(out, dtype=np.float32)
 
     def _order(self, epoch):
-        perm = np.random.default_rng([int(self.F.rand_seed) & 0x7FFFFFFF, 0x5EED, int(epoch)]).permutation(self.image_count)
+        perm = np.random.default_rng([int(self.F.rand_seed) & 0x7FFFFFFF, 0x5EED, int(epoch)] + self.salt).permutation(self.image_count)
         return perm[self.rank::self.world]
+
+    def _indices(self, step):
+        epoch, k = divmod(step, self.steps_per_epoch)
+        B = self.F.batch_size
+        return epoch, self._order(epoch)[k * B:(k + 1) * B]
+
+    def _empty_batch(self):
+        import torch
+        out = torch.empty((self.F.batch_size, self.F.RNN_N, self.tar_size, self.tar_size, 3), dtype=torch.float32)
+        return out.pin_memory() if torch.cuda.is_available() else out
+
+    def batch(self, step):
+        """Batch number `step` of the endless stream `batches()` yields, decoded on the calling thread."""
+        import torch
+        epoch, idx = self._indices(step)
+        out = self._empty_batch()
+        for b, i in enumerate(idx):
+            out[b] = torch.from_numpy(self.sample(int(i), epoch))
+        return out
 
     def batches(self, start_step=0):
         """Endless iterator over torch tensors [B, RNN_N, tar, tar, 3]; `start_step` lets a resumed run skip ahead."""
         import torch
-        B, T, tar = self.F.batch_size, self.F.RNN_N, self.tar_size
-        pin = torch.cuda.is_available()
-        spe = self.steps_per_epoch
-
-        def build(step):
-            epoch, k = divmod(step, spe)
-            idx = self._order(epoch)[k * B:(k + 1) * B]
-            return epoch, idx
-        with concurrent.futures.ThreadPoolExecutor(max_workers=max(1, int(self.F.queue_thread))) as pool:
+        build = self._indices
+        with concurrent.futures.ThreadPoolExecutor(max_workers=max(1, self.queue_thread)) as pool:
             pending = collections.deque()
 
             def submit(step):
@@ -175,10 +200,22 @@ class HRClipLoader:
             while True:
                 futs = pending.popleft()
                 submit(step + self.prefetch)
-                out = torch.empty((B, T, tar, tar, 3), dtype=torch.float32)
-                if pin:
-                    out = out.pin_memory()
+                out = self._empty_batch()
                 for b, f in enumerate(futs):
                     out[b] = torch.from_numpy(f.result())
                 yield out
                 step += 1
+
+
+VALIDATION_SALT = 0x7A1D
+
+
+def validation_loader(FLAGS):
+    """The held-out scenes end_dir+1 .. end_dir_val (reference lib/dataloader.py:287-297: same loader and augmentation,
+    queue_thread = 1) as (HRClipLoader, None), or (None, reason) when that range holds no usable scene or fewer samples
+    than one batch -- the reference raises there; here training goes on without validation."""
+    try:
+        return HRClipLoader(FLAGS, dirs=(FLAGS.end_dir + 1, FLAGS.end_dir_val), salt=VALIDATION_SALT, queue_thread=1), None
+    except EmptyClipSet as e:
+        return None, '%s (scenes %s_%04d .. %s_%04d)' % (e, FLAGS.input_video_pre, FLAGS.end_dir + 1,
+                                                         FLAGS.input_video_pre, FLAGS.end_dir_val)
