@@ -46,6 +46,8 @@ SIGNATURES = {
     "teco_conv3x3_wgrad_tc": [_I32, _I32, _I32, _I32, _I32, _I32, _I32, _P, _P, _P, _I32, _P],
     "teco_conv3x3_lin_supported": [_I32, _I32, _I32, _I32],
     "teco_conv3x3_lin_tc": [_I32, _I32, _I32, _I32, _P, _P, _P, _P, _P, _P, _P],
+    "teco_conv3x3_lin_in_smem": [_I32, _I32, _I32, _I32, _P],
+    "teco_conv3x3_lin_clusters": [],
     "teco_warp_f32": [_P, _P, _P, _I32, _I32, _I32, _I32, _P],
     "teco_warp_bwd_f32": [_P, _P, _P, _P, _P, _I32, _I32, _I32, _I32, _P],
     "teco_warp_s2d_fused": [_P, _P, _P, _P, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _F, _F, _P],

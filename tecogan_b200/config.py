@@ -2,7 +2,7 @@
 import contextlib as _contextlib
 import os as _os
 
-_cfg = {"precision": "bf16", "train_precision": "fp32", "lin_trunk": _os.environ.get("TECO_LIN_TRUNK", "0") == "1",
+_cfg = {"precision": "bf16", "train_precision": "fp32", "lin_trunk": {"1": True, "0": False}.get(_os.environ.get("TECO_LIN_TRUNK")),
         "train_tc_all": _os.environ.get("TECO_TRAIN_TC_ALL", "1") == "1", "train_forward": False}
 
 
@@ -52,17 +52,23 @@ def training_kernels(grad_enabled):
 
 
 def set_lin_trunk(on):
-    """32-pixel-wide frames (the metric configuration's 32x32 LR clips): run the generator's input conv + all residual
-    blocks as ONE launch of the multi-layer chain kernel (teco_conv3x3_lin_tc; every CTA keeps its own clips for all
-    layers), for batches of at least 8 clips.  Off by default: on an H100 the 33 per-layer launches are faster at every
-    batch measured (8 to 264 clips: 1.4x to 7.6x) -- both have one CTA per SM in flight, but the chain's CTA owns whole
-    images through all 33 layers while the per-layer kernel spreads each layer's small tiles over every SM -- so bench.py
-    times the chain next to them instead."""
-    _cfg["lin_trunk"] = bool(on)
+    """32x32 frames (the metric configuration's LR clips): whether the generator's input conv + residual blocks run as ONE
+    launch that keeps each clip's activations in shared memory (teco_conv3x3_lin_tc; a cluster of two CTAs owns a clip
+    through all 33 layers) instead of 33 per-layer launches.  None (the default, or TECO_LIN_TRUNK unset): automatic, the
+    one launch when the batch fills at least LIN_TRUNK_MIN_FILL of the rounds of G clusters it needs (G: clusters resident
+    at once, 66 on an H100 SXM), where it measured faster; True / False (TECO_LIN_TRUNK=1 / 0) force it on (for batches of
+    at least 8 clips) or off."""
+    _cfg["lin_trunk"] = None if on is None else bool(on)
 
 
 def lin_trunk():
     return _cfg["lin_trunk"]
+
+
+# A round of the one-launch trunk takes about as long whether it holds 1 or G clips, while the per-layer launches scale
+# with the batch: on an H100 SXM (700 W) the one launch was 1.20-1.32x faster at 66, 132, 198 and 264 clips (full rounds)
+# and 0.71-0.81x at 8 and 67 (1 / 8 and 1 / 2 of a round used); see tools/ab_trunk.py and DESIGN 4.1b.
+LIN_TRUNK_MIN_FILL = 0.8
 
 
 def train_tc_all():

@@ -234,109 +234,9 @@ conv3x3_wgmma_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p)
   }
 }
 
-// ------------------------------------------------------------------ multi-layer chain (generator trunk)
-// L consecutive 3x3 64 -> 64 layers (bias, ReLU / LeakyReLU / none, optional residual) on 32-pixel-wide images in ONE
-// launch.  CTA c owns images c, c + G, ... for EVERY layer, so the input tiles of layer l + 1 were written by this very
-// CTA: a CTA-wide barrier (after a generic -> async proxy fence, because the next layer's halo arrives by TMA) is the only
-// dependency between layers, there is no grid-wide one and no kernel boundary.  Weights of layer l + 1 are in flight in
-// the second weight buffer while layer l computes; within a layer the halo of the next tile is in flight while the
-// current one runs its MMAs and epilogue.  Same MMA and epilogue code as conv3x3_wgmma_kernel.
+// teco_conv3x3_lin_tc: chains of 3x3 64 -> 64 layers on 32-pixel-wide images
 constexpr int LIN_W = 32, LIN_ROWS = 4, LIN_MAX_LAYERS = 40;
 constexpr uint32_t LAYER_W_BYTES = 9u * 64u * 128u;   // one packed 64 x 64 layer: 73728
-
-struct ChainParams {
-  int N, H, L, tiles_y;
-  int8_t plan[LIN_MAX_LAYERS][4];   // input buffer, output buffer, residual buffer or -1, activation
-  __nv_bfloat16* bufs[3];
-  const uint8_t* wpk;
-  const float* bias;
-};
-
-__global__ void __launch_bounds__(NUM_THREADS, 1)
-conv3x3_chain_kernel(const __grid_constant__ CUtensorMap tmap0, const __grid_constant__ CUtensorMap tmap1,
-                     const __grid_constant__ CUtensorMap tmap2, const ChainParams p) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint8_t* ring = smem;                                   // 2 halo stages
-  uint8_t* wbuf = smem + 2 * HALO_STAGE;                  // 2 layers of weights
-  uint64_t* full = reinterpret_cast<uint64_t*>(wbuf + 2 * LAYER_W_BYTES);   // [2]
-  uint64_t* w_full = full + 2;                                              // [2]
-  const int tid = threadIdx.x, wg = tid >> 7;
-  const int G = gridDim.x;
-  const int tiles_per_image = (LIN_W / TILE_COLS) * p.tiles_y;
-  const int my_images = (int)blockIdx.x < p.N ? (p.N - (int)blockIdx.x + G - 1) / G : 0;
-  const int T = my_images * tiles_per_image;              // tiles of this CTA per layer
-  const int nsteps = p.L * T;
-
-  if (tid == 0) {
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(smem_u32(&full[i]), 1);
-      mbar_init(smem_u32(&w_full[i]), 1);
-    }
-    fence_mbar_init();
-  }
-  __syncthreads();
-  if (T == 0) return;
-
-  auto tile_coords = [&](int it, int& n, int& y0, int& x0) {
-    const int k = it / tiles_per_image, r = it - k * tiles_per_image;
-    n = (int)blockIdx.x + k * G;
-    x0 = (r % (LIN_W / TILE_COLS)) * TILE_COLS;
-    y0 = (r / (LIN_W / TILE_COLS)) * TILE_ROWS;
-  };
-  auto issue = [&](int s) {     // halo of step s = (layer s / T, tile s % T) into ring stage s & 1
-    const int l = s / T;
-    int n, y0, x0;
-    tile_coords(s - l * T, n, y0, x0);
-    const int in = p.plan[l][0];
-    const CUtensorMap* map = in == 0 ? &tmap0 : (in == 1 ? &tmap1 : &tmap2);
-    const uint32_t bar = smem_u32(&full[s & 1]);
-    mbar_expect_tx(bar, HALO_BYTES);
-    tma_load_4d(smem_u32(ring + (size_t)(s & 1) * HALO_STAGE), map, bar, 0, x0 - 1, y0 - 1, n);
-  };
-  auto issue_weights = [&](int l) {   // layer l into weight buffer l & 1
-    const uint32_t bar = smem_u32(&w_full[l & 1]);
-    mbar_expect_tx(bar, LAYER_W_BYTES);
-    for (int t = 0; t < 9; ++t)
-      bulk_load_1d(smem_u32(wbuf + (size_t)(l & 1) * LAYER_W_BYTES + t * 8192u), p.wpk + (size_t)l * LAYER_W_BYTES + t * 8192u,
-                   8192u, bar);
-  };
-  if (tid == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap0) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap1) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap2) : "memory");
-    issue_weights(0);
-    if (p.L > 1) issue_weights(1);
-    issue(0);
-  }
-
-  TcParams q = {};
-  q.H = p.H; q.W = LIN_W; q.Cout = 64;
-  float acc[1][32];
-  for (int s = 0; s < nsteps; ++s) {
-    const int l = s / T, it = s - l * T;
-    // the next tile of the same layer: its input does not change during this layer, its stage was released at the end of
-    // step s - 1.  The first tile of the next layer waits for this layer's last outputs (below).
-    if (tid == 0 && it + 1 < T) issue(s + 1);
-    if (it == 0) mbar_wait(smem_u32(&w_full[l & 1]), (uint32_t)((l >> 1) & 1));
-#pragma unroll
-    for (int r = 0; r < 32; ++r) acc[0][r] = 0.f;
-    mbar_wait(smem_u32(&full[s & 1]), (uint32_t)((s >> 1) & 1));
-    mma_block<0, 64, 1>(acc, smem_u32(ring + (size_t)(s & 1) * HALO_STAGE), smem_u32(wbuf + (size_t)(l & 1) * LAYER_W_BYTES), wg);
-    q.act = p.plan[l][3];
-    q.y = p.bufs[p.plan[l][1]];
-    q.res = p.plan[l][2] >= 0 ? p.bufs[p.plan[l][2]] : nullptr;
-    int n, y0, x0;
-    tile_coords(it, n, y0, x0);
-    epilogue<0, 64, 1>(acc, q, p.bias + 64 * l, 0, n, y0, x0);
-    if (it == T - 1) fence_proxy_async_global();   // this layer's stores -> visible to the next layer's TMA loads
-    __syncthreads();
-    if (tid == 0 && it == T - 1) {
-      if (l + 2 < p.L) issue_weights(l + 2);         // buffer l & 1 is free: every MMA of layer l has completed
-      if (s + 1 < nsteps) issue(s + 1);
-    }
-  }
-}
 
 // ------------------------------------------------------------------ warp-specialised 64 -> 64 layer (one K block)
 // Mode 0, Cin = 64, 64 output channels per CTA, bf16 output: the generator trunk, FNet's 64-channel layers and the
@@ -589,6 +489,243 @@ conv3x3_ws_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constan
   if (leader) bulk_wait_all();
 }
 
+// ------------------------------------------------------------------ generator trunk in shared memory (32 x 32 images)
+// A chain of 3x3 64 -> 64 layers on 32 x 32 images in one launch, the activations never leaving shared memory.  A cluster
+// of two CTAs (one per SM, persistent) owns clips c, c + G, ... (G clusters); CTA r of the cluster owns image rows
+// 16 r .. 16 r + 15 for every layer.
+//   - Two activation slots per CTA, each [18 rows][34 px][64 ch] bf16 in the SW128 image: the own rows, one halo row above
+//     and below, a zero column either side.  Slot 0 holds the plan's buffer 0 (x_in, read by layer 0 only) and then
+//     buffer 2; slot 1 holds buffer 1.  Layer l reads slot l & 1 and writes the other.  x_in arrives as one 4-D TMA box
+//     {64, 34, 18} at (0, -1, 16 r - 1, n), whose out-of-bounds zero fill is the padding; slot 1 is zeroed once, and rows and
+//     columns no layer writes stay zero.
+//   - The MMAs and the epilogue arithmetic are those of conv3x3_ws_kernel<0>, so the results are bit-identical to it: per
+//     16 x 8 tile one m64n128k16 accumulator, the weight tap as A and the slot at the tap's offset as B (8-pixel groups one
+//     34-pixel row apart), taps 0..8 x K-steps 0..3, scale-d = 0 first; bias -> activation -> (+ bf16 residual) -> bf16.
+//     Consumer warpgroup g owns column strips 2 g and 2 g + 1 (two accumulators) and issues tap-outer, alternating
+//     between them, one commit group per tap.
+//   - One producer warp streams the taps of every layer through a ring of TR_WSLOTS 8 KB slots; a slot is released once
+//     wgmma.wait_group shows its tap's MMAs complete in both warpgroups (one arrival per consumer warp).
+//   - The epilogue stmatrix-es the bf16 outputs straight into the other slot (an in-place residual is ldmatrix-ed from the
+//     same place first); the 128-byte swizzle chunk is taken from the address, as the TMA and the MMAs apply it.  After
+//     a generic -> async proxy fence and a barrier over the consumers, one thread bulk-copies the CTA's boundary row into
+//     the partner's halo row of the same slot (16 rows x 4352 B is a multiple of 1024: the swizzled bytes copy unchanged),
+//     completing on the partner's row_full[slot] mbarrier.
+//   - After a clip's last layer the consumers copy the CTA's own 16 rows of each slot the plan wrote to global memory with
+//     16-byte stores (un-swizzling the address); after a barrier one thread loads the next clip's x_in into slot 0.
+// Lock step: a CTA's layer l reads the partner's layer l - 1 row, which the partner sends only after all of its layer
+// l - 1 MMAs (both warpgroups waited for them before their epilogues) -- and those needed this CTA's layer l - 2 row.
+// Hence (a) when this CTA's layer-l row lands in the partner's slot, the partner has finished reading that slot (its layer
+// l - 1 input); (b) the source row of this CTA's layer-l copy is rewritten at layer l + 2 only after the partner received
+// it, so the copy has read it; (c) row_full[s] completes one phase per two layers, the next copy into slot s needing the
+// row this CTA sends after waiting for the current one.  Across clips the partner's first copy (layer 0, slot 1) waits on
+// peer_free, which this CTA arrives on remotely once it has waited for the partner's last row of the clip.
+constexpr int TR_COLS = LIN_W + 2;                                        // 34: a zero column either side
+constexpr int TR_ROWS = 16 + 2;                                           // own rows + a halo row above and below
+constexpr uint32_t TR_ROW_BYTES = TR_COLS * 128u;                         // 4352: wgmma SBO between tile rows
+constexpr uint32_t TR_SLOT = (TR_ROWS * TR_ROW_BYTES + 1023u) & ~1023u;   // 78848: slots start on the swizzle period
+constexpr int TR_WSLOTS = 8;                                              // weight ring depth (taps)
+constexpr uint32_t TR_TAP = 64u * 128u;                                   // one packed tap [64 cout][64 cin]
+constexpr uint32_t TR_EDGE_BYTES = LIN_W * 128u;                          // one boundary row without its zero columns
+constexpr int TR_BARS = 2 * TR_WSLOTS + 4;                                // full[], empty[], row_full[2], x_full, peer_free
+constexpr size_t TR_SMEM = 1024 + 2 * (size_t)TR_SLOT + TR_WSLOTS * (size_t)TR_TAP + TR_BARS * sizeof(uint64_t);
+static_assert(TR_SMEM <= SMEM_MAX, "conv3x3_trunk_cluster_kernel: shared memory budget");
+static_assert((16 * TR_ROW_BYTES) % 1024 == 0, "a boundary row and the partner's halo row share their swizzle phase");
+
+struct TrunkParams {
+  int N, L;
+  uint64_t res_mask;                 // bit l: layer l adds its output buffer's previous value (in place)
+  uint64_t relu_mask, lrelu_mask;    // bit l: layer l's activation (neither: none)
+  const uint8_t* wpk;                // L packed layers back to back
+  const float* bias;                 // [L][64]
+  __nv_bfloat16* a;                  // buffer 1 (slot 1)
+  __nv_bfloat16* b;                  // buffer 2 (slot 0 after layer 0)
+};
+
+// The CTA's own rows y0 .. y0 + 15 of image n in the slot at `slot` -> dst [N,32,32,64]: consecutive threads store
+// consecutive 16-byte chunks of global memory, chunk q of slot pixel P read from chunk q ^ (P & 7).
+__device__ __forceinline__ void trunk_store_rows(uint32_t slot, __nv_bfloat16* dst, int n, int y0, int tid) {
+  uint4* out = reinterpret_cast<uint4*>(dst + ((size_t)n * LIN_W + y0) * LIN_W * 64);
+#pragma unroll 4
+  for (int c = tid; c < 16 * LIN_W * 8; c += NUM_THREADS) {
+    const int px = c >> 3, q = c & 7;
+    const int P = (1 + px / LIN_W) * TR_COLS + 1 + px % LIN_W;
+    uint4 v;
+    asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];"
+                 : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w)
+                 : "r"(slot + (uint32_t)(P * 128 + ((q ^ (P & 7)) << 4))));
+    out[c] = v;
+  }
+}
+
+// Epilogue of one 16 x 8 tile at column x0 of the CTA's rows, into the slot at `slot`: ws_epilogue<ACT, 0> with the tile's
+// pixel (row R, column C) at slot pixel P = (1 + R) * 34 + 1 + x0 + C, chunk q at q ^ (P & 7).
+template <int ACT>
+__device__ __forceinline__ void trunk_epilogue(const float (&acc)[64], const float (&b)[2], uint32_t slot, int x0, bool res,
+                                               int wq, int lane) {
+  const int q = 2 * wq + ((lane >> 3) & 1);
+  const int p0 = (1 + (lane >> 4)) * TR_COLS + 1 + x0 + (lane & 7);
+#pragma unroll
+  for (int jj = 0; jj < TILE_ROWS / 2; ++jj) {
+    const int px = p0 + 2 * jj * TR_COLS;
+    const uint32_t a = slot + (uint32_t)(px * 128 + ((q ^ (px & 7)) << 4));
+    uint32_t r[4];
+    if (res) ldmatrix_x4_trans(r, a);
+#pragma unroll
+    for (int m = 0; m < 4; ++m) {
+      const int j = 2 * jj + (m >> 1), i = m & 1;
+      float v0 = teco_act(acc[4 * j + 2 * i] + b[i], ACT);
+      float v1 = teco_act(acc[4 * j + 2 * i + 1] + b[i], ACT);
+      if (res) {
+        const float2 rf = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&r[m]));
+        v0 += rf.x;
+        v1 += rf.y;
+      }
+      const __nv_bfloat162 o = __floats2bfloat162_rn(v0, v1);
+      r[m] = *reinterpret_cast<const uint32_t*>(&o);
+    }
+    stmatrix_x4_trans(a, r);
+  }
+}
+
+template <int ACT>
+__device__ __forceinline__ void trunk_epilogue2(const float (&acc0)[64], const float (&acc1)[64], const float (&b)[2],
+                                                uint32_t slot, int x0, bool res, int wq, int lane) {
+  trunk_epilogue<ACT>(acc0, b, slot, x0, res, wq, lane);
+  trunk_epilogue<ACT>(acc1, b, slot, x0 + TILE_COLS, res, wq, lane);
+}
+
+__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(WS_THREADS, 1)
+conv3x3_trunk_cluster_kernel(const __grid_constant__ CUtensorMap xmap, const TrunkParams p) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  uint8_t* wring = smem + 2 * (size_t)TR_SLOT;
+  uint64_t* full = reinterpret_cast<uint64_t*>(wring + TR_WSLOTS * (size_t)TR_TAP);   // [TR_WSLOTS]
+  uint64_t* empty = full + TR_WSLOTS;                                                 // [TR_WSLOTS]
+  uint64_t* row_full = empty + TR_WSLOTS;        // [2]: the partner's boundary row has landed in slot s
+  uint64_t* x_full = row_full + 2;               // x_in of the clip has landed in slot 0
+  uint64_t* peer_free = x_full + 1;              // the partner has taken this CTA's last row of the previous clip
+
+  const int tid = threadIdx.x, wg = tid >> 7;
+  const uint32_t rank = cluster_ctarank(), peer = rank ^ 1u;
+  const int cl = (int)blockIdx.x >> 1, G = (int)gridDim.x >> 1;
+  const int my_clips = cl < p.N ? (p.N - cl + G - 1) / G : 0;
+
+  if (tid == 0) {
+    for (int s = 0; s < TR_WSLOTS; ++s) {
+      mbar_init(smem_u32(&full[s]), 1);
+      mbar_init(smem_u32(&empty[s]), 8);         // one arrival per consumer warp
+    }
+    for (int i = 0; i < 4; ++i) mbar_init(smem_u32(&row_full[i]), 1);   // row_full[2], x_full, peer_free
+    fence_mbar_init();
+  }
+  for (uint32_t i = tid; i < TR_SLOT / 16; i += WS_THREADS)    // slot 1 is never TMA-loaded: its padding is zeroed here
+    asm volatile("st.shared.v4.u32 [%0], {%1, %1, %1, %1};" ::"r"(smem_u32(smem + TR_SLOT) + 16 * i), "r"(0) : "memory");
+  fence_async_smem();
+  cluster_sync();                                // both CTAs' barriers are initialised before any remote access
+
+  if (wg == 2) {                                 // producer warp: one lane streams every tap of every layer and clip
+    if (tid == NUM_THREADS) {
+      const int per_clip = 9 * p.L, total = my_clips * per_clip;
+      for (int q = 0, lt = 0; q < total; ++q, lt = lt + 1 == per_clip ? 0 : lt + 1) {
+        const int s = q % TR_WSLOTS;
+        if (q >= TR_WSLOTS) mbar_wait(smem_u32(&empty[s]), (uint32_t)((q / TR_WSLOTS - 1) & 1));
+        mbar_expect_tx(smem_u32(&full[s]), TR_TAP);
+        bulk_load_1d(smem_u32(wring + s * TR_TAP), p.wpk + (size_t)lt * TR_TAP, TR_TAP, smem_u32(&full[s]));
+      }
+    }
+    __syncwarp();
+    cluster_sync();
+    return;
+  }
+
+  const int wq = (tid >> 5) & 3, lane = tid & 31;
+  const uint32_t slot0 = smem_u32(smem), wring_a = smem_u32(wring);
+  const int y0 = 16 * (int)rank;                 // first image row of this CTA
+  // this CTA's boundary row (buffer row 16 for r = 0, 1 for r = 1) -> the partner's halo row (0, resp. 17); column 1 on
+  const uint32_t edge_src = (rank == 0 ? 16u : 1u) * TR_ROW_BYTES + 128u;
+  const uint32_t edge_dst = (rank == 0 ? 0u : 17u) * TR_ROW_BYTES + 128u;
+  const int xa = 2 * TILE_COLS * wg;             // strips 2 wg and 2 wg + 1 start at columns xa and xa + 8
+  auto load_x = [&](int n) {
+    mbar_expect_tx(smem_u32(x_full), TR_ROWS * TR_ROW_BYTES);
+    tma_load_4d(slot0, &xmap, smem_u32(x_full), 0, -1, y0 - 1, n);
+  };
+  if (tid == 0 && my_clips > 0) {
+    asm volatile("prefetch.tensormap [%0];" ::"l"(&xmap) : "memory");
+    load_x(cl);
+  }
+
+  float acc0[64], acc1[64];
+  uint32_t q = 0;                                // taps consumed
+  uint32_t row_par = 0;                          // bit s: phase parity of row_full[s]
+  for (int k = 0; k < my_clips; ++k) {
+    const int n = cl + k * G;
+    for (int l = 0; l < p.L; ++l) {
+      const uint32_t si = (uint32_t)l & 1u, so = si ^ 1u;
+      if (l == 0) {
+        mbar_wait(smem_u32(x_full), (uint32_t)k & 1u);
+      } else {
+        mbar_wait(smem_u32(&row_full[si]), (row_par >> si) & 1u);
+        row_par ^= 1u << si;
+      }
+      const float* bl = p.bias + 64 * l;
+      const float b[2] = {bl[16 * wq + (lane >> 2)], bl[16 * wq + 8 + (lane >> 2)]};
+      const uint32_t in_a = slot0 + si * TR_SLOT + (uint32_t)xa * 128u;
+#pragma unroll
+      for (int t = 0; t < 9; ++t, ++q) {
+        const uint32_t s = q % TR_WSLOTS;
+        mbar_wait(smem_u32(&full[s]), (q / TR_WSLOTS) & 1u);
+        wgmma_fence();
+        const uint32_t a0 = wring_a + s * TR_TAP;
+        const uint32_t b0 = in_a + (uint32_t)(((t / 3) * TR_COLS + t % 3) * 128);
+#pragma unroll
+        for (int kk = 0; kk < CB / 16; ++kk)
+          Wgmma<128, 0, 0>::run(acc0, gmma_desc_sw128(a0 + 32u * kk, 16u, 1024u), gmma_desc_sw128(b0 + 32u * kk, 16u, TR_ROW_BYTES),
+                                t == 0 && kk == 0 ? 0u : 1u);
+#pragma unroll
+        for (int kk = 0; kk < CB / 16; ++kk)
+          Wgmma<128, 0, 0>::run(acc1, gmma_desc_sw128(a0 + 32u * kk, 16u, 1024u),
+                                gmma_desc_sw128(b0 + TILE_COLS * 128u + 32u * kk, 16u, TR_ROW_BYTES), t == 0 && kk == 0 ? 0u : 1u);
+        wgmma_commit();
+        if (t > 0) {
+          wgmma_wait<1>();                       // tap t - 1 has completed in this warpgroup
+          mbar_arrive_if(smem_u32(&empty[(q - 1) % TR_WSLOTS]), lane == 0);
+        }
+      }
+      wgmma_wait_all_fence(acc0);
+      wgmma_wait_all_fence(acc1);
+      if (lane == 0) mbar_arrive(smem_u32(&empty[(q - 1) % TR_WSLOTS]));
+
+      const uint32_t out_a = slot0 + so * TR_SLOT;
+      const bool res = (p.res_mask >> l) & 1u;
+      // once per layer: the element loop is compiled per activation
+      if ((p.relu_mask >> l) & 1u) trunk_epilogue2<TECO_ACT_RELU>(acc0, acc1, b, out_a, xa, res, wq, lane);
+      else if ((p.lrelu_mask >> l) & 1u) trunk_epilogue2<TECO_ACT_LRELU02>(acc0, acc1, b, out_a, xa, res, wq, lane);
+      else trunk_epilogue2<TECO_ACT_NONE>(acc0, acc1, b, out_a, xa, res, wq, lane);
+      fence_async_smem();                        // the stmatrix writes -> visible to the MMAs and the bulk copies
+      named_bar_sync(1, NUM_THREADS);            // the whole layer is in slot so (and every MMA on slot si is done)
+      if (tid == 0) {
+        mbar_expect_tx(smem_u32(&row_full[so]), TR_EDGE_BYTES);   // the partner's row of this layer
+        if (l == 0 && k > 0) mbar_wait(smem_u32(peer_free), (uint32_t)(k - 1) & 1u);
+        bulk_copy_to_peer(mapa_shared(out_a + edge_dst, peer), out_a + edge_src, TR_EDGE_BYTES,
+                          mapa_shared(smem_u32(&row_full[so]), peer));
+      }
+    }
+    // the partner's row of the last layer: no layer reads it, but its copy must have landed before the slot is reused
+    const uint32_t sf = (uint32_t)((p.L - 1) & 1) ^ 1u;
+    mbar_wait(smem_u32(&row_full[sf]), (row_par >> sf) & 1u);
+    row_par ^= 1u << sf;
+    trunk_store_rows(slot0 + TR_SLOT, p.a, n, y0, tid);
+    if (p.L > 1) trunk_store_rows(slot0, p.b, n, y0, tid);
+    fence_async_smem();                          // these generic reads before the next clip's TMA and bulk-copy writes
+    named_bar_sync(1, NUM_THREADS);
+    if (tid == 0 && k + 1 < my_clips) {
+      mbar_arrive_peer(mapa_shared(smem_u32(peer_free), peer));
+      load_x(n + G);
+    }
+  }
+  cluster_sync();                                // no CTA leaves while its partner may still address its shared memory
+}
+
 // ------------------------------------------------------------------ weight packing
 // out[blk][tap][cout_pad][64] bf16 in the SWIZZLE_128B image (16-byte chunk j of row r stored at chunk j ^ (r & 7))
 //   <- w[3,3,cin,cout] (or [3,3,cout,cin] when transpose_layout); packed input channel k reads cin_perm[k] (-1 = zero).
@@ -749,6 +886,65 @@ int launch_conv3x3(const teco_tc_desc* d, const void* x, const void* wpk, const 
   return TECO_OK;
 }
 
+// The plans conv3x3_trunk_cluster_kernel runs: 32 x 32 images; layer 0 reads x_in (buffer 0) into buffer 1 without a
+// residual; every later layer reads the previous layer's output and writes the other one of buffers 1 and 2, with no
+// residual or an in-place one on a buffer an earlier layer wrote.  So layer l writes buffer 1 (slot 1) for even l and
+// buffer 2 (slot 0) for odd l, and no layer reads a buffer's contents from before the launch except x_in.
+bool trunk_plan_fits(int H, int W, int L, const int32_t* plan) {
+  if (H != LIN_W || W != LIN_W || L < 1 || L > LIN_MAX_LAYERS) return false;
+  for (int l = 0; l < L; ++l) {
+    const int32_t* pl = plan + 4 * l;
+    const int in = l == 0 ? 0 : (l & 1 ? 1 : 2), out = l & 1 ? 2 : 1;
+    if (pl[0] != in || pl[1] != out || pl[3] < 0 || pl[3] >= TECO_ACT_TANH24) return false;
+    if (pl[2] != -1 && !(pl[2] == out && (out == 1 ? l >= 2 : l >= 3))) return false;
+  }
+  return true;
+}
+
+// Clusters of conv3x3_trunk_cluster_kernel resident at once on this device (cached).
+int trunk_clusters(int* G) {
+  static int cached = 0;
+  if (!cached) {
+    TECO_CUDA_CALL(cudaFuncSetAttribute(conv3x3_trunk_cluster_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TR_SMEM));
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(2 * (unsigned)teco_sm_count());
+    cfg.blockDim = dim3(WS_THREADS);
+    cfg.dynamicSmemBytes = TR_SMEM;
+    int n = 0;
+    TECO_CUDA_CALL(cudaOccupancyMaxActiveClusters(&n, conv3x3_trunk_cluster_kernel, &cfg));
+    if (n < 1) {
+      teco_set_error("conv3x3_trunk_cluster_kernel: no cluster of two CTAs with %zu bytes of shared memory each fits", TR_SMEM);
+      return TECO_E_CUDA;
+    }
+    cached = n;
+  }
+  *G = cached;
+  return TECO_OK;
+}
+
+int launch_trunk(int N, int L, const void* x_in, void* buf_a, void* buf_b, const void* wpk_all, const float* bias_all,
+                 const int32_t* plan, cudaStream_t stream) {
+  TrunkParams p = {};
+  p.N = N; p.L = L;
+  for (int l = 0; l < L; ++l) {
+    if (plan[4 * l + 3] == TECO_ACT_RELU) p.relu_mask |= 1ull << l;
+    if (plan[4 * l + 3] == TECO_ACT_LRELU02) p.lrelu_mask |= 1ull << l;
+    if (plan[4 * l + 2] >= 0) p.res_mask |= 1ull << l;
+  }
+  p.wpk = (const uint8_t*)wpk_all; p.bias = bias_all;
+  p.a = (__nv_bfloat16*)buf_a; p.b = (__nv_bfloat16*)buf_b;
+  CUtensorMap xmap;                 // one CTA's slot: 18 rows x 34 pixels x 64 channels
+  const int rc_map = encode_halo_map(&xmap, x_in, N, LIN_W, LIN_W, 64, "teco_conv3x3_lin_tc", TR_COLS, TR_ROWS);
+  if (rc_map != TECO_OK) return rc_map;
+  int G = 0;
+  const int rc = trunk_clusters(&G);
+  if (rc != TECO_OK) return rc;
+  const unsigned grid = 2u * (unsigned)(N < G ? N : G);
+  conv3x3_trunk_cluster_kernel<<<grid, WS_THREADS, TR_SMEM, stream>>>(xmap, p);
+  TECO_CUDA_LAUNCH_CHECK("teco_conv3x3_lin_tc");
+  return TECO_OK;
+}
+
 }  // namespace
 
 extern "C" int64_t teco_packed_weight_bytes(int32_t cin_pad, int32_t cout_pad) {
@@ -797,29 +993,32 @@ extern "C" int teco_conv3x3_lin_tc(int32_t N, int32_t H, int32_t W, int32_t num_
   TECO_CHECK_ARG((((uintptr_t)x_in) & 15) == 0 && (((uintptr_t)buf_a) & 15) == 0 && (((uintptr_t)buf_b) & 15) == 0 &&
                      (((uintptr_t)wpk_all) & 15) == 0,
                  "teco_conv3x3_lin_tc: tensors must be 16-byte aligned");
-  ChainParams p = {};
-  p.N = N; p.H = H; p.L = num_layers; p.tiles_y = teco_ceil_div(H, TILE_ROWS);
   for (int l = 0; l < num_layers; ++l) {
     const int32_t* pl = plan_host + 4 * l;
     TECO_CHECK_ARG(pl[0] >= 0 && pl[0] <= 2 && (pl[1] == 1 || pl[1] == 2) && pl[0] != pl[1] && pl[2] >= -1 && pl[2] <= 2 &&
                        pl[3] >= 0 && pl[3] < TECO_ACT_TANH24,
                    "teco_conv3x3_lin_tc: bad plan row %d {%d, %d, %d, %d}", l, pl[0], pl[1], pl[2], pl[3]);
-    for (int k = 0; k < 4; ++k) p.plan[l][k] = (int8_t)pl[k];
   }
-  p.bufs[0] = (__nv_bfloat16*)const_cast<void*>(x_in); p.bufs[1] = (__nv_bfloat16*)buf_a; p.bufs[2] = (__nv_bfloat16*)buf_b;
-  p.wpk = (const uint8_t*)wpk_all; p.bias = bias_all;
-  CUtensorMap maps[3];
-  for (int i = 0; i < 3; ++i) {
-    const int rc = encode_halo_map(&maps[i], p.bufs[i], N, H, LIN_W, 64, "teco_conv3x3_lin_tc");
+  if (trunk_plan_fits(H, W, num_layers, plan_host))
+    return launch_trunk(N, num_layers, x_in, buf_a, buf_b, wpk_all, bias_all, plan_host, (cudaStream_t)stream);
+  // any other plan or height: one conv3x3_ws_kernel<0> launch per layer
+  void* bufs[3] = {const_cast<void*>(x_in), buf_a, buf_b};
+  for (int l = 0; l < num_layers; ++l) {
+    const int32_t* pl = plan_host + 4 * l;
+    const teco_tc_desc d = {N, H, W, 64, 64, pl[3], 0, 0, 1.f, 0.f};
+    const int rc = launch_conv3x3(&d, bufs[pl[0]], (const uint8_t*)wpk_all + (size_t)l * LAYER_W_BYTES, bias_all + 64 * l,
+                                  pl[2] >= 0 ? bufs[pl[2]] : nullptr, bufs[pl[1]], nullptr, nullptr, (cudaStream_t)stream);
     if (rc != TECO_OK) return rc;
   }
-  const size_t smem = 1024 + 2 * (size_t)HALO_STAGE + 2 * (size_t)LAYER_W_BYTES + 64;
-  int per_sm = 0;
-  const int rc = resident_ctas((const void*)conv3x3_chain_kernel, smem, &per_sm);
-  if (rc != TECO_OK) return rc;
-  const long long slots = (long long)per_sm * teco_sm_count();
-  const unsigned grid = (unsigned)(N < slots ? N : slots);
-  conv3x3_chain_kernel<<<grid, NUM_THREADS, smem, (cudaStream_t)stream>>>(maps[0], maps[1], maps[2], p);
-  TECO_CUDA_LAUNCH_CHECK("teco_conv3x3_lin_tc");
   return TECO_OK;
+}
+
+extern "C" int teco_conv3x3_lin_in_smem(int32_t N, int32_t H, int32_t W, int32_t num_layers, const int32_t* plan_host) {
+  return plan_host && teco_conv3x3_lin_supported(N, H, W, num_layers) && trunk_plan_fits(H, W, num_layers, plan_host) ? 1 : 0;
+}
+
+extern "C" int teco_conv3x3_lin_clusters(void) {
+  int G = 0;
+  const int rc = trunk_clusters(&G);
+  return rc == TECO_OK ? G : rc;
 }

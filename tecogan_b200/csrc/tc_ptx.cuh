@@ -50,6 +50,12 @@ __device__ __forceinline__ void bulk_load_1d(uint32_t dst, const void* src, uint
 __device__ __forceinline__ void mbar_arrive(uint32_t bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
+// mbar_arrive by the threads with pred set, without a branch (a divergent path between wgmmas serialises them)
+__device__ __forceinline__ void mbar_arrive_if(uint32_t bar, bool pred) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %1, 0;\n\t@p mbarrier.arrive.shared::cta.b64 _, [%0];\n\t}" ::"r"(bar),
+               "r"((uint32_t)pred)
+               : "memory");
+}
 // shared -> global tensor store (out-of-bounds elements of the box are not written), tracked by bulk async-groups
 __device__ __forceinline__ void tma_store_4d(const CUtensorMap* map, uint32_t src, int c0, int c1, int c2, int c3) {
   asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
@@ -84,9 +90,39 @@ __device__ __forceinline__ uint64_t gmma_desc_sw128(uint32_t saddr, uint32_t lbo
          ((uint64_t)((sbo >> 4) & 0x3FFFu) << 32) | (1ull << 62);
 }
 
+// ---- thread-block clusters: distributed shared memory
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+  return r;
+}
+// the shared::cluster address of this CTA's shared::cta address `addr` in CTA `rank` of the cluster
+__device__ __forceinline__ uint32_t mapa_shared(uint32_t addr, uint32_t rank) {
+  uint32_t r;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(rank));
+  return r;
+}
+// every thread of every CTA of the cluster: arrive (release) and wait (acquire)
+__device__ __forceinline__ void cluster_sync() {
+  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+// shared::cta -> another CTA's shared memory (dst and bar: shared::cluster addresses); completes bytes on bar
+__device__ __forceinline__ void bulk_copy_to_peer(uint32_t dst, uint32_t src, uint32_t bytes, uint32_t bar) {
+  asm volatile("cp.async.bulk.shared::cluster.shared::cta.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst),
+               "r"(src), "r"(bytes), "r"(bar)
+               : "memory");
+}
+// arrive (release at cluster scope) on an mbarrier of another CTA of the cluster (bar: shared::cluster address)
+__device__ __forceinline__ void mbar_arrive_peer(uint32_t bar) {
+  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(bar) : "memory");
+}
+
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// all but the newest N committed wgmma groups of this warpgroup have completed
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 // wgmma_wait_all() for a register array the compiler must not move across the wait (the asm names it as read and written)
 template <int R>
 __device__ __forceinline__ void wgmma_wait_all_fence(float (&d)[R]) {

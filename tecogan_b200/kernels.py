@@ -516,18 +516,39 @@ def conv3x3_lin_supported(N, H, W, num_layers):
     return bool(lib().teco_conv3x3_lin_supported(N, H, W, num_layers))
 
 
-def conv3x3_lin_chain(x_in, buf_a, buf_b, wpk_all, bias_all, plan):
-    """A chain of 3x3 64->64 layers on 32-pixel-wide images in one launch (teco_conv3x3_lin_tc).  x_in / buf_a / buf_b:
-    [N,H,32,64] bf16 (buffer ids 0 / 1 / 2); plan: list of (input id, output id, residual id or -1, activation) per layer;
-    wpk_all: the packed layers back to back; bias_all: [L,64] fp32."""
+def _flat_plan(plan):
     import ctypes
+    flat = (ctypes.c_int32 * (4 * len(plan)))(*[int(v) for row in plan for v in row])
+    return ctypes.cast(flat, ctypes.c_void_p), flat
+
+
+def conv3x3_lin_in_smem(N, H, W, plan):
+    """True when conv3x3_lin_chain runs `plan` as one launch with the activations in shared memory (32x32 images, a
+    generator-trunk-shaped plan); otherwise it issues one launch per layer."""
+    from ._ffi import lib
+    p, _keep = _flat_plan(plan)
+    return bool(lib().teco_conv3x3_lin_in_smem(N, H, W, len(plan), p))
+
+
+def conv3x3_lin_clusters():
+    """Clusters of the one-launch trunk resident at once on the current device (its persistent grid)."""
+    from ._ffi import lib
+    g = lib().teco_conv3x3_lin_clusters()
+    if g <= 0:
+        raise RuntimeError("teco_conv3x3_lin_clusters failed (%d): %s" % (g, lib().teco_last_error().decode()))
+    return g
+
+
+def conv3x3_lin_chain(x_in, buf_a, buf_b, wpk_all, bias_all, plan):
+    """A chain of 3x3 64->64 layers on 32-pixel-wide images (teco_conv3x3_lin_tc).  x_in / buf_a / buf_b: [N,H,32,64] bf16
+    (buffer ids 0 / 1 / 2); plan: list of (input id, output id, residual id or -1, activation) per layer; wpk_all: the
+    packed layers back to back; bias_all: [L,64] fp32."""
     N, H, W, C = x_in.shape
     if C != 64:
         raise ValueError("conv3x3_lin_chain: 64-channel NHWC bf16 tensors only (got %d channels)" % C)
-    L = len(plan)
-    flat = (ctypes.c_int32 * (4 * L))(*[int(v) for row in plan for v in row])
-    call("teco_conv3x3_lin_tc", N, H, W, L, ptr(x_in, bf16), ptr(buf_a, bf16), ptr(buf_b, bf16), ptr(wpk_all, bf16),
-         ptr(bias_all, f32), ctypes.cast(flat, ctypes.c_void_p), stream_ptr())
+    p, _keep = _flat_plan(plan)
+    call("teco_conv3x3_lin_tc", N, H, W, len(plan), ptr(x_in, bf16), ptr(buf_a, bf16), ptr(buf_b, bf16), ptr(wpk_all, bf16),
+         ptr(bias_all, f32), p, stream_ptr())
 
 
 def f32_to_bf16_pad(src, dst, C, c_off=0, scale=1.0, shift=0.0):

@@ -126,15 +126,23 @@ class GeneratorPlan:
         self.bic = torch.zeros((B, 4 * h, 4 * w, 3), device=device, dtype=f32)
         self.out = torch.zeros((B, 4 * h, 4 * w, 3), device=device, dtype=f32)
         self.launches = 2 * num_resblock + 5 + 1
-        # 32-pixel-wide frames in a batch: the whole trunk can run as one launch of the multi-layer chain kernel (opt-in,
-        # config.set_lin_trunk; bench.py times it against the per-layer launches)
-        self.lin = config.lin_trunk() and B >= 8 and K.conv3x3_lin_supported(B, h, w, 2 * num_resblock + 1)
-        if K.conv3x3_lin_supported(B, h, w, 2 * num_resblock + 1):
+        # 32-pixel-wide frames: the whole trunk can run as one teco_conv3x3_lin_tc call; on 32x32 frames that is one
+        # launch with the activations in shared memory, chosen from the batch unless config.set_lin_trunk forces it
+        L = 2 * num_resblock + 1
+        self.lin = False
+        if K.conv3x3_lin_supported(B, h, w, L):
             layers = [self.l_in] + [l for pair in self.l_res for l in pair]
             self.trunk_w = torch.cat([l.wpk for l in layers]).contiguous()
             self.trunk_b = torch.cat([l.bias for l in layers]).contiguous()
             # buffer ids: 0 = x_in, 1 = a, 2 = b.  input conv x_in -> a (ReLU); block: a -> b (ReLU), b -> a (+ a)
             self.trunk_plan = [(0, 1, -1, ACT_RELU)] + [(1, 2, -1, ACT_RELU), (2, 1, 1, ACT_NONE)] * num_resblock
+            forced = config.lin_trunk()
+            if forced is None:
+                G = K.conv3x3_lin_clusters()
+                self.lin = (K.conv3x3_lin_in_smem(B, h, w, self.trunk_plan) and
+                            B >= config.LIN_TRUNK_MIN_FILL * G * -(-B // G))
+            else:
+                self.lin = forced and B >= 8
         if self.lin:
             self.launches = 1 + 4 + 1
 
