@@ -172,6 +172,13 @@ int teco_depth_to_space4_f32(const float* y, float* x, int32_t N, int32_t h, int
 /* tf_data_gaussDownby4 lib/ops.py:347-367: 9x9 sigma-1.5 Gaussian, stride 4, VALID, per channel. */
 int teco_gauss_down4_f32(const float* hr, float* lr, int32_t N, int32_t H, int32_t W, int32_t C, void* stream);
 
+/* Training clips from the device-resident frame store (the pixel half of loadHR, lib/dataloader.py:206-258:
+ * random crop, left-right flip, tf.image.convert_image_dtype).  store: uint8 RGB frames back to back.
+ * table: n rows of int64 {byte offset of the crop's top-left pixel, row pitch in bytes, flip}.
+ *   out[i, y, x, c] = store[table[i][0] + y * table[i][1] + 3 * (flip ? S-1-x : x) + c] / 255   (fp32, correctly rounded)
+ * out: [n, S, S, 3] fp32.  The caller keeps every crop inside its frame; 0 < n <= 65535. */
+int teco_gather_clips_u8(const uint8_t* store, const int64_t* table, int32_t n, int32_t S, float* out, void* stream);
+
 /* generic elementwise y = f(a*x + b) with f in TECO_ACT_*; n elements. preprocess/deprocess lib/ops.py:13-22 */
 int teco_affine_act_f32(const float* x, float* y, int64_t n, float a, float b, int32_t act, void* stream);
 /* dx = dy * act'(pre) expressed on the activation OUTPUT y (relu/lrelu/tanh24/sigmoid are invertible enough). */

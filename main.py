@@ -11,7 +11,10 @@ Differences forced by the environment, stated once:
     augmentations (tecogan_b200/lib/dataloader.py::HRClipLoader, after lib/dataloader.py:147-273) instead of TF queue
     runners; an empty flag raises as in the reference unless --synthetic_data is given (seeded synthetic HR clips and,
     without --vgg_ckpt, a seeded random frozen VGG -- for benchmarks and tests only); the device half (Gaussian
-    down-sampling, crops) is the same either way;
+    down-sampling, crops) is the same either way.  When every frame of the training (and held-out) scenes fits in device
+    memory beside training, the frames are decoded once into a device-resident frame store and the clips are cut on the
+    GPU from the same draws (FrameStore; select_training_input decides after the first step), so the batches are the host
+    loader's, bit for bit;
   * --precision {bf16,fp32} selects wgmma tensor-core or fp32 CUDA-core convolutions for inference;
     --train_precision {fp32,bf16} does the same for training (default fp32, the reference's arithmetic);
   * under `torchrun` each rank trains on its own clip shard with one NCCL all-reduce per step;
@@ -285,8 +288,74 @@ def validation_source(FLAGS, dev):
         if loader is None:
             print('[main] validation skipped: %s' % why)
             return None
-        return lambda k: loader.batch(k).to(dev)
+
+        def fetch(k):
+            return loader.batch(k).to(dev)
+        fetch.loader = loader               # train() moves validation onto the frame store with it
+        return fetch
     return lambda k: synthetic_hr_batch(FLAGS, k, 0, dev, validation=True)
+
+
+def frame_store_fits(store_bytes, free_bytes, reserved_bytes, peak_bytes, total_bytes):
+    """Whether the device frame store (lib/dataloader.py::FrameStore) fits beside training: (fits, message).
+
+    The reserve is a measured peak.  train() decides after the first training step, after the test-sequence pass (at the
+    start, with --summary_dir) and after one validation pass, so `peak_bytes` (torch.cuda.max_memory_allocated) is the most
+    those passes and the model have held at once.  The process can use `free_bytes` (cudaMemGetInfo) plus what PyTorch's
+    allocator has reserved (`reserved_bytes`); the store fits when it leaves the peak and a margin of max(1 GiB, 5 % of the
+    device's `total_bytes`) -- allocator fragmentation, NCCL and library workspaces -- inside that."""
+    margin = max(1 << 30, total_bytes // 20)
+    room = free_bytes + reserved_bytes - peak_bytes - margin
+    gib = lambda b: b / float(1 << 30)
+    fits = store_bytes <= room
+    msg = ('frame store %.2f GiB %s the %.2f GiB left beside a measured peak of %.2f GiB and a %.2f GiB margin'
+           % (gib(store_bytes), 'fits in' if fits else 'does not fit in', gib(max(room, 0)), gib(peak_bytes), gib(margin)))
+    return fits, msg
+
+
+def select_training_input(FLAGS, Net, loader, val_hr, batch, next_step, dev, rank, world, monitor):
+    """After the first training step from disk: read the training (and validation) clips from a FrameStore on the device
+    when it fits (frame_store_fits; under torchrun every rank must agree), otherwise from the host loader's thread pool.
+    Either way the batches are the same, bit for bit.  Returns (next_hr, val_hr)."""
+    import torch
+    import torch.distributed as dist
+    from tecogan_b200.lib.dataloader import FrameStore, validation_loader
+    val_loader = None
+    if monitor and val_hr is not None:
+        val_loader = val_hr.loader
+        Net.train.evaluate(*batch)        # the validation pass's allocations count in the peak (nothing is written)
+    elif FLAGS.summary_dir and not monitor:
+        val_loader = validation_loader(FLAGS)[0]     # rank 0 validates: every rank stores the same scenes
+    loaders = [loader] + ([val_loader] if val_loader is not None else [])
+    torch.cuda.synchronize()
+    store_bytes = FrameStore.estimate_bytes(loaders)
+    free, total = torch.cuda.mem_get_info(dev)
+    fits, msg = frame_store_fits(store_bytes, free, torch.cuda.memory_reserved(dev), torch.cuda.max_memory_allocated(dev), total)
+    if world > 1:
+        agree = torch.tensor([1 if fits else 0], dtype=torch.int32, device=dev)
+        dist.all_reduce(agree, op=dist.ReduceOp.MIN)
+        if fits and not agree.item():
+            msg += ' on this rank, not on every rank'
+        fits = bool(agree.item())
+    if rank == 0:
+        print('[main] %s: training reads its clips from the %s' % (msg, 'frame store on the device' if fits else
+                                                                     'host loader (%d threads)' % loader.queue_thread))
+    if not fits:
+        clip_iter = loader.batches(start_step=next_step)
+        return (lambda gstep: next(clip_iter).to(dev, non_blocking=True)), val_hr
+    store = FrameStore(loaders, dev, rank=rank, world=world)
+    if rank == 0:
+        print('[main] frame store: %d frames, %.2f GiB, built in %.1f s' % (len(store.paths), store.nbytes / float(1 << 30),
+                                                                           store.build_seconds))
+    clip_iter = store.batches(start_step=next_step)
+    if val_loader is not None and val_hr is not None:
+        vstore = store.view(val_loader)
+
+        def fetch(k):
+            return vstore.batch(k)
+        fetch.loader = val_loader
+        val_hr = fetch
+    return (lambda gstep: next(clip_iter)), val_hr
 
 
 def train(FLAGS):
@@ -346,8 +415,9 @@ def train(FLAGS):
         test_while_train(FLAGS, start_step)
     tested = {start_step}
     if loader is not None:
-        clip_iter = loader.batches(start_step=start_step)
-        next_hr = lambda gstep: next(clip_iter).to(dev, non_blocking=True)
+        # the first step's batch is decoded on this thread; after that step select_training_input moves the input to
+        # the device frame store when it fits, or to the host loader's thread pool
+        next_hr = lambda gstep: loader.batch(gstep).to(dev, non_blocking=True)
     else:
         next_hr = lambda gstep: synthetic_hr_batch(FLAGS, gstep, rank, dev)   # seeded by the GLOBAL step
     frame_len = (FLAGS.RNN_N * 2 - 1) if FLAGS.pingpang else FLAGS.RNN_N
@@ -383,6 +453,9 @@ def train(FLAGS):
                 if monitor:
                     test_while_train(FLAGS, run_step)
                     tested.add(run_step)
+            if step == 0 and loader is not None:
+                next_hr, val_hr = select_training_input(FLAGS, Net, loader, val_hr if monitor else None, (lr_, tg_),
+                                                        start_step + 1, dev, rank, world, monitor)
     except KeyboardInterrupt:
         if rank == 0:
             print('main.py: KeyboardInterrupt->saving the checkpoint')

@@ -454,6 +454,16 @@ def gauss_down4(hr):
     return lr
 
 
+def gather_clips_u8(store, table, S):
+    """Frames cut from the uint8 frame store: table int64 [n, 3] CUDA rows {byte offset of the crop's top-left pixel, row
+    pitch in bytes, flip} -> fp32 [n, S, S, 3] = u8 / 255 (correctly rounded, numpy's float32 division).  The caller keeps
+    every crop inside its frame (lib/dataloader.py::FrameStore checks it against the frame table)."""
+    n = table.shape[0]
+    out = torch.empty((n, S, S, 3), device=store.device, dtype=f32)
+    call("teco_gather_clips_u8", ptr(store, torch.uint8), ptr(_cc(table), torch.int64), n, S, ptr(out, f32), stream_ptr())
+    return out
+
+
 def to_u8(x01):
     y = torch.empty(x01.shape, device=x01.device, dtype=torch.uint8)
     call("teco_to_u8", ptr(_cc(x01), f32), ptr(y, torch.uint8), x01.numel(), stream_ptr())

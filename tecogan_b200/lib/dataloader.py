@@ -3,10 +3,13 @@ frvsr_gpu_data_loader (lib/dataloader.py:306-332) and -- as the caller side of t
 HR training clips (`HRClipLoader`) that follows `loadHR` + `tf.train.shuffle_batch` (lib/dataloader.py:147-273): same
 directory layout, frame windows, moving-first-frame / random-crop / flip augmentation, a thread pool instead of TF queue
 runners.  The validation split (lib/dataloader.py:287-296) is a second `HRClipLoader` over the held-out scenes
-(`validation_loader`); it feeds the val_* summaries of main.py --mode train --summary_dir."""
+(`validation_loader`); it feeds the val_* summaries of main.py --mode train --summary_dir.  `FrameStore` is the device
+half: the frames of those scenes decoded once into device memory, the same batches cut there by teco_gather_clips_u8."""
 import collections
 import concurrent.futures
 import os
+import struct
+import time
 
 import numpy as np
 
@@ -66,6 +69,11 @@ class EmptyClipSet(ValueError):
     """The scene range holds no usable clip, or fewer samples than one batch."""
 
 
+# One sample's draws: scene index into HRClipLoader.clips, the RNN_N source frame numbers, int64 [RNN_N, 2] top-left
+# (y, x) of each frame's window in its source frame, and the left-right flip.
+ClipDraw = collections.namedtuple('ClipDraw', 'clip, frames, origin, flip')
+
+
 class HRClipLoader:
     """Host half of the training input (reference lib/dataloader.py:147-273, `loadHR`; main.py flags :60-78).
 
@@ -88,7 +96,10 @@ class HRClipLoader:
     `dirs` = (first, last) overrides str_dir..end_dir and `salt` != 0 moves every permutation and augmentation draw to a
     stream of its own: the validation loader (`validation_loader`, reference lib/dataloader.py:287-297) reads the held-out
     scenes end_dir+1..end_dir_val with the same augmentation, and its draws never repeat the training loader's.  With the
-    defaults the training batches are those of a loader without these arguments, byte for byte."""
+    defaults the training batches are those of a loader without these arguments, byte for byte.
+
+    sample() = assemble(draw()): draw() makes every random choice of a sample from the frame size alone (PNG header),
+    assemble() decodes and cuts the pixels; FrameStore cuts the same draws from frames held on the device."""
 
     def __init__(self, FLAGS, tar_size=None, rank=0, world=1, prefetch=4, dirs=None, salt=0, queue_thread=None):
         self.F = FLAGS
@@ -96,6 +107,7 @@ class HRClipLoader:
         self.rank, self.world, self.prefetch = rank, world, max(1, prefetch)
         self.salt = [int(salt)] if salt else []       # last seed word; salt 0 leaves the training seeds as they were
         self.queue_thread = int(FLAGS.queue_thread if queue_thread is None else queue_thread)
+        self._sizes, self._order_cache = {}, None
         first, last = dirs if dirs is not None else (FLAGS.str_dir, FLAGS.end_dir)
         if FLAGS.input_video_dir == '':
             raise ValueError('Video input directory input_video_dir is not provided')
@@ -124,17 +136,36 @@ class HRClipLoader:
         return self.image_count
 
     @staticmethod
-    def _read(path):
+    def decode(path):
+        """A frame as uint8 RGB [H, W, 3] (a view of cv2's BGR array); decode_png of the reference."""
         import cv2 as cv
         im = cv.imread(path, cv.IMREAD_COLOR)
         if im is None:
             raise ValueError('HRClipLoader: cannot decode ' + path)
-        return np.ascontiguousarray(im[:, :, ::-1]).astype(np.float32) / 255.0       # decode_png + convert_image_dtype
+        return im[:, :, ::-1]
 
-    def sample(self, index, epoch=0):
-        """One augmented clip [RNN_N, tar, tar, 3]; deterministic in (rand_seed, epoch, index)."""
+    def frame_path(self, clip, frame):
+        return os.path.join(self.clips[clip], 'col_high_%04d.png' % frame)
+
+    def frame_size(self, path):
+        """(height, width) of a frame, from its PNG header (a file that is not a PNG is decoded); cached per path."""
+        hw = self._sizes.get(path)
+        if hw is None:
+            with open(path, 'rb') as f:
+                head = f.read(24)
+            if len(head) == 24 and head[:8] == b'\x89PNG\r\n\x1a\n' and head[12:16] == b'IHDR':
+                w, h = struct.unpack('>II', head[16:24])
+                hw = (int(h), int(w))
+            else:
+                hw = tuple(self.decode(path).shape[:2])
+            self._sizes[path] = hw
+        return hw
+
+    def draw(self, index, epoch=0):
+        """The random half of sample(): which frames, where, flipped or not -- a ClipDraw; deterministic in
+        (rand_seed, epoch, index).  Needs the frame size only, which comes from the PNG header."""
         F, T, tar = self.F, self.F.RNN_N, self.tar_size
-        clip, start = self.clips[index // self.windows], index % self.windows
+        ci, start = index // self.windows, index % self.windows
         rng = np.random.default_rng([int(F.rand_seed) & 0x7FFFFFFF, int(epoch), int(index)] + self.salt)
         moving = False
         if F.movingFirstFrame:
@@ -143,27 +174,44 @@ class HRClipLoader:
             span = pos.max(axis=0) - pos.min(axis=0)                  # [shrink x, shrink y]
             lefttop = pos - pos.min(axis=0)
             moving = not (rng.uniform() < 0.7)
-        if moving:
-            first = self._read(os.path.join(clip, 'col_high_%04d.png' % start))
-            h, w = first.shape[0] - int(span[1]), first.shape[1] - int(span[0])
-            frames = [first[int(lefttop[t][1]):int(lefttop[t][1]) + h, int(lefttop[t][0]):int(lefttop[t][0]) + w] for t in range(T)]
-        else:
-            frames = [self._read(os.path.join(clip, 'col_high_%04d.png' % (start + t))) for t in range(T)]
         if not F.random_crop:
             raise Exception('Not implemented')      # reference :250: train data have different resolutions, crop is necessary
-        h, w = frames[0].shape[:2]
+        h, w = self.frame_size(self.frame_path(ci, start))
+        if moving:      # crops of the first frame sliding along the path, each (h - shrink y) x (w - shrink x)
+            h, w = h - int(span[1]), w - int(span[0])
+            frames, origin = (start,) * T, lefttop[:, ::-1].astype(np.int64)
+        else:
+            frames, origin = tuple(range(start, start + T)), np.zeros((T, 2), np.int64)
         if h < tar or w < tar:
-            raise ValueError('HRClipLoader: %s frames (%dx%d after augmentation) are smaller than the %d-pixel crop' % (clip, h, w, tar))
+            raise ValueError('HRClipLoader: %s frames (%dx%d after augmentation) are smaller than the %d-pixel crop'
+                             % (self.clips[ci], h, w, tar))
         off_w = int(np.floor(rng.uniform(0, float(w) - tar)))
         off_h = int(np.floor(rng.uniform(0, float(h) - tar)))
-        out = np.stack([f[off_h:off_h + tar, off_w:off_w + tar] for f in frames])
-        if getattr(F, 'flip', True) and rng.uniform() < 0.5:
+        flip = bool(getattr(F, 'flip', True) and rng.uniform() < 0.5)
+        return ClipDraw(ci, frames, origin + np.array([off_h, off_w], np.int64), flip)
+
+    def assemble(self, d):
+        """The pixel half of sample(): the tar x tar windows of a ClipDraw, flipped when drawn so, as float32 u8 / 255
+        (convert_image_dtype: numpy's correctly rounded float32 division)."""
+        tar = self.tar_size
+        img = {f: self.decode(self.frame_path(d.clip, f)) for f in sorted(set(d.frames))}
+        out = np.stack([img[f][y:y + tar, x:x + tar] for f, (y, x) in zip(d.frames, d.origin.tolist())])
+        if d.flip:
             out = out[:, :, ::-1]
-        return np.ascontiguousarray(out, dtype=np.float32)
+        return np.divide(out.astype(np.float32), np.float32(255.0))
+
+    def sample(self, index, epoch=0):
+        """One augmented clip [RNN_N, tar, tar, 3]; deterministic in (rand_seed, epoch, index)."""
+        return self.assemble(self.draw(index, epoch))
 
     def _order(self, epoch):
+        cached = self._order_cache
+        if cached is not None and cached[0] == epoch:
+            return cached[1]
         perm = np.random.default_rng([int(self.F.rand_seed) & 0x7FFFFFFF, 0x5EED, int(epoch)] + self.salt).permutation(self.image_count)
-        return perm[self.rank::self.world]
+        order = perm[self.rank::self.world]
+        self._order_cache = (epoch, order)
+        return order
 
     def _indices(self, step):
         epoch, k = divmod(step, self.steps_per_epoch)
@@ -219,3 +267,155 @@ def validation_loader(FLAGS):
     except EmptyClipSet as e:
         return None, '%s (scenes %s_%04d .. %s_%04d)' % (e, FLAGS.input_video_pre, FLAGS.end_dir + 1,
                                                          FLAGS.input_video_pre, FLAGS.end_dir_val)
+
+
+class FrameStore:
+    """Every frame of the scenes of one or more HRClipLoaders (training and held-out scenes), decoded once into one flat
+    uint8 RGB device buffer, and the batches of those loaders cut from it on the GPU.
+
+    Frame i sits at byte offsets[i] with shape sizes[i] = (H, W); sizes come from the PNG headers, so the offsets are known
+    before anything is decoded, and scenes may differ in size.  The frames are decoded on `queue_thread` host threads in
+    chunks of about `chunk_bytes` through a pinned staging buffer.  With world > 1 (an initialised torch.distributed group
+    whose backend can broadcast `device` tensors: NCCL under torchrun) rank r decodes the r-th contiguous share of the
+    frames and broadcasts it, so every rank holds the whole store after 1/world of the decoding.
+
+    batch(step) is HRClipLoader.batch(step) of the first loader, uploaded to `device`, bit for bit: the same draws
+    (HRClipLoader.draw: permutation, epochs, rank shard, salt) and the same pixels, cut by teco_gather_clips_u8.
+    view(loader) is the same store serving another of the loaders it was built from (the validation scenes)."""
+
+    def __init__(self, loaders, device, rank=0, world=1, queue_thread=None, chunk_bytes=256 << 20):
+        import torch
+        loaders = list(loaders)
+        self.loader, self.device = loaders[0], torch.device(device)
+        paths, self._bases = [], {}
+        index = {}
+        for L in loaders:
+            base = np.empty(len(L.clips), np.int64)
+            for ci in range(len(L.clips)):
+                first = L.frame_path(ci, 0)
+                if first not in index:               # a scene two loaders share is stored once
+                    index[first] = len(paths)
+                    paths += [L.frame_path(ci, f) for f in range(L.F.max_frm + 1)]
+                base[ci] = index[first]
+            self._bases[id(L)] = base
+        hw = np.array([self.loader.frame_size(p) for p in paths], np.int64).reshape(-1, 2)
+        for L in loaders[1:]:                        # the views' draws read frame sizes through their own loader
+            L._sizes.update(zip(paths, map(tuple, hw.tolist())))
+        nbytes = hw[:, 0] * hw[:, 1] * 3
+        self.sizes, self.paths = hw, paths
+        self.offsets = np.concatenate([[0], np.cumsum(nbytes)]).astype(np.int64)
+        self.nbytes = int(self.offsets[-1])
+        t0 = time.time()
+        self.buf = torch.empty(self.nbytes, dtype=torch.uint8, device=self.device)
+        shares = frame_shares(len(paths), world)
+        threads = max(1, int(self.loader.queue_thread if queue_thread is None else queue_thread))
+        self._decode(paths, *shares[rank], threads, chunk_bytes)
+        if world > 1:
+            import torch.distributed as dist
+            for r, (a, b) in enumerate(shares):
+                if b > a:
+                    dist.broadcast(self.buf[int(self.offsets[a]):int(self.offsets[b])], src=r)
+        torch.cuda.synchronize(self.device)
+        self.build_seconds = time.time() - t0
+
+    @staticmethod
+    def estimate_bytes(loaders):
+        """Bytes a FrameStore of these loaders would take, from the PNG headers alone (nothing decoded)."""
+        seen, total = set(), 0
+        for L in loaders:
+            for ci in range(len(L.clips)):
+                if L.clips[ci] in seen:
+                    continue
+                seen.add(L.clips[ci])
+                for f in range(L.F.max_frm + 1):
+                    h, w = L.frame_size(L.frame_path(ci, f))
+                    total += h * w * 3
+        return total
+
+    def _decode(self, paths, a, b, threads, chunk_bytes):
+        import torch
+        if b <= a:
+            return
+        off = self.offsets
+        stage = torch.empty(int(min(off[b] - off[a], max(chunk_bytes, int((off[a + 1:b + 1] - off[a:b]).max())))),
+                            dtype=torch.uint8).pin_memory()
+        host = stage.numpy()
+        with concurrent.futures.ThreadPoolExecutor(max_workers=threads) as pool:
+            i = a
+            while i < b:
+                j = i + 1
+                while j < b and off[j + 1] - off[i] <= stage.numel():
+                    j += 1
+
+                def put(k, i=i):
+                    im = self.loader.decode(paths[k])
+                    h, w = self.sizes[k]
+                    if im.shape[:2] != (h, w):
+                        raise ValueError('FrameStore: %s decodes to %dx%d, its header says %dx%d' % (paths[k], im.shape[0], im.shape[1], h, w))
+                    host[off[k] - off[i]:off[k + 1] - off[i]].reshape(h, w, 3)[...] = im
+                list(pool.map(put, range(i, j)))
+                self.buf[int(off[i]):int(off[j])].copy_(stage[:int(off[j] - off[i])])   # synchronous: the stage is reused
+                i = j
+
+    def view(self, loader):
+        """This store serving `loader`, one of the loaders it was built from."""
+        if id(loader) not in self._bases:
+            raise ValueError('FrameStore.view: the store was not built from this loader')
+        v = object.__new__(FrameStore)
+        v.__dict__.update(self.__dict__)
+        v.loader = loader
+        return v
+
+    def table(self, step):
+        """int64 [B * RNN_N, 3] rows of teco_gather_clips_u8 for batch `step` of this store's loader."""
+        L = self.loader
+        tar = L.tar_size
+        epoch, idx = L._indices(step)
+        base = self._bases[id(L)]
+        fid, org, flip = [], [], []
+        for i in idx:
+            d = L.draw(int(i), epoch)
+            fid.append(base[d.clip] + np.asarray(d.frames, np.int64))
+            org.append(d.origin)
+            flip.append(np.full(len(d.frames), d.flip, np.int64))
+        fid, org, flip = np.concatenate(fid), np.concatenate(org), np.concatenate(flip)
+        h, w = self.sizes[fid, 0], self.sizes[fid, 1]
+        if (org < 0).any() or (org[:, 0] + tar > h).any() or (org[:, 1] + tar > w).any():
+            bad = int(np.flatnonzero((org[:, 0] + tar > h) | (org[:, 1] + tar > w) | (org < 0).any(axis=1))[0])
+            raise ValueError('FrameStore: a %d-pixel window at %s does not fit in %s (%dx%d)'
+                             % (tar, org[bad].tolist(), self.paths[fid[bad]], h[bad], w[bad]))
+        return np.stack([self.offsets[fid] + (org[:, 0] * w + org[:, 1]) * 3, w * 3, flip], axis=1)
+
+    def _gather(self, tbl):
+        import torch
+        L = self.loader
+        t = torch.from_numpy(tbl).pin_memory().to(self.device, non_blocking=True)
+        out = K.gather_clips_u8(self.buf, t, L.tar_size)
+        return out.reshape(L.F.batch_size, L.F.RNN_N, L.tar_size, L.tar_size, 3)
+
+    def batch(self, step):
+        """Batch number `step` of the loader, fp32 [B, RNN_N, tar, tar, 3] on the device: HRClipLoader.batch(step)."""
+        return self._gather(self.table(step))
+
+    def batches(self, start_step=0, prefetch=4):
+        """Endless iterator over batch(start_step), batch(start_step + 1), ...; the draws of the next `prefetch` steps are
+        made on a worker thread while the device works."""
+        with concurrent.futures.ThreadPoolExecutor(max_workers=1) as pool:
+            pending = collections.deque(pool.submit(self.table, s) for s in range(start_step, start_step + prefetch))
+            step = start_step
+            while True:
+                tbl = pending.popleft().result()
+                pending.append(pool.submit(self.table, step + prefetch))
+                yield self._gather(tbl)
+                step += 1
+
+    def checksum(self):
+        """SHA-256 of the store's bytes (to compare the stores of several ranks)."""
+        import hashlib
+        return hashlib.sha256(self.buf.cpu().numpy().tobytes()).hexdigest()
+
+
+def frame_shares(n, world):
+    """Contiguous [a, b) frame ranges, one per rank, covering 0..n with sizes differing by at most one."""
+    cuts = [n * r // world for r in range(world + 1)]
+    return [(cuts[r], cuts[r + 1]) for r in range(world)]
