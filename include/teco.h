@@ -95,6 +95,10 @@ int teco_pack_conv3x3_bf16(const float* w, int32_t cin, int32_t cout, int32_t ci
 int64_t teco_packed_weight_bytes(int32_t cin_pad, int32_t cout_pad);
 int teco_conv3x3_tc(const teco_tc_desc* d, const void* x, const void* wpk, const float* bias,
                     const void* res, void* y, const float* res_f32, float* out_f32, void* stream);
+/* The same 3x3 SAME convolution (mode 0, bf16 output, no residual) tiled over 128 output pixels in flat N*H*W order, so a
+ * tile spans several images: for images smaller than teco_conv3x3_tc's 16 x 8 tile (FNet's 8x8 and 4x4 levels).
+ * Cin and Cout multiples of 64 in [64,512]; d->mode and d->out_f32_c must be 0.  Bit-identical to teco_conv3x3_tc. */
+int teco_conv3x3_im2col_tc(const teco_tc_desc* d, const void* x, const void* wpk, const float* bias, void* y, void* stream);
 
 /* Bias gradient of conv2() (slim.conv2d biases, reference lib/ops.py:47-56): db[c] (+)= sum over npix pixels of dy[pixel*cpitch + c]. */
 int teco_bias_grad_f32(const float* dy, float* db, int64_t npix, int32_t C, int32_t cpitch, int32_t accumulate, void* stream);

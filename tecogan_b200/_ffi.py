@@ -42,6 +42,7 @@ SIGNATURES = {
     "teco_pack_conv3x3_bf16": [_P, _I32, _I32, _I32, _I32, _I32, _P, _P, _P],
     "teco_packed_weight_bytes": [_I32, _I32],
     "teco_conv3x3_tc": [C.POINTER(TcDesc), _P, _P, _P, _P, _P, _P, _P, _P],
+    "teco_conv3x3_im2col_tc": [C.POINTER(TcDesc), _P, _P, _P, _P, _P],
     "teco_bias_grad_f32": [_P, _P, _I64, _I32, _I32, _I32, _P],
     "teco_conv3x3_wgrad_tc": [_I32, _I32, _I32, _I32, _I32, _I32, _I32, _P, _P, _P, _I32, _P],
     "teco_conv3x3_lin_supported": [_I32, _I32, _I32, _I32],

@@ -489,6 +489,142 @@ conv3x3_ws_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constan
   if (leader) bulk_wait_all();
 }
 
+// ------------------------------------------------------------------ im2col-tiled layer (images smaller than a tile)
+// Mode 0, 64-channel bf16 output slices, no residual, any Cin: FNet's 8 x 8 and 4 x 4 levels, where a 16 x 8 tile of one
+// image would be one half or one eighth full.  The tile is IC_PIX = 128 output pixels in flat N*H*W order and spans as
+// many images as it needs.
+//   - Per (64-channel K block b, tap t) one im2col-mode TMA box brings the tile's 128 input pixels at the tap's offset,
+//     64 channels each, as 128-byte SWIZZLE_128B rows: the map's bounding box (corners -1, -1) walks the output pixels in
+//     flat order and each pixel is read at (x - 1 + kx, y - 1 + ky); the zero fill outside every image is the 'SAME'
+//     padding, and past the last image it feeds pixels whose outputs are not stored.  Pixel row p of the box is row p of
+//     the K-major B operand (8-row groups 1024 B apart).
+//   - MMAs as conv3x3_ws_kernel<0>: M = the CTA's 64 output channels (blockIdx.y), A = the packed weight tap, N = the
+//     tile's 128 pixels; taps in (K block, tap, K-step) order, scale-d = 0 first.  Per output element that is the order
+//     of conv3x3_wgmma_kernel (nblk > 1) and of conv3x3_ws_kernel<0> (nblk = 1), so the results are bit-identical to the
+//     layer's teco_conv3x3_tc launch.
+//   - Cin up to 512 is 9 x 8 weight taps of 8 KB per Cout slice, too many to keep resident: one producer warp streams
+//     (pixel box, weight tap) pairs through an IC_STAGES-deep ring; a stage is released once the MMAs that read it have
+//     completed (one arrival per consumer warp, after wgmma.wait_group of the next step).
+//   - Persistent CTAs; the two consumer warpgroups take alternate tiles of the CTA's walk and take turns to issue their
+//     tiles' MMAs (named barriers 1 and 2, as in conv3x3_ws_kernel), so one warpgroup's epilogue overlaps the other's
+//     MMAs.
+//   - Epilogue: ws_epilogue<ACT, 0> (bias -> activation -> bf16, stmatrix) into the warpgroup's staging tile, whose pixel
+//     p is row p as in the ws kernel; one TMA store of the [128 pixels, 64 channels] box on the flat [N*H*W, Cout] view,
+//     clipped after the last pixel.
+constexpr int IC_PIX = 128;                                  // output pixels per tile
+constexpr uint32_t IC_BOX = IC_PIX * 128u;                   // one pixel box or staging tile: 16384
+constexpr uint32_t IC_TAP = 64u * 128u;                      // one packed weight tap of a 64-channel Cout slice
+constexpr uint32_t IC_STAGE = IC_BOX + IC_TAP;               // 24576: stages stay 1024-byte aligned
+constexpr int IC_STAGES = 8;
+constexpr size_t IC_SMEM = 1024 + IC_STAGES * (size_t)IC_STAGE + 2 * (size_t)IC_BOX + 2 * IC_STAGES * sizeof(uint64_t) +
+                           64 * sizeof(float);
+static_assert(IC_SMEM <= SMEM_MAX, "conv3x3_im2col_kernel: shared memory budget");
+
+struct IcParams {
+  int H, W, Cout, nblk, act, num_tiles;
+  const uint8_t* wpk;
+  const float* bias;
+};
+
+__global__ void __launch_bounds__(WS_THREADS, 1)
+conv3x3_im2col_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_constant__ CUtensorMap ymap, const IcParams p) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  uint8_t* ring = smem;                                                  // IC_STAGES x [pixel box | weight tap]
+  uint8_t* outs = ring + IC_STAGES * (size_t)IC_STAGE;                   // [2] staging tiles
+  uint64_t* full = reinterpret_cast<uint64_t*>(outs + 2 * (size_t)IC_BOX);   // [IC_STAGES]
+  uint64_t* empty = full + IC_STAGES;                                    // [IC_STAGES]
+  float* s_bias = reinterpret_cast<float*>(empty + IC_STAGES);           // [64]
+
+  const int tid = threadIdx.x, wg = tid >> 7;
+  const int n0 = blockIdx.y * 64;
+  const int G = gridDim.x;
+  const int my_tiles = (int)blockIdx.x < p.num_tiles ? (p.num_tiles - (int)blockIdx.x + G - 1) / G : 0;
+
+  for (int c = tid; c < 64; c += WS_THREADS) s_bias[c] = p.bias ? p.bias[n0 + c] : 0.f;
+  if (tid == 0) {
+    for (int s = 0; s < IC_STAGES; ++s) {
+      mbar_init(smem_u32(&full[s]), 1);
+      mbar_init(smem_u32(&empty[s]), 4);      // one arrival per warp of the consumer warpgroup reading the stage
+    }
+    fence_mbar_init();
+  }
+  __syncthreads();
+  if (my_tiles == 0) return;
+
+  if (wg == 2) {                              // producer warp: one lane issues every load of the ring
+    if (tid == NUM_THREADS) {
+      asm volatile("prefetch.tensormap [%0];" ::"l"(&xmap) : "memory");
+      const int HW = p.H * p.W;
+      for (int k = 0, q = 0; k < my_tiles; ++k) {
+        const int p0 = ((int)blockIdx.x + k * G) * IC_PIX;
+        const int n = p0 / HW, r = p0 - n * HW, oy = r / p.W, ox = r - oy * p.W;
+        for (int b = 0; b < p.nblk; ++b)
+          for (int t = 0; t < 9; ++t, ++q) {
+            const int st = q % IC_STAGES;
+            if (q >= IC_STAGES) mbar_wait(smem_u32(&empty[st]), (uint32_t)((q / IC_STAGES - 1) & 1));
+            const uint32_t base = smem_u32(ring + (size_t)st * IC_STAGE), bar = smem_u32(&full[st]);
+            mbar_expect_tx(bar, IC_STAGE);
+            tma_load_im2col_4d(base, &xmap, bar, b * CB, ox - 1, oy - 1, n, (uint16_t)(t % 3), (uint16_t)(t / 3));
+            bulk_load_1d(base + IC_BOX, p.wpk + ((size_t)(b * 9 + t) * p.Cout + n0) * 128, IC_TAP, bar);
+          }
+      }
+    }
+    return;
+  }
+
+  // consumer warpgroup wg: tiles wg, wg + 2, ... of the walk; tile k issues its MMAs in turn k
+  const int wq = (tid >> 5) & 3, lane = tid & 31;
+  const bool leader = (tid & 127) == 0;       // issues this warpgroup's output stores
+  const int my_turn = 1 + wg, other_turn = 2 - wg;
+  const float bias_r[2] = {s_bias[16 * wq + (lane >> 2)], s_bias[16 * wq + 8 + (lane >> 2)]};
+  const uint32_t ring_a = smem_u32(ring), out_a = smem_u32(outs + (size_t)wg * IC_BOX);
+  const int steps = 9 * p.nblk;
+  float acc[1][64];
+  for (int k = wg; k < my_tiles; k += 2) {
+    int q = k * steps;                        // ring steps of the tiles before this one
+    if (k > 0) named_bar_sync(my_turn, 2 * 128);
+    for (int b = 0; b < p.nblk; ++b) {
+#pragma unroll
+      for (int t = 0; t < 9; ++t, ++q) {
+        const int st = q % IC_STAGES;
+        mbar_wait(smem_u32(&full[st]), (uint32_t)((q / IC_STAGES) & 1));
+        const uint32_t box_a = ring_a + (uint32_t)st * IC_STAGE, w_a = box_a + IC_BOX;
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < CB / 16; ++kk)
+          Wgmma<128, 0, 0>::run(acc[0], gmma_desc_sw128(w_a + 32u * kk, 16u, 1024u), gmma_desc_sw128(box_a + 32u * kk, 16u, 1024u),
+                                b == 0 && t == 0 && kk == 0 ? 0u : 1u);
+        wgmma_commit();
+        if (b > 0 || t > 0) {
+          wgmma_wait<1>();                    // the previous step's MMAs have completed: release its stage
+          mbar_arrive_if(smem_u32(&empty[(q - 1) % IC_STAGES]), lane == 0);
+        }
+      }
+    }
+    if (k + 1 < my_tiles) named_bar_arrive(other_turn, 2 * 128);
+    wgmma_wait_all_fence(acc);
+    if (lane == 0) mbar_arrive(smem_u32(&empty[(q - 1) % IC_STAGES]));
+
+    if (leader) bulk_wait_read<0>();          // this warpgroup's previous store has read the staging tile
+    named_bar_sync(3 + wg, 128);
+    switch (p.act) {                          // once per tile: the element loop is compiled per activation
+      case TECO_ACT_RELU: ws_epilogue<TECO_ACT_RELU, 0>(acc, s_bias, bias_r, out_a, false, wq, lane); break;
+      case TECO_ACT_LRELU02: ws_epilogue<TECO_ACT_LRELU02, 0>(acc, s_bias, bias_r, out_a, false, wq, lane); break;
+      case TECO_ACT_TANH24: ws_epilogue<TECO_ACT_TANH24, 0>(acc, s_bias, bias_r, out_a, false, wq, lane); break;
+      case TECO_ACT_SIGMOID: ws_epilogue<TECO_ACT_SIGMOID, 0>(acc, s_bias, bias_r, out_a, false, wq, lane); break;
+      default: ws_epilogue<TECO_ACT_NONE, 0>(acc, s_bias, bias_r, out_a, false, wq, lane); break;
+    }
+    fence_async_smem();                       // the staging writes -> visible to the TMA store
+    named_bar_sync(3 + wg, 128);
+    if (leader) {
+      tma_store_2d(&ymap, out_a, n0, ((int)blockIdx.x + k * G) * IC_PIX);
+      bulk_commit();
+    }
+  }
+  if (leader) bulk_wait_all();
+}
+
 // ------------------------------------------------------------------ generator trunk in shared memory (32 x 32 images)
 // A chain of 3x3 64 -> 64 layers on 32 x 32 images in one launch, the activations never leaving shared memory.  A cluster
 // of two CTAs (one per SM, persistent) owns clips c, c + G, ... (G clusters); CTA r of the cluster owns image rows
@@ -755,15 +891,28 @@ typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_
                                     const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
                                     CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 
+typedef CUresult (*PFN_encodeIm2col)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
+                                     const cuuint64_t*, const int*, const int*, cuuint32_t, cuuint32_t, const cuuint32_t*,
+                                     CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion,
+                                     CUtensorMapFloatOOBfill);
+
+void* driver_entry(const char* name) {
+  void* p = nullptr;
+  cudaDriverEntryPointQueryResult qres;
+  if (cudaGetDriverEntryPoint(name, &p, cudaEnableDefault, &qres) == cudaSuccess && qres == cudaDriverEntryPointSuccess)
+    return p;
+  return nullptr;
+}
+
 PFN_encodeTiled get_encode() {
   static PFN_encodeTiled fn = nullptr;
-  if (!fn) {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) == cudaSuccess &&
-        qres == cudaDriverEntryPointSuccess)
-      fn = (PFN_encodeTiled)p;
-  }
+  if (!fn) fn = (PFN_encodeTiled)driver_entry("cuTensorMapEncodeTiled");
+  return fn;
+}
+
+PFN_encodeIm2col get_encode_im2col() {
+  static PFN_encodeIm2col fn = nullptr;
+  if (!fn) fn = (PFN_encodeIm2col)driver_entry("cuTensorMapEncodeIm2col");
   return fn;
 }
 
@@ -785,6 +934,42 @@ int encode_halo_map(CUtensorMap* map, const void* x, int N, int H, int W, int C,
                           CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (cr != CUDA_SUCCESS) {
     teco_set_error("%s: cuTensorMapEncodeTiled failed with CUresult %d (N=%d H=%d W=%d C=%d)", who, (int)cr, N, H, W, C);
+    return TECO_E_CUDA;
+  }
+  return TECO_OK;
+}
+
+// conv3x3_im2col_kernel's maps: x [N,H,W,Cin] in im2col mode, IC_PIX pixels x 64 channels per load with the 3 x 3 'SAME'
+// bounding box (corners -1, -1: output pixel (y, x) starts at input (y - 1, x - 1)); y as a 2-D [N*H*W, Cout] view
+// stored in boxes of IC_PIX pixels x 64 channels.  Both SWIZZLE_128B.
+int encode_im2col_maps(CUtensorMap* xmap, CUtensorMap* ymap, const void* x, const void* y, int N, int H, int W, int Cin,
+                       int Cout) {
+  const char* who = "teco_conv3x3_im2col_tc";
+  PFN_encodeIm2col enc = get_encode_im2col();
+  if (!enc || !get_encode()) {
+    teco_set_error("%s: cuTensorMapEncodeIm2col is unavailable (no CUDA driver?)", who);
+    return TECO_E_CUDA;
+  }
+  const cuuint64_t gdim[4] = {(cuuint64_t)Cin, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)N};
+  const cuuint64_t gstr[3] = {(cuuint64_t)Cin * 2, (cuuint64_t)W * Cin * 2, (cuuint64_t)H * W * Cin * 2};
+  const int lower[2] = {-1, -1}, upper[2] = {-1, -1};
+  const cuuint32_t estr[4] = {1, 1, 1, 1};
+  CUresult cr = enc(xmap, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(x), gdim, gstr, lower, upper, CB, IC_PIX,
+                    estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (cr != CUDA_SUCCESS) {
+    teco_set_error("%s: cuTensorMapEncodeIm2col failed with CUresult %d (N=%d H=%d W=%d C=%d)", who, (int)cr, N, H, W, Cin);
+    return TECO_E_CUDA;
+  }
+  const cuuint64_t ydim[2] = {(cuuint64_t)Cout, (cuuint64_t)N * H * W};
+  const cuuint64_t ystr[1] = {(cuuint64_t)Cout * 2};
+  const cuuint32_t ybox[2] = {(cuuint32_t)CB, (cuuint32_t)IC_PIX};
+  cr = get_encode()(ymap, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(y), ydim, ystr, ybox, estr,
+                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (cr != CUDA_SUCCESS) {
+    teco_set_error("%s: cuTensorMapEncodeTiled failed with CUresult %d (output N*H*W=%lld C=%d)", who, (int)cr,
+                   (long long)N * H * W, Cout);
     return TECO_E_CUDA;
   }
   return TECO_OK;
@@ -886,6 +1071,29 @@ int launch_conv3x3(const teco_tc_desc* d, const void* x, const void* wpk, const 
   return TECO_OK;
 }
 
+int launch_conv3x3_im2col(const teco_tc_desc* d, const void* x, const void* wpk, const float* bias, void* y,
+                          cudaStream_t stream) {
+  IcParams p;
+  p.H = d->H; p.W = d->W; p.Cout = d->Cout; p.nblk = d->Cin / CB; p.act = d->act;
+  p.wpk = (const uint8_t*)wpk; p.bias = bias;
+  const long long tiles = ((long long)d->N * d->H * d->W + IC_PIX - 1) / IC_PIX;
+  TECO_CHECK_ARG(tiles * IC_PIX < (1LL << 31), "teco_conv3x3_im2col_tc: too many pixels");
+  p.num_tiles = (int)tiles;
+  CUtensorMap xmap, ymap;
+  const int rc_map = encode_im2col_maps(&xmap, &ymap, x, y, d->N, d->H, d->W, d->Cin, d->Cout);
+  if (rc_map != TECO_OK) return rc_map;
+  int per_sm = 0;
+  const int rc_occ = resident_ctas((const void*)conv3x3_im2col_kernel, IC_SMEM, &per_sm, WS_THREADS);
+  if (rc_occ != TECO_OK) return rc_occ;
+  // persistent: as many CTAs as are resident at once, spread over the Cout slices
+  const int nsplit = d->Cout / 64;
+  const long long slots = ((long long)per_sm * teco_sm_count() + nsplit - 1) / nsplit;
+  const unsigned gx = (unsigned)(tiles < slots ? tiles : slots);
+  conv3x3_im2col_kernel<<<dim3(gx, (unsigned)nsplit), WS_THREADS, IC_SMEM, stream>>>(xmap, ymap, p);
+  TECO_CUDA_LAUNCH_CHECK("teco_conv3x3_im2col_tc");
+  return TECO_OK;
+}
+
 // The plans conv3x3_trunk_cluster_kernel runs: 32 x 32 images; layer 0 reads x_in (buffer 0) into buffer 1 without a
 // residual; every later layer reads the previous layer's output and writes the other one of buffers 1 and 2, with no
 // residual or an in-place one on a buffer an earlier layer wrote.  So layer l writes buffer 1 (slot 1) for even l and
@@ -979,6 +1187,21 @@ extern "C" int teco_conv3x3_tc(const teco_tc_desc* d, const void* x, const void*
                      (((uintptr_t)res) & 15) == 0,
                  "teco_conv3x3_tc: tensors must be 16-byte aligned");
   return launch_conv3x3(d, x, wpk, bias, res, y, res_f32, out_f32, (cudaStream_t)stream);
+}
+
+extern "C" int teco_conv3x3_im2col_tc(const teco_tc_desc* d, const void* x, const void* wpk, const float* bias, void* y,
+                                      void* stream) {
+  TECO_CHECK_ARG(d && x && wpk && y, "teco_conv3x3_im2col_tc: NULL argument");
+  TECO_CHECK_ARG(d->N > 0 && d->H > 0 && d->W > 0, "teco_conv3x3_im2col_tc: bad shape N=%d H=%d W=%d", d->N, d->H, d->W);
+  TECO_CHECK_ARG(d->Cin >= 64 && d->Cin % 64 == 0 && d->Cin <= 512,
+                 "teco_conv3x3_im2col_tc: Cin must be a multiple of 64 in [64,512] (got %d)", d->Cin);
+  TECO_CHECK_ARG(d->Cout >= 64 && d->Cout % 64 == 0 && d->Cout <= 512,
+                 "teco_conv3x3_im2col_tc: Cout must be a multiple of 64 in [64,512] (got %d)", d->Cout);
+  TECO_CHECK_ARG(d->mode == 0 && d->out_f32_c == 0, "teco_conv3x3_im2col_tc: mode 0 with a bf16 output only");
+  TECO_CHECK_ARG(d->act >= 0 && d->act <= TECO_ACT_SIGMOID, "teco_conv3x3_im2col_tc: unknown activation %d", d->act);
+  TECO_CHECK_ARG((((uintptr_t)x) & 15) == 0 && (((uintptr_t)wpk) & 15) == 0 && (((uintptr_t)y) & 15) == 0,
+                 "teco_conv3x3_im2col_tc: tensors must be 16-byte aligned");
+  return launch_conv3x3_im2col(d, x, wpk, bias, y, (cudaStream_t)stream);
 }
 
 extern "C" int teco_conv3x3_lin_supported(int32_t N, int32_t H, int32_t W, int32_t num_layers) {

@@ -521,6 +521,17 @@ def conv3x3_tc(x, wpk, bias, y=None, *, cout, act=ACT_NONE, res=None, mode=0, ou
     return y if out_f32 is None else out_f32
 
 
+def conv3x3_im2col_tc(x, wpk, bias, y=None, *, cout, act=ACT_NONE):
+    """The same convolution as conv3x3_tc (mode 0, bf16 output, no residual) on 128-pixel tiles in flat N*H*W order,
+    for images smaller than conv3x3_tc's 16 x 8 tile.  x [N,H,W,Cin] bf16; y [N,H,W,cout] bf16 (allocated if None)."""
+    N, H, W, Cin = x.shape
+    if y is None:
+        y = torch.empty((N, H, W, cout), device=x.device, dtype=bf16)
+    d = TcDesc(N=N, H=H, W=W, Cin=Cin, Cout=cout, act=act, mode=0, out_f32_c=0, post_scale=1.0, post_shift=0.0)
+    call("teco_conv3x3_im2col_tc", d, ptr(x, bf16), ptr(wpk, bf16), ptr(bias, f32), ptr(y, bf16), stream_ptr())
+    return y
+
+
 def conv3x3_lin_supported(N, H, W, num_layers):
     from ._ffi import lib
     return bool(lib().teco_conv3x3_lin_supported(N, H, W, num_layers))

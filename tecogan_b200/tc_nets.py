@@ -205,9 +205,11 @@ class FNetPlan:
         n = self.n
         flow = self.flow if flow_out is None else flow_out
         for i, ((c1, c2), (t1, t2, t3)) in enumerate(zip(self.layers, self.bufs)):
-            K.conv3x3_tc(x, c1.wpk, c1.bias, t1, cout=c1.cout_pad, act=ACT_LRELU02)
-            K.conv3x3_tc(t1, c2.wpk, c2.bias, t2, cout=c2.cout_pad, act=ACT_LRELU02)
             _, hh, ww, cc = t2.shape
+            # levels smaller than conv3x3_tc's 16 x 8 tile of one image: 128-pixel tiles across images
+            conv = K.conv3x3_im2col_tc if hh < 16 or ww < 8 else K.conv3x3_tc
+            conv(x, c1.wpk, c1.bias, t1, cout=c1.cout_pad, act=ACT_LRELU02)
+            conv(t1, c2.wpk, c2.bias, t2, cout=c2.cout_pad, act=ACT_LRELU02)
             if i < 3:
                 call("teco_maxpool2_bf16", ptr(t2, bf16), ptr(t3, bf16), n, hh, ww, cc, stream_ptr())
             else:
