@@ -100,6 +100,28 @@ int teco_conv3x3_tc(const teco_tc_desc* d, const void* x, const void* wpk, const
  * Cin and Cout multiples of 64 in [64,512]; d->mode and d->out_f32_c must be 0.  Bit-identical to teco_conv3x3_tc. */
 int teco_conv3x3_im2col_tc(const teco_tc_desc* d, const void* x, const void* wpk, const float* bias, void* y, void* stream);
 
+/* conv2() 4x4 stride 2 SAME (discriminator_F's disblocks, reference lib/Teco.py:35-41,54-67) on the tensor cores, through
+ * its space-to-depth-2 form.  On even H, W TF pads one row / column before, so with xs = space-to-depth-2 of x
+ * [N,H/2,W/2,4*Cin], channel (py*2 + px)*Cin + ci = x[2i + py, 2j + px, ci], the convolution is the 3x3 stride-1 SAME one
+ *   y = conv3x3(xs, W'),  W'[ty][tx][(py*2 + px)*Cin + ci][co] = w[2ty + py - 1][2tx + px - 1][ci][co]
+ * (zero where a kernel index leaves 0..3: 16 of the 36 (tap, phase) slots are live).  Its input gradient is
+ * dxs = conv3x3(dz, W'') with W'' the flipped-tap transpose of W', and dx = depth-to-space-2(dxs); its weight gradient is
+ * teco_conv3x3_wgrad_tc(xs, dz) at the 16 live slots.  H and W even, Cin 64 or 128, Cout a multiple of 64 in [64,512];
+ * anything else -> TECO_E_INVALID.  Maps smaller than a 16 x 8 tile run on teco_conv3x3_im2col_tc's kernel.
+ * teco_pack_conv4x4s2_bf16: w [4,4,Cin,Cout] fp32 -> W' packed as teco_pack_conv3x3_bf16 packs a [3,3,4Cin,Cout] weight
+ *   (dgrad 0, 36*Cin*Cout bf16), or W'' as its flag 3 packs W' (dgrad 1, same size).
+ * teco_conv4x4s2_tc: xs bf16 [N,H/2,W/2,4Cin] -> y bf16 [N,H/2,W/2,Cout] = act(conv(x, w) + bias); bias may be NULL.
+ * teco_conv4x4s2_dgrad_tc: dz bf16 [N,H/2,W/2,Cout] -> dxs bf16 [N,H/2,W/2,4Cin].  H, W: the full-resolution input size. */
+int teco_pack_conv4x4s2_bf16(const float* w, int32_t cin, int32_t cout, int32_t dgrad, void* wpk, void* stream);
+int teco_conv4x4s2_tc(int32_t N, int32_t H, int32_t W, int32_t Cin, int32_t Cout, int32_t act, const void* xs,
+                      const void* wpk, const float* bias, void* y, void* stream);
+int teco_conv4x4s2_dgrad_tc(int32_t N, int32_t H, int32_t W, int32_t Cin, int32_t Cout, const void* dz, const void* wpk_t,
+                            void* dxs, void* stream);
+/* The conversions around it: x fp32 [N,H,W,C] -> xs bf16 [N,H/2,W/2,4C] (space-to-depth-2 as above), and
+ * dxs bf16 [N,H/2,W/2,4C] -> dx fp32 [N,H,W,C] (its inverse).  H, W even, C % 4 == 0, 16-byte aligned tensors. */
+int teco_f32_to_bf16_s2d2(const float* x, void* xs, int32_t N, int32_t H, int32_t W, int32_t C, void* stream);
+int teco_bf16_d2s2_to_f32(const void* dxs, float* dx, int32_t N, int32_t H, int32_t W, int32_t C, void* stream);
+
 /* Bias gradient of conv2() (slim.conv2d biases, reference lib/ops.py:47-56): db[c] (+)= sum over npix pixels of dy[pixel*cpitch + c]. */
 int teco_bias_grad_f32(const float* dy, float* db, int64_t npix, int32_t C, int32_t cpitch, int32_t accumulate, void* stream);
 

@@ -72,6 +72,7 @@ LIN_TRUNK_MIN_FILL = 0.8
 
 
 def train_tc_all():
-    """bf16 training mode: also run conv2_tran (forward, input and weight gradient) and the narrow-output convolutions
-    (generator 64 -> 3, fnet 32 -> 2) on wgmma instead of the fp32 kernels (TECO_TRAIN_TC_ALL=0 restores the latter)."""
+    """bf16 training mode: also run conv2_tran (forward, input and weight gradient), the narrow-output convolutions
+    (generator 64 -> 3, fnet 32 -> 2) and the discriminator's 4x4 stride-2 convolutions on wgmma instead of the fp32
+    kernels (TECO_TRAIN_TC_ALL=0 restores the latter)."""
     return _cfg["train_tc_all"]

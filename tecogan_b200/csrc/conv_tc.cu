@@ -887,6 +887,32 @@ __global__ void pack_conv3x3_kernel(const float* __restrict__ w, int cin, int co
   }
 }
 
+// The 4x4 stride-2 SAME convolution w[4,4,cin,cout] as a 3x3 one on its space-to-depth-2 input (teco_conv4x4s2_tc):
+// W'[ty][tx][(py*2 + px)*cin + ci][co] = w[2ty + py - 1][2tx + px - 1][ci][co], zero where a kernel index falls outside
+// 0..3.  dgrad == 0 packs W' in pack_conv3x3_kernel's image ([4cin/64][9][cout][64]); dgrad == 1 packs the input-gradient
+// convolution of W', taps flipped and channels swapped ([cout/64][9][4cin][64]).
+__global__ void pack_conv4x4s2_kernel(const float* __restrict__ w, int cin, int cout, int dgrad, __nv_bfloat16* __restrict__ out) {
+  const int kdim = dgrad ? cout : 4 * cin, ndim = dgrad ? 4 * cin : cout;
+  const long long total = 9LL * kdim * ndim;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const int e = (int)(i & 7);
+    const int jpos = (int)((i >> 3) & 7);
+    long long t = i >> 6;
+    const int n = (int)(t % ndim);
+    t /= ndim;
+    const int tap = (int)(t % 9);
+    const int k = (int)(t / 9) * 64 + (jpos ^ (n & 7)) * 8 + e;
+    const int s = dgrad ? 8 - tap : tap;         // tap of W'
+    const int sc = dgrad ? n : k;                // space-to-depth channel (phase, ci)
+    const int co = dgrad ? k : n;
+    const int ph = sc / cin, ci = sc - ph * cin;
+    const int ky = 2 * (s / 3) + (ph >> 1) - 1, kx = 2 * (s % 3) + (ph & 1) - 1;
+    float v = 0.f;
+    if (ky >= 0 && ky < 4 && kx >= 0 && kx < 4) v = w[((long long)(ky * 4 + kx) * cin + ci) * cout + co];
+    out[i] = __float2bfloat16_rn(v);
+  }
+}
+
 typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                     const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
                                     CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -1202,6 +1228,59 @@ extern "C" int teco_conv3x3_im2col_tc(const teco_tc_desc* d, const void* x, cons
   TECO_CHECK_ARG((((uintptr_t)x) & 15) == 0 && (((uintptr_t)wpk) & 15) == 0 && (((uintptr_t)y) & 15) == 0,
                  "teco_conv3x3_im2col_tc: tensors must be 16-byte aligned");
   return launch_conv3x3_im2col(d, x, wpk, bias, y, (cudaStream_t)stream);
+}
+
+// Shapes of the 4x4 stride-2 convolution on its space-to-depth-2 form: even H, W; Cin a multiple of 64 with 4 * Cin <= 512
+// (the input of the forward 3x3 and the output of its input gradient); Cout a multiple of 64 in [64,512].
+static int conv4x4s2_check(int N, int H, int W, int Cin, int Cout, const char* who) {
+  TECO_CHECK_ARG(N > 0 && H > 0 && W > 0 && H % 2 == 0 && W % 2 == 0, "%s: H and W must be even (got N=%d H=%d W=%d)", who, N, H, W);
+  TECO_CHECK_ARG(Cin >= 64 && Cin % 64 == 0 && Cin <= 128, "%s: Cin must be 64 or 128 (got %d)", who, Cin);
+  TECO_CHECK_ARG(Cout >= 64 && Cout % 64 == 0 && Cout <= 512, "%s: Cout must be a multiple of 64 in [64,512] (got %d)", who, Cout);
+  return TECO_OK;
+}
+
+// The 3x3 launch on the half-resolution grid: 128-pixel tiles across images below conv3x3_tc's 16 x 8 tile, as FNet's
+// small levels do.
+static int launch_conv3x3_s2d(const teco_tc_desc* d, const void* x, const void* wpk, const float* bias, void* y,
+                              cudaStream_t stream) {
+  if (d->H < TILE_ROWS || d->W < TILE_COLS) return launch_conv3x3_im2col(d, x, wpk, bias, y, stream);
+  return launch_conv3x3(d, x, wpk, bias, nullptr, y, nullptr, nullptr, stream);
+}
+
+extern "C" int teco_pack_conv4x4s2_bf16(const float* w, int32_t cin, int32_t cout, int32_t dgrad, void* wpk, void* stream) {
+  TECO_CHECK_ARG(w && wpk, "teco_pack_conv4x4s2_bf16: NULL tensor");
+  TECO_CHECK_ARG(dgrad == 0 || dgrad == 1, "teco_pack_conv4x4s2_bf16: dgrad must be 0 or 1 (got %d)", dgrad);
+  const int rc = conv4x4s2_check(1, 2, 2, cin, cout, "teco_pack_conv4x4s2_bf16");
+  if (rc != TECO_OK) return rc;
+  const long long total = 36LL * cin * cout;
+  int blocks = teco_ceil_div(total, 256);
+  if (blocks > 4096) blocks = 4096;
+  pack_conv4x4s2_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(w, cin, cout, dgrad, (__nv_bfloat16*)wpk);
+  TECO_CUDA_LAUNCH_CHECK("teco_pack_conv4x4s2_bf16");
+  return TECO_OK;
+}
+
+extern "C" int teco_conv4x4s2_tc(int32_t N, int32_t H, int32_t W, int32_t Cin, int32_t Cout, int32_t act, const void* xs,
+                                 const void* wpk, const float* bias, void* y, void* stream) {
+  TECO_CHECK_ARG(xs && wpk && y, "teco_conv4x4s2_tc: NULL argument");
+  const int rc = conv4x4s2_check(N, H, W, Cin, Cout, "teco_conv4x4s2_tc");
+  if (rc != TECO_OK) return rc;
+  TECO_CHECK_ARG(act >= 0 && act <= TECO_ACT_SIGMOID, "teco_conv4x4s2_tc: unknown activation %d", act);
+  TECO_CHECK_ARG((((uintptr_t)xs) & 15) == 0 && (((uintptr_t)wpk) & 15) == 0 && (((uintptr_t)y) & 15) == 0,
+                 "teco_conv4x4s2_tc: tensors must be 16-byte aligned");
+  const teco_tc_desc d = {N, H / 2, W / 2, 4 * Cin, Cout, act, 0, 0, 1.f, 0.f};
+  return launch_conv3x3_s2d(&d, xs, wpk, bias, y, (cudaStream_t)stream);
+}
+
+extern "C" int teco_conv4x4s2_dgrad_tc(int32_t N, int32_t H, int32_t W, int32_t Cin, int32_t Cout, const void* dz,
+                                       const void* wpk_t, void* dxs, void* stream) {
+  TECO_CHECK_ARG(dz && wpk_t && dxs, "teco_conv4x4s2_dgrad_tc: NULL argument");
+  const int rc = conv4x4s2_check(N, H, W, Cin, Cout, "teco_conv4x4s2_dgrad_tc");
+  if (rc != TECO_OK) return rc;
+  TECO_CHECK_ARG((((uintptr_t)dz) & 15) == 0 && (((uintptr_t)wpk_t) & 15) == 0 && (((uintptr_t)dxs) & 15) == 0,
+                 "teco_conv4x4s2_dgrad_tc: tensors must be 16-byte aligned");
+  const teco_tc_desc d = {N, H / 2, W / 2, Cout, 4 * Cin, TECO_ACT_NONE, 0, 0, 1.f, 0.f};
+  return launch_conv3x3_s2d(&d, dz, wpk_t, nullptr, dxs, (cudaStream_t)stream);
 }
 
 extern "C" int teco_conv3x3_lin_supported(int32_t N, int32_t H, int32_t W, int32_t num_layers) {

@@ -460,7 +460,66 @@ __global__ void f32_to_bf16_rowpad_kernel(const float* __restrict__ src, __nv_bf
     dst[i] = __float2bfloat16_rn(c < C ? src[p * src_cpitch + c] : 0.f);
   }
 }
+
+// Offset, in 4-channel groups, of full-resolution pixel (n, y, x) group c4 in the space-to-depth-2 image [N,H/2,W/2,4C]
+// whose channel (py*2 + px)*C + c holds pixel (2i + py, 2j + px) channel c; g indexes the full-resolution image's groups.
+__device__ __forceinline__ long long s2d2_group(long long g, int H, int W, int C4) {
+  const long long p = g / C4;
+  const int c4 = (int)(g - p * C4);
+  const int x = (int)(p % W);
+  const long long r = p / W;
+  const int y = (int)(r % H);
+  const long long n = r / H;
+  return ((n * (H / 2) + (y >> 1)) * (W / 2) + (x >> 1)) * (4LL * C4) + ((y & 1) * 2 + (x & 1)) * C4 + c4;
+}
+
+__global__ void f32_to_bf16_s2d2_kernel(const float4* __restrict__ x, uint2* __restrict__ xs, long long groups, int H, int W,
+                                        int C4) {
+  GRID_STRIDE(g, groups) {
+    const float4 v = x[g];
+    __nv_bfloat162 lo = __floats2bfloat162_rn(v.x, v.y), hi = __floats2bfloat162_rn(v.z, v.w);
+    uint2 o;
+    o.x = *reinterpret_cast<uint32_t*>(&lo);
+    o.y = *reinterpret_cast<uint32_t*>(&hi);
+    xs[s2d2_group(g, H, W, C4)] = o;
+  }
+}
+
+__global__ void bf16_d2s2_to_f32_kernel(const uint2* __restrict__ xs, float4* __restrict__ x, long long groups, int H, int W,
+                                        int C4) {
+  GRID_STRIDE(g, groups) {
+    const uint2 v = xs[s2d2_group(g, H, W, C4)];
+    const float2 lo = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&v.x));
+    const float2 hi = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&v.y));
+    x[g] = make_float4(lo.x, lo.y, hi.x, hi.y);
+  }
+}
+
+int s2d2_check(const void* a, const void* b, int N, int H, int W, int C, const char* who) {
+  TECO_CHECK_ARG(a && b && N > 0 && H > 0 && W > 0 && H % 2 == 0 && W % 2 == 0 && C > 0 && C % 4 == 0,
+                 "%s: needs even H, W and C a multiple of 4 (got N=%d H=%d W=%d C=%d)", who, N, H, W, C);
+  TECO_CHECK_ARG((((uintptr_t)a) & 15) == 0 && (((uintptr_t)b) & 15) == 0, "%s: tensors must be 16-byte aligned", who);
+  return TECO_OK;
+}
 }  // namespace
+
+extern "C" int teco_f32_to_bf16_s2d2(const float* x, void* xs, int32_t N, int32_t H, int32_t W, int32_t C, void* stream) {
+  const int rc = s2d2_check(x, xs, N, H, W, C, "teco_f32_to_bf16_s2d2");
+  if (rc != TECO_OK) return rc;
+  const long long groups = (long long)N * H * W * (C / 4);
+  f32_to_bf16_s2d2_kernel<<<grid_for(groups), TPB, 0, (cudaStream_t)stream>>>((const float4*)x, (uint2*)xs, groups, H, W, C / 4);
+  TECO_CUDA_LAUNCH_CHECK("teco_f32_to_bf16_s2d2");
+  return TECO_OK;
+}
+
+extern "C" int teco_bf16_d2s2_to_f32(const void* xs, float* x, int32_t N, int32_t H, int32_t W, int32_t C, void* stream) {
+  const int rc = s2d2_check(xs, x, N, H, W, C, "teco_bf16_d2s2_to_f32");
+  if (rc != TECO_OK) return rc;
+  const long long groups = (long long)N * H * W * (C / 4);
+  bf16_d2s2_to_f32_kernel<<<grid_for(groups), TPB, 0, (cudaStream_t)stream>>>((const uint2*)xs, (float4*)x, groups, H, W, C / 4);
+  TECO_CUDA_LAUNCH_CHECK("teco_bf16_d2s2_to_f32");
+  return TECO_OK;
+}
 
 extern "C" int teco_bf16_to_f32_add(const void* src, const float* add, float* dst, int64_t npix, int32_t C,
                                     int32_t src_cpitch, int32_t dst_cpitch, void* stream) {

@@ -807,3 +807,99 @@ class _ConvTranspose2xTC(torch.autograd.Function):
 
 def conv_transpose2x_train_tc(x, w, b=None, act=ACT_NONE):
     return _ConvTranspose2xTC.apply(x, w, b, act)
+
+
+# conv2() 4x4 stride 2 SAME in bf16 training mode (discriminator_F's disblocks).  On even H, W TF pads one row / column
+# before, so with xs = space-to-depth-2 of x, channel (py, px, ci), the convolution is a 3x3 stride-1 SAME one on the
+# half-resolution grid (include/teco.h, teco_conv4x4s2_tc):
+#   ky -> (tap row ty, phase py) = 0 -> (0, 1), 1 -> (1, 0), 2 -> (1, 1), 3 -> (2, 0), i.e. ky = 2 ty + py - 1   (columns alike)
+#   W'[ty, tx, (py, px, ci), co] = w[ky, kx, ci, co], zero in the 20 (tap, phase) slots no (ky, kx) reaches.
+# The input gradient is the flipped-tap transpose of W' on dz, then depth-to-space; the weight gradient is the 3x3 weight
+# gradient of (xs, dz) read at the 16 live slots.
+def conv4x4s2_tc_fits(H, W, cin, cout):
+    """Shapes teco_conv4x4s2_tc takes."""
+    return H % 2 == 0 and W % 2 == 0 and cin in (64, 128) and cout % 64 == 0 and 64 <= cout <= 512
+
+
+def _c4s2_rows():
+    """Row of the [36, Cin, Cout] view of W' = [ty, tx, phase] that holds w[ky, kx], for the sixteen (ky, kx) in ky-major
+    order."""
+    rows = []
+    for ky in range(4):
+        for kx in range(4):
+            (ty, py), (tx, px) = divmod(ky + 1, 2), divmod(kx + 1, 2)
+            rows.append((ty * 3 + tx) * 4 + py * 2 + px)
+    return rows
+
+
+_c4s2_idx = {}
+
+
+def _c4s2_index(device):
+    """_c4s2_rows() as a device tensor (created once per device, outside any CUDA-graph capture: the first step is eager)."""
+    t = _c4s2_idx.get(device)
+    if t is None:
+        t = _c4s2_idx[device] = torch.tensor(_c4s2_rows(), device=device, dtype=torch.int64)
+    return t
+
+
+def _c4s2_packed(w, dgrad):
+    key = (w.data_ptr(), tuple(w.shape), "c4s2", dgrad)
+    wpk = _tc_wcache.get(key)
+    if wpk is None:
+        Cin, Cout = w.shape[2], w.shape[3]
+        wpk = _tc_wcache[key] = torch.empty(36 * Cin * Cout, device=w.device, dtype=bf16)
+        call("teco_pack_conv4x4s2_bf16", ptr(_cc(w.detach()), f32), Cin, Cout, int(dgrad), ptr(wpk, bf16), stream_ptr())
+    return wpk
+
+
+class _Conv4x4S2TC(torch.autograd.Function):
+    """conv2() 4x4 stride 2 SAME on wgmma: forward and input gradient through teco_conv4x4s2_tc / _dgrad_tc, weight gradient
+    on teco_conv3x3_wgrad_tc.  Reference lib/ops.py:47-56 and its TF autodiff."""
+
+    @staticmethod
+    def forward(ctx, x, w, b, act):
+        x, w = _cc(x), _cc(w)
+        N, H, W, Cin = x.shape
+        Cout = w.shape[3]
+        xs = torch.empty((N, H // 2, W // 2, 4 * Cin), device=x.device, dtype=bf16)
+        call("teco_f32_to_bf16_s2d2", ptr(x, f32), ptr(xs, bf16), N, H, W, Cin, stream_ptr())
+        ys = torch.empty((N, H // 2, W // 2, Cout), device=x.device, dtype=bf16)
+        call("teco_conv4x4s2_tc", N, H, W, Cin, Cout, act, ptr(xs, bf16), ptr(_c4s2_packed(w, 0), bf16),
+             ptr(None if b is None else _cc(b.detach()), f32), ptr(ys, bf16), stream_ptr())
+        y = _from_bf16_rows(ys, Cout)
+        ctx.cfg = (act, b is not None)
+        # the bf16 space-to-depth copy of x is the weight gradient's input
+        ctx.save_for_backward(xs if ctx.needs_input_grad[1] else None, w, y if act != ACT_NONE else None)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        act, has_b = ctx.cfg
+        xs, w, y = ctx.saved_tensors
+        dy = _cc(dy)
+        dz = dy
+        if act != ACT_NONE:
+            dz = torch.empty_like(dy)
+            call("teco_act_bwd_f32", ptr(y, f32), ptr(dy, f32), ptr(dz, f32), dy.numel(), act, stream_ptr())
+        N, h, w2, Cout = dz.shape
+        H, W, Cin = 2 * h, 2 * w2, w.shape[2]
+        dzb = _to_bf16_rows(dz, Cout)
+        dx = dw = db = None
+        if ctx.needs_input_grad[0]:
+            dxs = torch.empty((N, h, w2, 4 * Cin), device=dz.device, dtype=bf16)
+            call("teco_conv4x4s2_dgrad_tc", N, H, W, Cin, Cout, ptr(dzb, bf16), ptr(_c4s2_packed(w, 1), bf16), ptr(dxs, bf16),
+                 stream_ptr())
+            dx = torch.empty((N, H, W, Cin), device=dz.device, dtype=f32)
+            call("teco_bf16_d2s2_to_f32", ptr(dxs, bf16), ptr(dx, f32), N, H, W, Cin, stream_ptr())
+        if ctx.needs_input_grad[1]:
+            dwp = torch.empty((3, 3, 4 * Cin, Cout), device=w.device, dtype=f32)
+            conv3x3_wgrad_tc(xs, dzb, dwp, 4 * Cin, Cout)
+            dw = dwp.view(36, Cin, Cout).index_select(0, _c4s2_index(w.device)).view(4, 4, Cin, Cout)
+            if has_b and ctx.needs_input_grad[2]:
+                db = bias_grad(dz)
+        return dx, dw, db, None
+
+
+def conv4x4s2_train_tc(x, w, b=None, act=ACT_NONE):
+    return _Conv4x4S2TC.apply(x, w, b, act)
