@@ -99,6 +99,12 @@ int teco_conv3x3_tc(const teco_tc_desc* d, const void* x, const void* wpk, const
  * tile spans several images: for images smaller than teco_conv3x3_tc's 16 x 8 tile (FNet's 8x8 and 4x4 levels).
  * Cin and Cout multiples of 64 in [64,512]; d->mode and d->out_f32_c must be 0.  Bit-identical to teco_conv3x3_tc. */
 int teco_conv3x3_im2col_tc(const teco_tc_desc* d, const void* x, const void* wpk, const float* bias, void* y, void* stream);
+/* The fp32 output stage of teco_conv3x3_tc (the generator's 64 -> 3 output conv, FNet's 64 -> 2 flow head) on a pipelined
+ * kernel: the same arguments, the same MMAs and epilogue, bit-identical outputs.  Takes mode 0, Cin 64, Cout 16 (the
+ * packed slice), out_f32_c 2 or 3 with W*out_f32_c*4 a multiple of 16 bytes, optional res_f32, any activation and post
+ * transform; res and y must be NULL, and out_f32 / res_f32 16-byte aligned.  Anything else -> TECO_E_INVALID. */
+int teco_conv3x3_f32out_tc(const teco_tc_desc* d, const void* x, const void* wpk, const float* bias,
+                           const void* res, void* y, const float* res_f32, float* out_f32, void* stream);
 
 /* conv2() 4x4 stride 2 SAME (discriminator_F's disblocks, reference lib/Teco.py:35-41,54-67) on the tensor cores, through
  * its space-to-depth-2 form.  On even H, W TF pads one row / column before, so with xs = space-to-depth-2 of x

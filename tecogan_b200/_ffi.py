@@ -43,6 +43,7 @@ SIGNATURES = {
     "teco_packed_weight_bytes": [_I32, _I32],
     "teco_conv3x3_tc": [C.POINTER(TcDesc), _P, _P, _P, _P, _P, _P, _P, _P],
     "teco_conv3x3_im2col_tc": [C.POINTER(TcDesc), _P, _P, _P, _P, _P],
+    "teco_conv3x3_f32out_tc": [C.POINTER(TcDesc), _P, _P, _P, _P, _P, _P, _P, _P],
     "teco_pack_conv4x4s2_bf16": [_P, _I32, _I32, _I32, _P, _P],
     "teco_conv4x4s2_tc": [_I32, _I32, _I32, _I32, _I32, _I32, _P, _P, _P, _P, _P],
     "teco_conv4x4s2_dgrad_tc": [_I32, _I32, _I32, _I32, _I32, _P, _P, _P, _P],

@@ -24,6 +24,8 @@
 // 64-channel input block and 64-channel bf16 output slices (mode 0, or mode 1 without a residual) run on
 // conv3x3_ws_kernel instead: the same MMAs and epilogue arithmetic behind a producer warp, a deeper ring and TMA-staged
 // residuals and stores.
+// The fp32 output stage (Cin = 64, Cout = 16, two or three fp32 channels) has its own entry point,
+// teco_conv3x3_f32out_tc, on conv3x3_f32out_kernel: the same MMAs and epilogue arithmetic, pipelined the same way.
 #include <cuda.h>
 #include "teco_common.cuh"
 #include "tc_ptx.cuh"
@@ -625,6 +627,182 @@ conv3x3_im2col_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_con
   if (leader) bulk_wait_all();
 }
 
+// ------------------------------------------------------------------ fp32 output stage (64 -> 2 or 3 channels)
+// Mode 0, Cin = 64, the 16-channel packed Cout slice, an fp32 output of C = 2 or 3 channels with an optional fp32
+// residual and post scale / shift: the generator's output stage (64 -> 3, + bicubic, * 2 - 1) and FNet's flow head
+// (64 -> 2, tanh * 24).  The products are those of conv3x3_wgmma_kernel<0, 16>: per 64-pixel half of the 16 x 8 tile the
+// unswapped m64n16k16 of mma_issue, the halo as A and the packed weights as B, taps 0..8 x K-steps 0..3 (scale-d = 0
+// first); the epilogue runs epilogue()'s fp32 operations in its order, so the outputs are bit-identical to
+// teco_conv3x3_tc's.  What differs is the pipeline, after conv3x3_ws_kernel<0>:
+//   - one producer warp bulk-copies the 18 KB of weights once and TMA-loads the halo of each tile into an F32_STAGES-deep
+//     ring;
+//   - one consumer warpgroup owns a whole tile (both halves, 2 x 8 accumulator registers per thread); the two take
+//     alternate tiles of the CTA's walk and take turns to issue their MMAs (named barriers 1 and 2), so one warpgroup's
+//     epilogue overlaps the other's MMAs;
+//   - two CTAs per SM, three halo stages each: four issuing warpgroups keep the tensor pipe fed better than one CTA with
+//     an eight-stage ring (at 264 clips x 128 x 128 on an H100 at 700 W: 292 us against 350 us; three CTAs of two stages:
+//     305 us);
+//   - the residual and the output are boxes of 16 rows x 8 C floats on the [N, H, W C] fp32 view.  The residual box of
+//     the warpgroup's next tile is TMA-loaded into its other staging box while this tile's MMAs run; the epilogue
+//     overwrites the residual with the result and one TMA store writes the box out, clipped at the image edges.
+constexpr int F32_STAGES = 3;
+constexpr int F32_CTAS_PER_SM = 2;
+constexpr int F32_BUFS = 2;                                                       // staging boxes per warpgroup
+constexpr uint32_t F32_W_BYTES = 9u * 16u * 128u;                                 // 18432: 9 taps x 16 cout x 64 cin
+constexpr uint32_t F32_BOX_BYTES = TILE_ROWS * TILE_COLS * 3 * sizeof(float);     // one box at C = 3: 1536
+constexpr size_t F32_SMEM = 1024 + F32_STAGES * (size_t)HALO_STAGE + F32_W_BYTES + 2 * F32_BUFS * (size_t)F32_BOX_BYTES +
+                            (2 * F32_STAGES + 1 + 2 * F32_BUFS) * sizeof(uint64_t) + 16 * sizeof(float);
+static_assert(F32_CTAS_PER_SM * (F32_SMEM + 1024) <= 233472, "conv3x3_f32out_kernel: two CTAs per SM (228 KB, 1 KB reserved each)");
+
+struct F32Params {
+  int C, act, has_res, tiles_x, tiles_y, num_tiles;
+  float post_scale, post_shift;
+  const uint8_t* wpk;
+  const float* bias;
+};
+
+// Epilogue of one tile into its staging box (pixel (row r, column x) at floats (8 r + x) C ..): this thread holds, per
+// half h, pixels (row 8 h + 2 wq + i, column lane / 4) at channels 2 (lane % 4) + {0, 1} of the accumulator's first
+// eight (C <= 3: only lanes with lane % 4 < 2 hold a stored channel).  bias -> activation -> (+ residual) -> * scale +
+// shift, as epilogue() computes it.
+template <int ACT>
+__device__ __forceinline__ void f32_epilogue(const float (&acc)[2][1][8], const float* s_bias, float* box, const F32Params& p,
+                                             int wq, int lane) {
+  const int C = p.C, c = 2 * (lane & 3);
+  if (c >= C) return;
+#pragma unroll
+  for (int h = 0; h < 2; ++h)
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      float* px = box + ((8 * h + 2 * wq + i) * TILE_COLS + (lane >> 2)) * C + c;
+      const float v0 = teco_act(acc[h][0][2 * i] + s_bias[c], ACT);
+      px[0] = (v0 + (p.has_res ? px[0] : 0.f)) * p.post_scale + p.post_shift;
+      if (c + 1 < C) {
+        const float v1 = teco_act(acc[h][0][2 * i + 1] + s_bias[c + 1], ACT);
+        px[1] = (v1 + (p.has_res ? px[1] : 0.f)) * p.post_scale + p.post_shift;
+      }
+    }
+}
+
+__global__ void __launch_bounds__(WS_THREADS, F32_CTAS_PER_SM)
+conv3x3_f32out_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ CUtensorMap omap,
+                      const __grid_constant__ CUtensorMap rmap, const F32Params p) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  uint8_t* ring = smem;                                                     // F32_STAGES halo stages
+  uint8_t* w_s = ring + F32_STAGES * (size_t)HALO_STAGE;                    // 9 taps x 16 x 64, resident
+  uint8_t* boxes = w_s + F32_W_BYTES;                                       // [2][F32_BUFS] staging boxes
+  uint64_t* full = reinterpret_cast<uint64_t*>(boxes + 2 * F32_BUFS * (size_t)F32_BOX_BYTES);   // [F32_STAGES]
+  uint64_t* empty = full + F32_STAGES;                                      // [F32_STAGES]
+  uint64_t* w_full = empty + F32_STAGES;
+  uint64_t* r_full = w_full + 1;                                            // [2][F32_BUFS] residual arrived
+  float* s_bias = reinterpret_cast<float*>(r_full + 2 * F32_BUFS);          // [16]
+
+  const int tid = threadIdx.x, wg = tid >> 7;
+  const int G = gridDim.x;
+  const int my_tiles = (int)blockIdx.x < p.num_tiles ? (p.num_tiles - (int)blockIdx.x + G - 1) / G : 0;
+
+  for (int c = tid; c < 16; c += WS_THREADS) s_bias[c] = p.bias ? p.bias[c] : 0.f;
+  if (tid == 0) {
+    for (int s = 0; s < F32_STAGES; ++s) {
+      mbar_init(smem_u32(&full[s]), 1);
+      mbar_init(smem_u32(&empty[s]), 4);      // one arrival per warp of the consumer warpgroup reading the stage
+    }
+    for (int i = 0; i < 1 + 2 * F32_BUFS; ++i) mbar_init(smem_u32(&w_full[i]), 1);   // w_full, r_full[]
+    fence_mbar_init();
+  }
+  __syncthreads();
+  if (my_tiles == 0) return;
+
+  auto tile_coords = [&](int it, int& n, int& y0, int& x0) {
+    int tile = (int)blockIdx.x + it * G;
+    const int tx = tile % p.tiles_x;
+    tile /= p.tiles_x;
+    const int ty = tile % p.tiles_y;
+    n = tile / p.tiles_y;
+    x0 = tx * TILE_COLS;
+    y0 = ty * TILE_ROWS;
+  };
+
+  if (wg == 2) {                              // producer warp: one lane issues every load of the ring
+    if (tid == NUM_THREADS) {
+      asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap) : "memory");
+      mbar_expect_tx(smem_u32(w_full), F32_W_BYTES);
+      bulk_load_1d(smem_u32(w_s), p.wpk, F32_W_BYTES, smem_u32(w_full));
+      for (int k = 0; k < my_tiles; ++k) {
+        const int st = k % F32_STAGES;
+        if (k >= F32_STAGES) mbar_wait(smem_u32(&empty[st]), (uint32_t)((k / F32_STAGES - 1) & 1));
+        int n, y0, x0;
+        tile_coords(k, n, y0, x0);
+        const uint32_t bar = smem_u32(&full[st]);
+        mbar_expect_tx(bar, HALO_BYTES);
+        tma_load_4d(smem_u32(ring + (size_t)st * HALO_STAGE), &tmap, bar, 0, x0 - 1, y0 - 1, n);
+      }
+    }
+    return;
+  }
+
+  // consumer warpgroup wg: tiles wg, wg + 2, ... of the walk; tile k issues its MMAs in turn k
+  const int wq = (tid >> 5) & 3, lane = tid & 31;
+  const bool leader = (tid & 127) == 0;       // issues this warpgroup's residual loads and output stores
+  const int my_turn = 1 + wg, other_turn = 2 - wg;
+  const uint32_t box_bytes = (uint32_t)(TILE_ROWS * TILE_COLS * p.C) * (uint32_t)sizeof(float);
+  auto box_at = [&](int b) { return reinterpret_cast<float*>(boxes + (F32_BUFS * wg + b) * (size_t)F32_BOX_BYTES); };
+  auto load_res = [&](int k, int b) {         // staging box b of this warpgroup <- the residual box of tile k
+    int n, y0, x0;
+    tile_coords(k, n, y0, x0);
+    const uint32_t bar = smem_u32(&r_full[F32_BUFS * wg + b]);
+    mbar_expect_tx(bar, box_bytes);
+    tma_load_3d(smem_u32(box_at(b)), &rmap, bar, x0 * p.C, y0, n);
+  };
+  uint32_t r_phase = 0;                       // bit b: parity of r_full[F32_BUFS wg + b]
+  if (p.has_res && leader && wg < my_tiles) load_res(wg, 0);
+  mbar_wait(smem_u32(w_full), 0);
+  const uint32_t w_a = smem_u32(w_s);
+  float acc[2][1][8];
+  for (int k = wg, m = 0; k < my_tiles; k += 2, ++m) {
+    const int st = k % F32_STAGES, sb = m % F32_BUFS, sb_next = (m + 1) % F32_BUFS;
+    int n, y0, x0;
+    tile_coords(k, n, y0, x0);
+    float* box = box_at(sb);
+    mbar_wait(smem_u32(&full[st]), (uint32_t)((k / F32_STAGES) & 1));
+    if (k > 0) named_bar_sync(my_turn, 2 * 128);
+    const uint32_t halo_a = smem_u32(ring + (size_t)st * HALO_STAGE);
+    mma_issue<0, 16, 1, true>(acc[0], halo_a, w_a, 0);
+    mma_issue<0, 16, 1, true>(acc[1], halo_a, w_a, 1);
+    if (k + 1 < my_tiles) named_bar_arrive(other_turn, 2 * 128);
+    if (p.has_res && leader && k + 2 < my_tiles) {
+      bulk_wait_read<F32_BUFS - 2>();         // the store of this warpgroup's previous tile has read box sb_next
+      load_res(k + 2, sb_next);
+    }
+    wgmma_wait_all_fence(acc[0]);
+    wgmma_wait_all_fence(acc[1]);
+    if (lane == 0) mbar_arrive(smem_u32(&empty[st]));
+
+    if (p.has_res) {
+      mbar_wait(smem_u32(&r_full[F32_BUFS * wg + sb]), (r_phase >> sb) & 1u);
+      r_phase ^= 1u << sb;
+    } else {
+      if (leader) bulk_wait_read<F32_BUFS - 1>();   // the store that last used box sb has read it
+      named_bar_sync(3 + wg, 128);
+    }
+    switch (p.act) {                          // once per tile: the element loop is compiled per activation
+      case TECO_ACT_RELU: f32_epilogue<TECO_ACT_RELU>(acc, s_bias, box, p, wq, lane); break;
+      case TECO_ACT_LRELU02: f32_epilogue<TECO_ACT_LRELU02>(acc, s_bias, box, p, wq, lane); break;
+      case TECO_ACT_TANH24: f32_epilogue<TECO_ACT_TANH24>(acc, s_bias, box, p, wq, lane); break;
+      case TECO_ACT_SIGMOID: f32_epilogue<TECO_ACT_SIGMOID>(acc, s_bias, box, p, wq, lane); break;
+      default: f32_epilogue<TECO_ACT_NONE>(acc, s_bias, box, p, wq, lane); break;
+    }
+    fence_async_smem();                       // the staging writes -> visible to the TMA store
+    named_bar_sync(3 + wg, 128);
+    if (leader) {
+      tma_store_3d(&omap, smem_u32(box), x0 * p.C, y0, n);
+      bulk_commit();
+    }
+  }
+  if (leader) bulk_wait_all();
+}
+
 // ------------------------------------------------------------------ generator trunk in shared memory (32 x 32 images)
 // A chain of 3x3 64 -> 64 layers on 32 x 32 images in one launch, the activations never leaving shared memory.  A cluster
 // of two CTAs (one per SM, persistent) owns clips c, c + G, ... (G clusters); CTA r of the cluster owns image rows
@@ -1120,6 +1298,60 @@ int launch_conv3x3_im2col(const teco_tc_desc* d, const void* x, const void* wpk,
   return TECO_OK;
 }
 
+// conv3x3_f32out_kernel's fp32 residual / output [N,H,W,C] as a 3-D [N, H, W*C] view stored in boxes of 16 rows x 8 C
+// floats (no swizzle, zero fill).  The row stride W*C*4 must be a multiple of 16 bytes (the caller checks).
+int encode_f32_box_map(CUtensorMap* map, const float* t, int N, int H, int W, int C) {
+  const char* who = "teco_conv3x3_f32out_tc";
+  PFN_encodeTiled enc = get_encode();
+  if (!enc) {
+    teco_set_error("%s: cuTensorMapEncodeTiled is unavailable (no CUDA driver?)", who);
+    return TECO_E_CUDA;
+  }
+  const cuuint64_t gdim[3] = {(cuuint64_t)W * C, (cuuint64_t)H, (cuuint64_t)N};
+  const cuuint64_t gstr[2] = {(cuuint64_t)W * C * 4, (cuuint64_t)H * W * C * 4};
+  const cuuint32_t box[3] = {(cuuint32_t)(TILE_COLS * C), (cuuint32_t)TILE_ROWS, 1};
+  const cuuint32_t estr[3] = {1, 1, 1};
+  const CUresult cr = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(t), gdim, gstr, box, estr,
+                          CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (cr != CUDA_SUCCESS) {
+    teco_set_error("%s: cuTensorMapEncodeTiled failed with CUresult %d (N=%d H=%d W=%d C=%d)", who, (int)cr, N, H, W, C);
+    return TECO_E_CUDA;
+  }
+  return TECO_OK;
+}
+
+int launch_conv3x3_f32out(const teco_tc_desc* d, const void* x, const void* wpk, const float* bias, const float* res_f32,
+                          float* out_f32, cudaStream_t stream) {
+  F32Params p;
+  p.C = d->out_f32_c; p.act = d->act; p.has_res = res_f32 != nullptr;
+  p.post_scale = d->post_scale; p.post_shift = d->post_shift;
+  p.wpk = (const uint8_t*)wpk; p.bias = bias;
+  p.tiles_x = teco_ceil_div(d->W, TILE_COLS);
+  p.tiles_y = teco_ceil_div(d->H, TILE_ROWS);
+  const long long tiles = (long long)d->N * p.tiles_x * p.tiles_y;
+  TECO_CHECK_ARG(tiles < (1LL << 31), "teco_conv3x3_f32out_tc: too many tiles");
+  p.num_tiles = (int)tiles;
+  CUtensorMap tmap, omap, rmap;
+  int rc = encode_halo_map(&tmap, x, d->N, d->H, d->W, d->Cin, "teco_conv3x3_f32out_tc");
+  if (rc != TECO_OK) return rc;
+  rc = encode_f32_box_map(&omap, out_f32, d->N, d->H, d->W, p.C);
+  if (rc != TECO_OK) return rc;
+  rmap = omap;
+  if (res_f32) {
+    rc = encode_f32_box_map(&rmap, res_f32, d->N, d->H, d->W, p.C);
+    if (rc != TECO_OK) return rc;
+  }
+  int per_sm = 0;
+  rc = resident_ctas((const void*)conv3x3_f32out_kernel, F32_SMEM, &per_sm, WS_THREADS);
+  if (rc != TECO_OK) return rc;
+  const long long slots = (long long)per_sm * teco_sm_count();   // persistent: as many CTAs as are resident at once
+  const unsigned gx = (unsigned)(tiles < slots ? tiles : slots);
+  conv3x3_f32out_kernel<<<gx, WS_THREADS, F32_SMEM, stream>>>(tmap, omap, rmap, p);
+  TECO_CUDA_LAUNCH_CHECK("teco_conv3x3_f32out_tc");
+  return TECO_OK;
+}
+
 // The plans conv3x3_trunk_cluster_kernel runs: 32 x 32 images; layer 0 reads x_in (buffer 0) into buffer 1 without a
 // residual; every later layer reads the previous layer's output and writes the other one of buffers 1 and 2, with no
 // residual or an in-place one on a buffer an earlier layer wrote.  So layer l writes buffer 1 (slot 1) for even l and
@@ -1228,6 +1460,26 @@ extern "C" int teco_conv3x3_im2col_tc(const teco_tc_desc* d, const void* x, cons
   TECO_CHECK_ARG((((uintptr_t)x) & 15) == 0 && (((uintptr_t)wpk) & 15) == 0 && (((uintptr_t)y) & 15) == 0,
                  "teco_conv3x3_im2col_tc: tensors must be 16-byte aligned");
   return launch_conv3x3_im2col(d, x, wpk, bias, y, (cudaStream_t)stream);
+}
+
+extern "C" int teco_conv3x3_f32out_tc(const teco_tc_desc* d, const void* x, const void* wpk, const float* bias, const void* res,
+                                      void* y, const float* res_f32, float* out_f32, void* stream) {
+  TECO_CHECK_ARG(d && x && wpk && out_f32, "teco_conv3x3_f32out_tc: NULL argument");
+  TECO_CHECK_ARG(!res && !y, "teco_conv3x3_f32out_tc: fp32 output only (no bf16 output or residual)");
+  TECO_CHECK_ARG(d->N > 0 && d->H > 0 && d->W > 0, "teco_conv3x3_f32out_tc: bad shape N=%d H=%d W=%d", d->N, d->H, d->W);
+  TECO_CHECK_ARG(d->Cin == 64 && d->Cout == 16 && d->mode == 0,
+                 "teco_conv3x3_f32out_tc: mode 0 with Cin 64 and Cout 16 only (got mode %d, Cin %d, Cout %d)", d->mode, d->Cin,
+                 d->Cout);
+  TECO_CHECK_ARG(d->act >= 0 && d->act <= TECO_ACT_SIGMOID, "teco_conv3x3_f32out_tc: unknown activation %d", d->act);
+  TECO_CHECK_ARG(d->out_f32_c == 2 || d->out_f32_c == 3, "teco_conv3x3_f32out_tc: out_f32_c must be 2 or 3 (got %d)",
+                 d->out_f32_c);
+  TECO_CHECK_ARG(((long long)d->W * d->out_f32_c * 4) % 16 == 0,
+                 "teco_conv3x3_f32out_tc: an fp32 row (W*out_f32_c*4 = %lld bytes) must be a multiple of 16 bytes",
+                 (long long)d->W * d->out_f32_c * 4);
+  TECO_CHECK_ARG((((uintptr_t)x) & 15) == 0 && (((uintptr_t)wpk) & 15) == 0 && (((uintptr_t)res_f32) & 15) == 0 &&
+                     (((uintptr_t)out_f32) & 15) == 0,
+                 "teco_conv3x3_f32out_tc: tensors must be 16-byte aligned");
+  return launch_conv3x3_f32out(d, x, wpk, bias, res_f32, out_f32, (cudaStream_t)stream);
 }
 
 // Shapes of the 4x4 stride-2 convolution on its space-to-depth-2 form: even H, W; Cin a multiple of 64 with 4 * Cin <= 512

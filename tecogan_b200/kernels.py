@@ -532,6 +532,23 @@ def conv3x3_im2col_tc(x, wpk, bias, y=None, *, cout, act=ACT_NONE):
     return y
 
 
+def conv3x3_f32out_fits(W, C):
+    """Whether teco_conv3x3_f32out_tc takes an fp32 output of C channels on W-pixel-wide images: C is 2 or 3 and an
+    fp32 row of W * C values is a whole number of 16-byte units (the TMA row stride)."""
+    return C in (2, 3) and (W * C * 4) % 16 == 0
+
+
+def conv3x3_f32out_tc(x, wpk, bias, y=None, *, cout, act=ACT_NONE, out_f32, res_f32=None, post=(1.0, 0.0)):
+    """conv3x3_tc's fp32 output stage (Cin 64, cout 16, out_f32 [N,H,W,2 or 3]) on its pipelined kernel, bit-identical;
+    called as conv3x3_tc is.  y must be None."""
+    N, H, W, Cin = x.shape
+    d = TcDesc(N=N, H=H, W=W, Cin=Cin, Cout=cout, act=act, mode=0, out_f32_c=out_f32.shape[-1], post_scale=post[0],
+               post_shift=post[1])
+    call("teco_conv3x3_f32out_tc", d, ptr(x, bf16), ptr(wpk, bf16), ptr(bias, f32), ptr(None), ptr(y, bf16), ptr(res_f32, f32),
+         ptr(out_f32, f32), stream_ptr())
+    return out_f32
+
+
 def conv3x3_lin_supported(N, H, W, num_layers):
     from ._ffi import lib
     return bool(lib().teco_conv3x3_lin_supported(N, H, W, num_layers))
@@ -625,17 +642,24 @@ def _pad64(c):
     return (c + 63) // 64 * 64
 
 
-def _tc_packed(w, b, flags, cin_pad, cout_pad):
-    key = (w.data_ptr(), tuple(w.shape), flags, cin_pad, cout_pad)   # (an address alone can be reused by another weight)
+def _tc_cached(w, key, make):
+    """_tc_wcache[key], made by make() on a miss.  Keys start with w's address; the entry keeps w alive, so no other
+    tensor can be allocated at that address and be handed this packing before the cache is cleared."""
     hit = _tc_wcache.get(key)
     if hit is None:
+        hit = _tc_wcache[key] = (w, make())
+    return hit[1]
+
+
+def _tc_packed(w, b, flags, cin_pad, cout_pad):
+    def make():
         wpk = packed_weight(w.detach(), cin_pad, cout_pad, flags)
         bp = None
         if b is not None:
             bp = torch.zeros(cout_pad, device=w.device, dtype=f32)
             bp[: b.numel()].copy_(b.detach())
-        hit = _tc_wcache[key] = (wpk, bp)
-    return hit
+        return wpk, bp
+    return _tc_cached(w, (w.data_ptr(), tuple(w.shape), flags, cin_pad, cout_pad), make)
 
 
 def _to_bf16_rows(x, cpad):
@@ -788,12 +812,11 @@ class _ConvTranspose2xTC(torch.autograd.Function):
         idx = _tconv_index(w.device)
         dx = dw = db = None
         if ctx.needs_input_grad[0]:
-            key = (w.data_ptr(), tuple(w.shape), "tconv_dgrad")
-            wpk2 = _tc_wcache.get(key)
-            if wpk2 is None:
+            def make():
                 wp = torch.zeros((36, Cout, Cin), device=w.device, dtype=f32)
                 wp.index_copy_(0, idx, w.detach().reshape(9, Cout, Cin))
-                wpk2 = _tc_wcache[key] = packed_weight(wp.view(3, 3, 4 * Cout, Cin), 4 * Cout, Cin, 0)
+                return packed_weight(wp.view(3, 3, 4 * Cout, Cin), 4 * Cout, Cin, 0)
+            wpk2 = _tc_cached(w, (w.data_ptr(), tuple(w.shape), "tconv_dgrad"), make)
             dxb = conv3x3_tc(dzs, wpk2, None, cout=Cin, act=ACT_NONE)
             dx = _from_bf16_rows(dxb, Cin)
         if ctx.needs_input_grad[1]:
@@ -844,13 +867,12 @@ def _c4s2_index(device):
 
 
 def _c4s2_packed(w, dgrad):
-    key = (w.data_ptr(), tuple(w.shape), "c4s2", dgrad)
-    wpk = _tc_wcache.get(key)
-    if wpk is None:
+    def make():
         Cin, Cout = w.shape[2], w.shape[3]
-        wpk = _tc_wcache[key] = torch.empty(36 * Cin * Cout, device=w.device, dtype=bf16)
+        wpk = torch.empty(36 * Cin * Cout, device=w.device, dtype=bf16)
         call("teco_pack_conv4x4s2_bf16", ptr(_cc(w.detach()), f32), Cin, Cout, int(dgrad), ptr(wpk, bf16), stream_ptr())
-    return wpk
+        return wpk
+    return _tc_cached(w, (w.data_ptr(), tuple(w.shape), "c4s2", dgrad), make)
 
 
 class _Conv4x4S2TC(torch.autograd.Function):

@@ -126,6 +126,8 @@ class GeneratorPlan:
         self.bic = torch.zeros((B, 4 * h, 4 * w, 3), device=device, dtype=f32)
         self.out = torch.zeros((B, 4 * h, 4 * w, 3), device=device, dtype=f32)
         self.launches = 2 * num_resblock + 5 + 1
+        # the fp32 output stage on its pipelined kernel wherever that takes the shape (any HR width a multiple of 4)
+        self.out_conv = K.conv3x3_f32out_tc if K.conv3x3_f32out_fits(4 * w, 3) else K.conv3x3_tc
         # 32-pixel-wide frames: the whole trunk can run as one teco_conv3x3_lin_tc call; on 32x32 frames that is one
         # launch with the activations in shared memory, chosen from the batch unless config.set_lin_trunk forces it
         L = 2 * num_resblock + 1
@@ -166,8 +168,8 @@ class GeneratorPlan:
         K.conv3x3_tc(self.a, self.l_t1.wpk, self.l_t1.bias, self.u1, cout=64, act=ACT_RELU, mode=1)
         K.conv3x3_tc(self.u1, self.l_t2.wpk, self.l_t2.bias, self.u2, cout=64, act=ACT_RELU, mode=1)
         # output stage: conv(64->3) + bicubic_four(LR), then preprocess (*2-1): lib/frvsr.py:79-87
-        K.conv3x3_tc(self.u2, self.l_out.wpk, self.l_out.bias, None, cout=16, act=ACT_NONE, out_f32=self.out,
-                     res_f32=self.bic, post=(2.0, -1.0))
+        self.out_conv(self.u2, self.l_out.wpk, self.l_out.bias, None, cout=16, act=ACT_NONE, out_f32=self.out,
+                      res_f32=self.bic, post=(2.0, -1.0))
         return self.out
 
 
@@ -198,6 +200,7 @@ class FNetPlan:
         self.o1 = z(n, ch, cw, 64)
         self.flow = torch.zeros((n, ch, cw, 2), device=device, dtype=f32)
         self.launches = 14 + 6
+        self.head_conv = K.conv3x3_f32out_tc if K.conv3x3_f32out_fits(cw, 2) else K.conv3x3_tc
 
     def run(self, flow_out=None):
         """flow_out: optional fp32 [n,fh,fw,2] destination (default self.flow)."""
@@ -216,7 +219,7 @@ class FNetPlan:
                 call("teco_resize2x_bf16", ptr(t2, bf16), ptr(t3, bf16), n, hh, ww, cc, stream_ptr())
             x = t3
         K.conv3x3_tc(x, self.l_o1.wpk, self.l_o1.bias, self.o1, cout=64, act=ACT_LRELU02)
-        K.conv3x3_tc(self.o1, self.l_o2.wpk, self.l_o2.bias, None, cout=16, act=ACT_TANH24, out_f32=flow)
+        self.head_conv(self.o1, self.l_o2.wpk, self.l_o2.bias, None, cout=16, act=ACT_TANH24, out_f32=flow)
         return flow
 
 

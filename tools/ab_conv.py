@@ -9,7 +9,9 @@ clips of 32x32, in-place residual), every activation, ragged images, an image sm
 SMs, a tile count that is not a multiple of the grid, FNet's 64-channel layers and the input-gradient convolution
 (flag-3 packing).  It also covers the generator's HR tail at the bench batch, each launch on its own: conv_tran1
 (32x32 -> 64x64) and conv_tran2 (64x64 -> 128x128), the fp32 output stage at 128x128 with the bicubic residual, and
-FNet's tanh*24 flow head, with ragged and smaller-than-a-tile cases of each."""
+FNet's tanh*24 flow head, with ragged and smaller-than-a-tile cases of each.  The output-stage and flow-head cases that
+teco_conv3x3_f32out_tc takes run once more on it, as '<case>+f32out' with the same operands; --compare checks those
+against the teco_conv3x3_tc case of the same run byte for byte, and across the two runs where both have them."""
 import argparse
 import json
 import os
@@ -55,8 +57,17 @@ CASES = {
 }
 
 
-def run_case(name, spec, reps):
+F32OUT = "+f32out"          # suffix of a case run on teco_conv3x3_f32out_tc
+
+
+def f32out_cases():
     from tecogan_b200 import kernels as K
+    return [n for n, s in CASES.items() if s[9] and K.conv3x3_f32out_fits(s[2], s[9])]
+
+
+def run_case(name, spec, reps, conv=None):
+    from tecogan_b200 import kernels as K
+    conv = conv or K.conv3x3_tc
     N, H, W, cin, cout, act, res, flags, mode, f32c = spec
     g = torch.Generator(device="cuda").manual_seed(sum(map(ord, name)))
     x = torch.randn(N, H, W, cin, device="cuda", generator=g).to(torch.bfloat16)
@@ -73,7 +84,7 @@ def run_case(name, spec, reps):
         post = (2.0, -1.0) if res == "f32" else (1.0, 0.0)
 
         def launch():
-            K.conv3x3_tc(x, wpk, bias, cout=cout, act=act, out_f32=out, res_f32=rf, post=post)
+            conv(x, wpk, bias, cout=cout, act=act, out_f32=out, res_f32=rf, post=post)
     else:
         r0 = torch.randn(N, H, W, cout, device="cuda", generator=g).to(torch.bfloat16) if res else None
         out = torch.empty(N, s * H, s * W, cout, device="cuda", dtype=torch.bfloat16)
@@ -130,13 +141,18 @@ def main():
         ta, tb = (json.load(open(os.path.join(d, "times.json"))) for d in (a, b))
         same = True
         print("%-34s %-10s %10s %10s %9s %9s" % ("case", "outputs", "A us", "B us", "B TFLOP/s", "B GB/s"))
-        for name, spec in CASES.items():
-            xa, xb = (np.load(os.path.join(d, name + ".npy")) for d in (a, b))
-            eq = xa.shape == xb.shape and xa.tobytes() == xb.tobytes()
+        for name in [n for n in tb if n in ta or n.endswith(F32OUT)]:
+            spec = CASES[name[:-len(F32OUT)] if name.endswith(F32OUT) else name]
+            xb = np.load(os.path.join(b, name + ".npy"))
+            # a '+f32out' case equals the teco_conv3x3_tc case of its own run, and its counterpart in A if A has one
+            refs = [os.path.join(b, name[:-len(F32OUT)] + ".npy")] if name.endswith(F32OUT) else []
+            refs += [os.path.join(a, name + ".npy")] if name in ta else []
+            eq = all(xa.shape == xb.shape and xa.tobytes() == xb.tobytes() for xa in map(np.load, refs))
             same &= eq
             flop, nbytes = work(spec)
-            print("%-34s %-10s %10.1f %10.1f %9.1f %9.0f" % (name, "identical" if eq else "DIFFERENT", ta[name], tb[name],
-                                                             flop / tb[name] * 1e-6, nbytes / tb[name] * 1e-3))
+            print("%-34s %-10s %10s %10.1f %9.1f %9.0f" % (name, "identical" if eq else "DIFFERENT",
+                                                           "%.1f" % ta[name] if name in ta else "-", tb[name],
+                                                           flop / tb[name] * 1e-6, nbytes / tb[name] * 1e-3))
         print("all outputs bit-identical" if same else "OUTPUTS DIFFER")
         sys.exit(0 if same else 1)
     if not args.out:
@@ -150,6 +166,12 @@ def main():
         np.save(os.path.join(args.out, name + ".npy"), out)
         times[name] = us
         print("%-34s %9.1f us per launch" % (name, us), flush=True)
+    from tecogan_b200 import kernels as K
+    for name in f32out_cases():
+        out, us = run_case(name, CASES[name], args.reps, K.conv3x3_f32out_tc)
+        np.save(os.path.join(args.out, name + F32OUT + ".npy"), out)
+        times[name + F32OUT] = us
+        print("%-34s %9.1f us per launch" % (name + F32OUT, us), flush=True)
     with open(os.path.join(args.out, "times.json"), "w") as f:
         json.dump(times, f, indent=1)
 
