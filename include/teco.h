@@ -139,19 +139,18 @@ int teco_bias_grad_f32(const float* dy, float* db, int64_t npix, int32_t C, int3
 int teco_conv3x3_wgrad_tc(int32_t N, int32_t H, int32_t W, int32_t cin_pad, int32_t cout_pad, int32_t cin, int32_t cout,
                           const void* x, const void* dz, float* dw, int32_t accumulate, void* stream);
 
-/* Multi-layer 3x3 64->64 chain for 32-pixel-wide images (the metric configuration's 32x32 LR clips): the same
- * layers of generator_F (input conv + residual blocks, reference lib/frvsr.py:59-70) -- or any chain of conv2(3x3, 64->64) + bias + ReLU /
- * LeakyReLU / none + optional residual.  32x32 images with a generator-trunk-shaped plan (teco_conv3x3_lin_in_smem) run as
- * ONE launch whose activations stay in shared memory: a cluster of two CTAs owns each image through all layers.  Any
- * other plan or height runs one launch per layer, with the same results.
- * x_in / buf_a / buf_b: NHWC bf16 [N,H,32,64] (buffer ids 0 / 1 / 2; x_in is never written).
+/* Multi-layer 3x3 64->64 chain on 32x32 images (the metric configuration's LR clips) in ONE launch whose activations
+ * stay in shared memory: a cluster of two CTAs owns each image through all layers.  The plan has the shape of
+ * generator_F's input conv + residual blocks (reference lib/frvsr.py:59-70): conv2(3x3, 64->64) + bias + ReLU /
+ * LeakyReLU / none + optional in-place residual per layer.  The results are bit-identical to one teco_conv3x3_tc launch
+ * per layer.
+ * x_in / buf_a / buf_b: NHWC bf16 [N,32,32,64] (buffer ids 0 / 1 / 2; x_in is never written).
  * plan_host: HOST array [num_layers][4] = {input buffer id, output buffer id, residual buffer id or -1, TECO_ACT_*}.
- *   A residual may be added in place (residual id == output id); the input is never the output.
  * wpk_all: num_layers packed layers back to back (teco_pack_conv3x3_bf16, 64x64 -> 73728 bytes each); bias_all [num_layers][64].
- * teco_conv3x3_lin_in_smem: 1 when teco_conv3x3_lin_tc runs the plan as the one shared-memory launch -- H == W == 32; layer 0
- *   is {0, 1, -1, act}; layer l >= 1 reads layer l-1's output and writes the other of buffers 1 and 2, with no residual or an
- *   in-place one on a buffer an earlier layer wrote.  Host-only, needs no device. */
-int teco_conv3x3_lin_supported(int32_t N, int32_t H, int32_t W, int32_t num_layers);
+ * teco_conv3x3_lin_in_smem: 1 for exactly the shapes and plans teco_conv3x3_lin_tc takes -- N > 0; H == W == 32; 1..40
+ *   layers; layer 0 is {0, 1, -1, act}; layer l >= 1 reads layer l-1's output and writes the other of buffers 1 and 2,
+ *   with no residual or an in-place one on a buffer an earlier layer wrote; act is none, ReLU or LeakyReLU.  Host-only,
+ *   needs no device.  teco_conv3x3_lin_tc returns TECO_E_INVALID for anything else. */
 int teco_conv3x3_lin_tc(int32_t N, int32_t H, int32_t W, int32_t num_layers, const void* x_in, void* buf_a, void* buf_b,
                         const void* wpk_all, const float* bias_all, const int32_t* plan_host, void* stream);
 int teco_conv3x3_lin_in_smem(int32_t N, int32_t H, int32_t W, int32_t num_layers, const int32_t* plan_host);

@@ -51,7 +51,6 @@ SIGNATURES = {
     "teco_bf16_d2s2_to_f32": [_P, _P, _I32, _I32, _I32, _I32, _P],
     "teco_bias_grad_f32": [_P, _P, _I64, _I32, _I32, _I32, _P],
     "teco_conv3x3_wgrad_tc": [_I32, _I32, _I32, _I32, _I32, _I32, _I32, _P, _P, _P, _I32, _P],
-    "teco_conv3x3_lin_supported": [_I32, _I32, _I32, _I32],
     "teco_conv3x3_lin_tc": [_I32, _I32, _I32, _I32, _P, _P, _P, _P, _P, _P, _P],
     "teco_conv3x3_lin_in_smem": [_I32, _I32, _I32, _I32, _P],
     "teco_conv3x3_lin_clusters": [],

@@ -236,8 +236,8 @@ conv3x3_wgmma_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p)
   }
 }
 
-// teco_conv3x3_lin_tc: chains of 3x3 64 -> 64 layers on 32-pixel-wide images
-constexpr int LIN_W = 32, LIN_ROWS = 4, LIN_MAX_LAYERS = 40;
+// teco_conv3x3_lin_tc: chains of 3x3 64 -> 64 layers on 32 x 32 images
+constexpr int LIN_W = 32, LIN_MAX_LAYERS = 40;
 constexpr uint32_t LAYER_W_BYTES = 9u * 64u * 128u;   // one packed 64 x 64 layer: 73728
 
 // ------------------------------------------------------------------ warp-specialised 64 -> 64 layer (one K block)
@@ -1535,40 +1535,20 @@ extern "C" int teco_conv4x4s2_dgrad_tc(int32_t N, int32_t H, int32_t W, int32_t 
   return launch_conv3x3_s2d(&d, dz, wpk_t, nullptr, dxs, (cudaStream_t)stream);
 }
 
-extern "C" int teco_conv3x3_lin_supported(int32_t N, int32_t H, int32_t W, int32_t num_layers) {
-  return (N > 0 && W == LIN_W && H >= LIN_ROWS && H % LIN_ROWS == 0 && H <= 4096 && num_layers >= 1 && num_layers <= LIN_MAX_LAYERS) ? 1 : 0;
+extern "C" int teco_conv3x3_lin_in_smem(int32_t N, int32_t H, int32_t W, int32_t num_layers, const int32_t* plan_host) {
+  return N > 0 && plan_host && trunk_plan_fits(H, W, num_layers, plan_host) ? 1 : 0;
 }
 
 extern "C" int teco_conv3x3_lin_tc(int32_t N, int32_t H, int32_t W, int32_t num_layers, const void* x_in, void* buf_a, void* buf_b,
                                    const void* wpk_all, const float* bias_all, const int32_t* plan_host, void* stream) {
-  TECO_CHECK_ARG(teco_conv3x3_lin_supported(N, H, W, num_layers),
-                 "teco_conv3x3_lin_tc: needs W == 32, H a multiple of 4, 1..%d layers (got N=%d H=%d W=%d L=%d)", LIN_MAX_LAYERS, N, H, W, num_layers);
-  TECO_CHECK_ARG(x_in && buf_a && buf_b && wpk_all && bias_all && plan_host, "teco_conv3x3_lin_tc: NULL argument");
+  TECO_CHECK_ARG(teco_conv3x3_lin_in_smem(N, H, W, num_layers, plan_host),
+                 "teco_conv3x3_lin_tc: needs N > 0, 32x32 images and a generator-trunk-shaped plan of 1..%d layers "
+                 "(teco_conv3x3_lin_in_smem; got N=%d H=%d W=%d L=%d)", LIN_MAX_LAYERS, N, H, W, num_layers);
+  TECO_CHECK_ARG(x_in && buf_a && buf_b && wpk_all && bias_all, "teco_conv3x3_lin_tc: NULL argument");
   TECO_CHECK_ARG((((uintptr_t)x_in) & 15) == 0 && (((uintptr_t)buf_a) & 15) == 0 && (((uintptr_t)buf_b) & 15) == 0 &&
                      (((uintptr_t)wpk_all) & 15) == 0,
                  "teco_conv3x3_lin_tc: tensors must be 16-byte aligned");
-  for (int l = 0; l < num_layers; ++l) {
-    const int32_t* pl = plan_host + 4 * l;
-    TECO_CHECK_ARG(pl[0] >= 0 && pl[0] <= 2 && (pl[1] == 1 || pl[1] == 2) && pl[0] != pl[1] && pl[2] >= -1 && pl[2] <= 2 &&
-                       pl[3] >= 0 && pl[3] < TECO_ACT_TANH24,
-                   "teco_conv3x3_lin_tc: bad plan row %d {%d, %d, %d, %d}", l, pl[0], pl[1], pl[2], pl[3]);
-  }
-  if (trunk_plan_fits(H, W, num_layers, plan_host))
-    return launch_trunk(N, num_layers, x_in, buf_a, buf_b, wpk_all, bias_all, plan_host, (cudaStream_t)stream);
-  // any other plan or height: one conv3x3_ws_kernel<0> launch per layer
-  void* bufs[3] = {const_cast<void*>(x_in), buf_a, buf_b};
-  for (int l = 0; l < num_layers; ++l) {
-    const int32_t* pl = plan_host + 4 * l;
-    const teco_tc_desc d = {N, H, W, 64, 64, pl[3], 0, 0, 1.f, 0.f};
-    const int rc = launch_conv3x3(&d, bufs[pl[0]], (const uint8_t*)wpk_all + (size_t)l * LAYER_W_BYTES, bias_all + 64 * l,
-                                  pl[2] >= 0 ? bufs[pl[2]] : nullptr, bufs[pl[1]], nullptr, nullptr, (cudaStream_t)stream);
-    if (rc != TECO_OK) return rc;
-  }
-  return TECO_OK;
-}
-
-extern "C" int teco_conv3x3_lin_in_smem(int32_t N, int32_t H, int32_t W, int32_t num_layers, const int32_t* plan_host) {
-  return plan_host && teco_conv3x3_lin_supported(N, H, W, num_layers) && trunk_plan_fits(H, W, num_layers, plan_host) ? 1 : 0;
+  return launch_trunk(N, num_layers, x_in, buf_a, buf_b, wpk_all, bias_all, plan_host, (cudaStream_t)stream);
 }
 
 extern "C" int teco_conv3x3_lin_clusters(void) {

@@ -549,11 +549,6 @@ def conv3x3_f32out_tc(x, wpk, bias, y=None, *, cout, act=ACT_NONE, out_f32, res_
     return out_f32
 
 
-def conv3x3_lin_supported(N, H, W, num_layers):
-    from ._ffi import lib
-    return bool(lib().teco_conv3x3_lin_supported(N, H, W, num_layers))
-
-
 def _flat_plan(plan):
     import ctypes
     flat = (ctypes.c_int32 * (4 * len(plan)))(*[int(v) for row in plan for v in row])
@@ -561,8 +556,8 @@ def _flat_plan(plan):
 
 
 def conv3x3_lin_in_smem(N, H, W, plan):
-    """True when conv3x3_lin_chain runs `plan` as one launch with the activations in shared memory (32x32 images, a
-    generator-trunk-shaped plan); otherwise it issues one launch per layer."""
+    """True when conv3x3_lin_chain takes `plan` on N images of H x W (32x32 images, a generator-trunk-shaped plan); it
+    raises ValueError for anything else."""
     from ._ffi import lib
     p, _keep = _flat_plan(plan)
     return bool(lib().teco_conv3x3_lin_in_smem(N, H, W, len(plan), p))
@@ -578,7 +573,8 @@ def conv3x3_lin_clusters():
 
 
 def conv3x3_lin_chain(x_in, buf_a, buf_b, wpk_all, bias_all, plan):
-    """A chain of 3x3 64->64 layers on 32-pixel-wide images (teco_conv3x3_lin_tc).  x_in / buf_a / buf_b: [N,H,32,64] bf16
+    """A chain of 3x3 64->64 layers on 32x32 images in one launch with the activations in shared memory
+    (teco_conv3x3_lin_tc; the plans conv3x3_lin_in_smem accepts).  x_in / buf_a / buf_b: [N,32,32,64] bf16
     (buffer ids 0 / 1 / 2); plan: list of (input id, output id, residual id or -1, activation) per layer; wpk_all: the
     packed layers back to back; bias_all: [L,64] fp32."""
     N, H, W, C = x_in.shape

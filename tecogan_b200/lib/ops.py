@@ -40,7 +40,7 @@ def conv2_tran(batch_input, kernel=3, output_channel=64, stride=1, use_bias=True
         w = get_variable('weights', (kernel, kernel, output_channel, cin),
                          fans=(kernel * kernel * output_channel, kernel * kernel * cin))
         b = get_variable('biases', (output_channel,), init='zeros') if use_bias else None
-    if (config.training_kernels(torch.is_grad_enabled()) and config.train_precision() == "bf16" and config.train_tc_all()
+    if (config.training_kernels(torch.is_grad_enabled()) and config.train_precision() == "bf16"
             and cin == 64 and output_channel == 64 and act in (ACT_NONE, ACT_RELU, ACT_LRELU02)):
         return K.conv_transpose2x_train_tc(batch_input, w, b, act)   # wgmma forward, input and weight gradients
     return K.conv2d_transpose(batch_input, w, b, act)
@@ -56,11 +56,10 @@ def conv2(batch_input, kernel=3, output_channel=64, stride=1, use_bias=True, sco
                          fans=(kernel * kernel * cin, kernel * kernel * output_channel))
         b = get_variable('biases', (output_channel,), init='zeros') if use_bias else None
     if (kernel == 3 and stride == 1 and config.training_kernels(torch.is_grad_enabled()) and config.train_precision() == "bf16"
-            and (output_channel >= 16 or config.train_tc_all())
             and (act in (ACT_NONE, ACT_RELU, ACT_LRELU02) or (act == ACT_TANH24 and output_channel < 16 and res is None))):
         return K.conv3x3_train_tc(batch_input, w, b, act, res)      # wgmma forward, input and weight gradients
     if (kernel == 4 and stride == 2 and config.training_kernels(torch.is_grad_enabled()) and config.train_precision() == "bf16"
-            and config.train_tc_all() and K.conv4x4s2_tc_fits(batch_input.shape[1], batch_input.shape[2], cin, output_channel)
+            and K.conv4x4s2_tc_fits(batch_input.shape[1], batch_input.shape[2], cin, output_channel)
             and act in (ACT_NONE, ACT_RELU, ACT_LRELU02) and res is None):
         return K.conv4x4s2_train_tc(batch_input, w, b, act)         # the discriminator's disblocks, through space-to-depth-2
     return K.conv2d(batch_input, w, b, stride, act, res)

@@ -9,7 +9,6 @@ import ctypes
 
 import torch
 
-from . import config
 from . import kernels as K
 from ._ffi import ACT_LRELU02, ACT_NONE, ACT_RELU, ACT_TANH24, call, ptr, stream_ptr
 from .variables import current_scope, default_store
@@ -104,6 +103,12 @@ def _ensure_vars_fnet():
         conv('conv2', 32, 2)
 
 
+# A round of the one-launch trunk takes about as long whether it holds 1 or G clips, while the per-layer launches scale
+# with the batch: on an H100 SXM (700 W) the one launch was 1.20-1.32x faster at 66, 132, 198 and 264 clips (full rounds)
+# and 0.71-0.81x at 8 and 67 (1 / 8 and 1 / 2 of a round used); see tools/ab_trunk.py and DESIGN 4.1b.
+LIN_TRUNK_MIN_FILL = 0.8
+
+
 class GeneratorPlan:
     """Pre-allocated buffers + packed layers for one (B,h,w) generator shape; `run` issues 2N+5 wgmma launches
     and one bicubic kernel, with no allocation -- safe to capture in a CUDA graph."""
@@ -128,23 +133,18 @@ class GeneratorPlan:
         self.launches = 2 * num_resblock + 5 + 1
         # the fp32 output stage on its pipelined kernel wherever that takes the shape (any HR width a multiple of 4)
         self.out_conv = K.conv3x3_f32out_tc if K.conv3x3_f32out_fits(4 * w, 3) else K.conv3x3_tc
-        # 32-pixel-wide frames: the whole trunk can run as one teco_conv3x3_lin_tc call; on 32x32 frames that is one
-        # launch with the activations in shared memory, chosen from the batch unless config.set_lin_trunk forces it
-        L = 2 * num_resblock + 1
+        # 32x32 frames: the whole trunk can run as one teco_conv3x3_lin_tc launch with the activations in shared memory,
+        # taken when the batch fills its rounds of clusters
+        # buffer ids: 0 = x_in, 1 = a, 2 = b.  input conv x_in -> a (ReLU); block: a -> b (ReLU), b -> a (+ a)
+        plan = [(0, 1, -1, ACT_RELU)] + [(1, 2, -1, ACT_RELU), (2, 1, 1, ACT_NONE)] * num_resblock
         self.lin = False
-        if K.conv3x3_lin_supported(B, h, w, L):
+        if K.conv3x3_lin_in_smem(B, h, w, plan):
             layers = [self.l_in] + [l for pair in self.l_res for l in pair]
             self.trunk_w = torch.cat([l.wpk for l in layers]).contiguous()
             self.trunk_b = torch.cat([l.bias for l in layers]).contiguous()
-            # buffer ids: 0 = x_in, 1 = a, 2 = b.  input conv x_in -> a (ReLU); block: a -> b (ReLU), b -> a (+ a)
-            self.trunk_plan = [(0, 1, -1, ACT_RELU)] + [(1, 2, -1, ACT_RELU), (2, 1, 1, ACT_NONE)] * num_resblock
-            forced = config.lin_trunk()
-            if forced is None:
-                G = K.conv3x3_lin_clusters()
-                self.lin = (K.conv3x3_lin_in_smem(B, h, w, self.trunk_plan) and
-                            B >= config.LIN_TRUNK_MIN_FILL * G * -(-B // G))
-            else:
-                self.lin = forced and B >= 8
+            self.trunk_plan = plan
+            G = K.conv3x3_lin_clusters()
+            self.lin = B >= LIN_TRUNK_MIN_FILL * G * -(-B // G)
         if self.lin:
             self.launches = 1 + 4 + 1
 

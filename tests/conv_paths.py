@@ -1,12 +1,12 @@
 """Host restatement of how teco_conv3x3_tc, teco_conv3x3_lin_tc and teco_conv3x3_wgrad_tc split a launch into kernels,
 Cout slices and tiles (csrc/conv_tc.cu, csrc/conv_wgrad_tc.cu), and of which code paths a launch reaches.
 
-route() mirrors launch_conv3x3 (conv_tc.cu:686-750) and pick_kernel (conv_tc.cu:660-665):
-  * nt = 64 output channels per CTA when Cout % 64 == 0 in mode 0, else 32 when Cout % 32 == 0, else 16 (conv_tc.cu:696);
+route() mirrors launch_conv3x3 and pick_kernel in conv_tc.cu:
+  * nt = 64 output channels per CTA when Cout % 64 == 0 in mode 0, else 32 when Cout % 32 == 0, else 16 (launch_conv3x3);
   * one 64-channel input block, 64-channel output slices, no fp32 output, and no residual in mode 1 run on
-    conv3x3_ws_kernel<mode> (conv_tc.cu:715), whose 72 KB of weights are always resident;
-  * everything else runs on conv3x3_wgmma_kernel<mode, nt>, with the weights resident when all Cin / 64 blocks fit next
-    to two halo stages (conv_tc.cu:704-705), otherwise streamed with each block.
+    conv3x3_ws_kernel<mode> (launch_conv3x3), whose 72 KB of weights are always resident;
+  * everything else runs on conv3x3_wgmma_kernel<mode, nt> (pick_kernel), with the weights resident when all Cin / 64
+    blocks fit next to two halo stages (launch_conv3x3's p.resident), otherwise streamed with each block.
 From that arithmetic: <0,64> is resident for Cin / 64 <= 2, <0,32> and <1,32> for Cin / 64 <= 4, <., 16> always.
 
 features() names what one launch reaches: the kernel, its activation, residual kind, Cout, output split, whether the
@@ -16,14 +16,17 @@ profiler sees.
 """
 from collections import namedtuple
 
-SMEM_MAX = 232448                                  # conv_tc.cu:43
-HALO_STAGE = 24576                                 # conv_tc.cu:41: 18 x 10 x 128 B rounded up to 1024
-TILE_ROWS, TILE_COLS = 16, 8                       # conv_tc.cu:35-36
+SMEM_MAX = 232448                                  # conv_tc.cu SMEM_MAX
+HALO_STAGE = 24576                                 # conv_tc.cu HALO_STAGE: 18 x 10 x 128 B rounded up to 1024
+TILE_ROWS, TILE_COLS = 16, 8                       # conv_tc.cu TILE_ROWS, TILE_COLS
 H100_SMS = 132
 # Every conv_tc instance needs at least 50 KB of shared memory (two halo stages), so at most four CTAs fit on an SM and a
 # persistent grid has at most 4 x SMs slots (H100 SXM: 132 SMs; fewer SMs only lower the bound).
 MAX_SLOTS = 4 * H100_SMS
-WG_ROWS, WG_COLS = 8, 16                           # conv_wgrad_tc.cu:21: weight-gradient tile
+# conv3x3_trunk_cluster_kernel: clusters of two CTAs, one CTA per SM, so at most SMs / 2 clusters are resident at once
+MAX_CLUSTERS = H100_SMS // 2
+TR_WSLOTS = 8                                      # conv_tc.cu TR_WSLOTS: weight ring depth in 3x3 taps
+WG_ROWS, WG_COLS = 8, 16                           # conv_wgrad_tc.cu WG_ROWS, WG_COLS: weight-gradient tile
 ACT_NAMES = ("none", "relu", "lrelu", "tanh24", "sigmoid")
 
 Route = namedtuple("Route", "kernel nt nsplit resident")
@@ -86,17 +89,16 @@ def features(mode, n, h, w, cin, cout, act, bias=True, res="", y=True, f32c=0, r
 
 
 def lin_features(n, h, plan):
-    """teco_conv3x3_lin_tc: one CTA per image (conv_tc.cu:816-821), two weight buffers used by layers in turn."""
-    out = {"lin L=%d" % len(plan)}
-    if len(plan) > 2:
-        out.add("lin weight buffers wrap")
-    if n > H100_SMS:
-        out.add("lin images>SMs")
+    """teco_conv3x3_lin_tc on n 32x32 images (h is 32): conv3x3_trunk_cluster_kernel, one cluster per image at a time
+    over a persistent grid of clusters, every layer's nine taps streamed through a TR_WSLOTS-deep weight ring."""
+    out = {"lin L=%d" % len(plan), "lin last output in buffer %d" % plan[-1][1]}
+    if 9 * len(plan) > 2 * TR_WSLOTS:
+        out.add("lin weight ring wraps")          # the ring's barriers run through both phase parities
+    if n > MAX_CLUSTERS:
+        out.add("lin clips>clusters")             # a cluster runs several clips: x_in reloaded, partner handshake
     for i, o, r, act in plan:
-        if r == o:
-            out.add("lin res=inplace")
-        elif r >= 0:
-            out.add("lin res=sep")
+        if r >= 0:
+            out.add("lin res=inplace on buffer %d" % r)
         out.add("lin act=%s" % ACT_NAMES[act])
     return out
 

@@ -108,7 +108,7 @@ def dispatch(monkeypatch):
     config.set_train_precision(prev)
 
 
-def test_dispatch_rule(dispatch, monkeypatch):
+def test_dispatch_rule(dispatch):
     assert dispatch((2, 128, 128, 64)) == "tc"
     assert dispatch((2, 16, 16, 128), cout=256) == "tc"
     assert dispatch((2, 127, 128, 64)) == "fp32"          # odd sizes: TF's SAME padding is not one row before
@@ -120,8 +120,5 @@ def test_dispatch_rule(dispatch, monkeypatch):
     assert dispatch((2, 32, 32, 64), grad=False) == "fp32"   # inference
     with config.train_forward():
         assert dispatch((2, 32, 32, 64), grad=False) == "tc"  # the trainer's evaluate() runs the step's kernels
-    monkeypatch.setitem(config._cfg, "train_tc_all", False)  # TECO_TRAIN_TC_ALL=0
-    assert dispatch((2, 128, 128, 64)) == "fp32"
-    monkeypatch.setitem(config._cfg, "train_tc_all", True)
     config.set_train_precision("fp32")
     assert dispatch((2, 128, 128, 64)) == "fp32"

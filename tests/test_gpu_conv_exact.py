@@ -101,18 +101,18 @@ REQUIRED = (
      "wgmma<0,16> res=inplace",
      "wgmma<1,32> cin=128", "wgmma<1,32> res=sep", "wgmma<1,32> out_f32", "wgmma<1,16> cout=48"})
 
-# teco_conv3x3_lin_tc: the plans of test_gpu_kernels.py::test_conv3x3_lin_chain_matches_oracle_on_bf16_operands, with
-# (input buffer, output buffer, residual buffer or -1, activation) per layer.  LeakyReLU only on a last layer: 0.2 v leaves
-# the grid the next layer needs.
+# teco_conv3x3_lin_tc: 32x32 images and trunk-shaped plans (the only ones it takes), with (input buffer, output buffer,
+# residual buffer or -1, activation) per layer.  LeakyReLU only on a last layer: 0.2 v leaves the grid the next layer needs.
 LIN_CASES = {
-    "one_strip": (1, 4, [(0, 1, -1, RELU)]),
     "linear": (3, 32, [(0, 1, -1, NONE)]),
-    "external_res_lrelu": (5, 8, [(0, 1, 2, LRELU)]),
+    "lrelu_into_b": (4, 32, [(0, 1, -1, RELU), (1, 2, -1, LRELU)]),
+    "inplace_res_lrelu_on_b": (5, 32, [(0, 1, -1, RELU), (1, 2, -1, RELU), (2, 1, -1, RELU), (1, 2, 2, LRELU)]),
     "res_block": (2, 32, [(0, 1, -1, RELU), (1, 2, -1, RELU), (2, 1, 1, NONE)]),
     "images_gt_sms": (150, 32, [(0, 1, -1, RELU), (1, 2, -1, RELU), (2, 1, 1, NONE), (1, 2, -1, RELU), (2, 1, 1, NONE)]),
-    "nine_layers": (7, 12, [(0, 1, -1, RELU)] + [(1, 2, -1, RELU), (2, 1, 1, NONE)] * 4),
+    "nine_layers_weight_ring": (7, 32, [(0, 1, -1, RELU)] + [(1, 2, -1, RELU), (2, 1, 1, NONE)] * 4),
 }
-LIN_REQUIRED = {"lin L=9", "lin weight buffers wrap", "lin images>SMs", "lin res=inplace", "lin res=sep", "lin act=lrelu"}
+LIN_REQUIRED = {"lin L=1", "lin L=9", "lin weight ring wraps", "lin clips>clusters", "lin res=inplace on buffer 1",
+                "lin res=inplace on buffer 2", "lin last output in buffer 2", "lin act=none", "lin act=relu", "lin act=lrelu"}
 
 # teco_conv3x3_wgrad_tc: the shapes of test_gpu_kernels.py::test_conv3x3_wgrad_tc_matches_autograd_on_bf16_operands
 WGRAD_CASES = [(1, 8, 16, 64, 64), (4, 32, 32, 64, 64), (2, 19, 21, 51, 64), (3, 16, 24, 128, 32), (2, 32, 32, 32, 256),
@@ -127,7 +127,9 @@ def _case_features(c):
 def test_case_tables_reach_every_required_path():
     """Host restatement of the dispatch (tests/conv_paths.py): each case reaches the paths it claims, and together the
     tables reach every kernel instance of teco_conv3x3_tc with each epilogue feature listed in REQUIRED, the chain's
-    weight-buffer wrap, residual kinds and more images than SMs, and the weight gradient's ragged and narrow shapes."""
+    weight-ring wrap, in-place residuals on either buffer and more clips than clusters (on plans its entry takes), and the
+    weight gradient's ragged and narrow shapes."""
+    from tecogan_b200 import kernels as K
     seen = set()
     for name, c in CASES.items():
         got = _case_features(c)
@@ -145,8 +147,9 @@ def test_case_tables_reach_every_required_path():
     assert route(0, 512, 16).resident and route(1, 512, 48).resident
     lin = set().union(*(lin_features(*v) for v in LIN_CASES.values()))
     assert LIN_REQUIRED <= lin, sorted(LIN_REQUIRED - lin)
-    for _, _, plan in LIN_CASES.values():
+    for n, h, plan in LIN_CASES.values():
         assert all(act != LRELU for _, _, _, act in plan[:-1])
+        assert K.conv3x3_lin_in_smem(n, h, 32, plan), plan
     wg = set().union(*(wgrad_features(*s) for s in WGRAD_CASES))
     assert WGRAD_REQUIRED <= wg, sorted(WGRAD_REQUIRED - wg)
 

@@ -149,30 +149,6 @@ def test_graph_replay_repacks_updated_weights():
     torch.testing.assert_close(outs[2], want[2], rtol=1e-5, atol=1e-5)
 
 
-@pytest.mark.parametrize("H,Cin,Cout", [(32, 64, 64), (16, 64, 128), (8, 128, 256)])
-def test_tc_all_off_runs_the_fp32_kernels_bit_for_bit(H, Cin, Cout, monkeypatch):
-    """TECO_TRAIN_TC_ALL=0: a disblock conv2() of the bf16 training graph is the fp32 K.conv2d, forward and gradients."""
-    from tecogan_b200 import config, kernels as K
-    from tecogan_b200.lib import ops
-    from tecogan_b200.variables import variable_scope
-    g = torch.Generator().manual_seed(H)
-    w = torch.randn(4, 4, Cin, Cout, generator=g) * 0.05
-    _fresh_store({"d/conv1/Conv/weights": w})
-    x = torch.randn(2, H, H, Cin, generator=g).cuda().requires_grad_(True)
-    dz = torch.randn(2, H // 2, H // 2, Cout, generator=g).cuda()
-    monkeypatch.setitem(config._cfg, "train_tc_all", False)
-    config.set_train_precision("bf16")
-    try:
-        with variable_scope("d"):
-            y = ops.conv2(x, 4, Cout, 2, use_bias=False, scope="conv1")
-    finally:
-        config.set_train_precision("fp32")
-    w_dev = x.new_tensor(w).requires_grad_(True)
-    y_ref = K.conv2d(x, w_dev, None, 2)
-    assert torch.equal(y, y_ref)
-    assert torch.equal(torch.autograd.grad(y, x, dz)[0], torch.autograd.grad(y_ref, x, dz)[0])
-
-
 def test_bf16_discriminator_close_to_reference_golden():
     """discriminator_F of the bf16 training graph (all four disblocks on the tensor cores) against the reference's golden
     at the bf16 tolerances of the training-step tests."""

@@ -330,29 +330,27 @@ def _lin_chain_reference(x, layers, plan):
 
 
 @pytest.mark.parametrize("n,h,plan", [
-    (1, 4, [(0, 1, -1, 1)]),                                               # one strip: every row is top and bottom padding
+    (1, 32, [(0, 1, -1, 1)]),
     (3, 32, [(0, 1, -1, 0)]),
-    (5, 8, [(0, 1, 2, 2)]),                                                # external residual from buf_b, LeakyReLU
+    (5, 32, [(0, 1, -1, 1), (1, 2, -1, 1), (2, 1, -1, 1), (1, 2, 2, 2)]),     # in-place residual on buf_b, LeakyReLU
     (2, 32, [(0, 1, -1, 1), (1, 2, -1, 1), (2, 1, 1, 0)]),                  # input conv + one residual block (in-place residual)
     (150, 32, [(0, 1, -1, 1), (1, 2, -1, 1), (2, 1, 1, 0), (1, 2, -1, 1), (2, 1, 1, 0)]),   # > 132 images: more images than SMs
-    (7, 12, [(0, 1, -1, 1)] + [(1, 2, -1, 1), (2, 1, 1, 0)] * 4),            # 9 layers: weight double buffer wraps
-])
+    (7, 32, [(0, 1, -1, 1)] + [(1, 2, -1, 1), (2, 1, 1, 0)] * 4),            # 9 layers: the weight ring wraps
+], ids=["relu", "linear", "inplace_res_lrelu_on_b", "res_block", "images_gt_sms", "nine_layers"])
 def test_conv3x3_lin_chain_matches_oracle_on_bf16_operands(n, h, plan):
-    """teco_conv3x3_lin_tc: the multi-layer chain on 32-pixel-wide images in one launch (CTA-local images across layers)."""
+    """teco_conv3x3_lin_tc: the multi-layer chain on 32x32 images in one launch (each image owned by one cluster across
+    layers)."""
     from tecogan_b200 import kernels as K
     L = len(plan)
     x = _bf(rnd(1, n, h, 32, 64))
-    ext = _bf(rnd(5, n, h, 32, 64))                                         # initial content of buf_b (external residual case)
     layers = [(_bf(rnd(10 + l, 3, 3, 64, 64) * (1.5 / 24.0)), rnd(50 + l, 64) * 0.1) for l in range(L)]
-    ref = _lin_chain_reference(x, layers, plan) if plan[0][2] < 0 else None
-    if ref is None:                                                          # single layer with the external residual
-        (wt, b), (_, _, _, act) = layers[0], plan[0]
-        ref = {1: _bf(O.lrelu(O.conv2d(x, wt, b)) + ext)}
-    assert K.conv3x3_lin_supported(n, h, 32, L) and not K.conv3x3_lin_supported(n, h, 40, L) and not K.conv3x3_lin_supported(n, 6, 32, L)
+    ref = _lin_chain_reference(x, layers, plan)
+    assert K.conv3x3_lin_in_smem(n, h, 32, plan) and not K.conv3x3_lin_in_smem(n, h, 40, plan)
+    assert not K.conv3x3_lin_in_smem(n, 6, 32, plan)
     wall = torch.cat([K.packed_weight(dev(wt), 64, 64) for wt, _ in layers]).contiguous()
     ball = torch.cat([dev(b) for _, b in layers]).contiguous()
     a = torch.zeros(n, h, 32, 64, device="cuda", dtype=torch.bfloat16)
-    bb = dev(ext).to(torch.bfloat16)
+    bb = torch.zeros_like(a)
     K.conv3x3_lin_chain(dev(x).to(torch.bfloat16), a, bb, wall, ball, plan)
     torch.cuda.synchronize()
     final = plan[-1][1]
@@ -361,8 +359,26 @@ def test_conv3x3_lin_chain_matches_oracle_on_bf16_operands(n, h, plan):
     assert_close(got, ref[final], 2e-3 * L, 1.0 / 128 * (1 + 0.5 * (L - 1)), what="conv3x3_lin chain (%d layers)" % L)
     if L == 1:
         # a single layer is the same arithmetic as teco_conv3x3_tc up to the fp32 summation order
-        other = K.conv3x3_tc(dev(x).to(torch.bfloat16), wall, ball, cout=64, act=plan[0][3], res=dev(ext).to(torch.bfloat16) if plan[0][2] >= 0 else None)
+        other = K.conv3x3_tc(dev(x).to(torch.bfloat16), wall, ball, cout=64, act=plan[0][3])
         assert (got.float() - other.float()).abs().max().item() <= 2.0 ** -6 * max(1.0, got.float().abs().max().item())
+
+
+def test_conv3x3_lin_chain_rejects_what_the_cluster_kernel_does_not_run():
+    """teco_conv3x3_lin_tc runs conv3x3_trunk_cluster_kernel and nothing else: images other than 32x32 and plans that are
+    not trunk-shaped (a residual from a buffer the chain has not written) raise ValueError before any launch."""
+    from tecogan_b200 import kernels as K
+    one = [(0, 1, -1, 1)]
+    nine = [(0, 1, -1, 1)] + [(1, 2, -1, 1), (2, 1, 1, 0)] * 4
+    external_res = [(0, 1, 2, 2)]
+    for n, h, w, plan in ((1, 4, 32, one), (7, 12, 32, nine), (5, 8, 32, external_res), (5, 32, 32, external_res),
+                          (1, 64, 32, one), (1, 32, 40, one), (2, 32, 32, [(0, 2, -1, 1)])):
+        assert not K.conv3x3_lin_in_smem(n, h, w, plan), (n, h, w, plan)
+        x = torch.zeros(n, h, w, 64, device="cuda", dtype=torch.bfloat16)
+        a, bb = torch.zeros_like(x), torch.zeros_like(x)
+        wall = torch.zeros(len(plan) * 9 * 64 * 64, device="cuda", dtype=torch.bfloat16)
+        ball = torch.zeros(len(plan), 64, device="cuda")
+        with pytest.raises(ValueError, match="teco_conv3x3_lin_tc"):
+            K.conv3x3_lin_chain(x, a, bb, wall, ball, plan)
 
 
 @pytest.mark.parametrize("n,h,w", [(1, 16, 8), (1, 32, 32), (2, 24, 20), (1, 64, 64), (5, 128, 128), (40, 64, 64), (3, 144, 120)])

@@ -215,7 +215,8 @@ def _y_psnr_delta(frames_lr, ours01, ref01):
 @pytest.mark.parametrize("B", [6, 12])
 def test_metric_config_clip_engine_matches_oracle_and_streaming_engine(B):
     """bench.py headline path: B clips x 10 frames 32x32 in lock-step, one CUDA graph, fnet for all pairs first.
-    B = 12 takes the one-launch trunk (teco_conv3x3_lin_tc, batches of >= 8 clips), B = 6 one launch per layer."""
+    B = 12 is put on the one-launch trunk (teco_conv3x3_lin_tc, which its batch alone would not pick), B = 6 stays on
+    one launch per layer."""
     from tecogan_b200 import config
     from tecogan_b200.engine import ClipEngine, InferenceEngine
     T, N = 10, 16
@@ -223,17 +224,20 @@ def test_metric_config_clip_engine_matches_oracle_and_streaming_engine(B):
     clips = _smooth_clips(T, B, 32, 32, seed=3)
     _fresh_store({**pg, **pf})
     config.set_precision("bf16")
-    prev_lin = config.lin_trunk()
-    config.set_lin_trunk(True)                           # the one-launch chain at B >= 8; the per-layer kernels below
-    eng = ClipEngine(32, 32, T, N, batch=B)
-    assert eng.gen.lin == (B >= 8)
+
+    def trunk(engine):                                   # the one-launch chain at B >= 8, set before the first run
+        if B >= 8:
+            engine.gen.lin = True
+        assert engine.gen.lin == (B >= 8)
+        return engine
+    eng = trunk(ClipEngine(32, 32, T, N, batch=B))
     u8 = eng.run(clips.cuda()).clone()
     u8_again = eng.run(clips.cuda()).clone()            # second replay of the captured graph: same bits
     assert torch.equal(u8, u8_again)
-    eager = ClipEngine(32, 32, T, N, batch=B, use_graph=False).run(clips.cuda())
+    eager = trunk(ClipEngine(32, 32, T, N, batch=B, use_graph=False)).run(clips.cuda())
     assert torch.equal(u8, eager)
     # same kernels as the streaming engine at the same batch -> bit-identical frames
-    stream = InferenceEngine(32, 32, N, batch=B).run_sequence([clips[t].cuda() for t in range(T)], out="u8")
+    stream = trunk(InferenceEngine(32, 32, N, batch=B)).run_sequence([clips[t].cuda() for t in range(T)], out="u8")
     for t in range(T):
         assert torch.equal(u8[t], stream[t]), t
     # against the oracle, clip by clip (fp32 CPU restatement of main.py:253-268)
@@ -248,16 +252,11 @@ def test_metric_config_clip_engine_matches_oracle_and_streaming_engine(B):
     assert worst_dy < 0.05, worst_dy
     if B >= 8:
         # the per-layer kernels on the same clips: same arithmetic up to the fp32 summation order inside a layer
-        config.set_lin_trunk(False)
-        try:
-            per_layer = ClipEngine(32, 32, T, N, batch=B)
-            assert not per_layer.gen.lin
-            u8_pl = per_layer.run(clips.cuda())
-        finally:
-            config.set_lin_trunk(prev_lin)
+        per_layer = ClipEngine(32, 32, T, N, batch=B)
+        per_layer.gen.lin = False
+        u8_pl = per_layer.run(clips.cuda())
         diff = (u8.float() - u8_pl.float()).abs()
         assert diff.max().item() <= 3 and diff.mean().item() < 0.05, (diff.max().item(), diff.mean().item())
-    config.set_lin_trunk(prev_lin)
 
 
 def test_configs1_128x128_lookahead_graph_32_frames_matches_oracle():

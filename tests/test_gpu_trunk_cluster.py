@@ -30,18 +30,9 @@ def test_dispatch_takes_exactly_the_trunk_shaped_plans_on_32x32():
     assert not ok([(0, 1, -1, TANH24)])
     assert ok(TRUNK + [(1, 2, -1, RELU), (2, 1, -1, RELU)] * 3 + [(1, 2, -1, RELU)])   # 40 layers
     assert not ok(TRUNK + [(1, 2, -1, RELU), (2, 1, -1, RELU)] * 4)          # 41
-
-
-def test_lin_trunk_switch_is_tristate():
-    from tecogan_b200 import config
-    prev = config.lin_trunk()
-    try:
-        for v in (None, True, False, None):
-            config.set_lin_trunk(v)
-            assert config.lin_trunk() is v
-    finally:
-        config.set_lin_trunk(prev)
-    assert 0.0 < config.LIN_TRUNK_MIN_FILL <= 1.0
+    assert not ok(TRUNK, n=0)
+    from tecogan_b200.tc_nets import LIN_TRUNK_MIN_FILL
+    assert 0.0 < LIN_TRUNK_MIN_FILL <= 1.0
 
 
 def _trunk_operands(B, seed):
@@ -126,9 +117,9 @@ def test_trunk_matches_float64_reference_bit_for_bit():
 
 @pytest.mark.gpu
 def test_clip_engine_takes_the_one_launch_trunk_from_the_batch_and_matches_per_layer_frames():
-    """Unforced, a batch of G clips (one full round of clusters) runs the one-launch trunk and G + 1 (a second round
-    almost empty) and 8 the per-layer launches; the frames of the former are byte-identical to an engine forced onto the
-    per-layer launches."""
+    """A batch of G clips (one full round of clusters) runs the one-launch trunk and G + 1 (a second round almost empty)
+    and 8 the per-layer launches; the frames of the former are byte-identical to an engine of the same batch put onto
+    the per-layer launches."""
     from tecogan_b200 import config
     from tecogan_b200.engine import ClipEngine
     from tests.test_gpu_models import _fresh_store, _smooth_clips
@@ -138,18 +129,12 @@ def test_clip_engine_takes_the_one_launch_trunk_from_the_batch_and_matches_per_l
     clips = _smooth_clips(T, B, 32, 32, seed=5)
     _fresh_store({**pg, **pf})
     config.set_precision("bf16")
-    prev = config.lin_trunk()
-    try:
-        config.set_lin_trunk(None)
-        assert not ClipEngine(32, 32, T, N, batch=8).gen.lin
-        assert not ClipEngine(32, 32, T, N, batch=B + 1).gen.lin
-        eng = ClipEngine(32, 32, T, N, batch=B)
-        assert eng.gen.lin
-        u8 = eng.run(clips.cuda()).clone()
-        config.set_lin_trunk(False)
-        per_layer = ClipEngine(32, 32, T, N, batch=B)
-        assert not per_layer.gen.lin
-        u8_pl = per_layer.run(clips.cuda())
-    finally:
-        config.set_lin_trunk(prev)
+    assert not ClipEngine(32, 32, T, N, batch=8).gen.lin
+    assert not ClipEngine(32, 32, T, N, batch=B + 1).gen.lin
+    eng = ClipEngine(32, 32, T, N, batch=B)
+    assert eng.gen.lin
+    u8 = eng.run(clips.cuda()).clone()
+    per_layer = ClipEngine(32, 32, T, N, batch=B)
+    per_layer.gen.lin = False                    # before the first replay captures the graph
+    u8_pl = per_layer.run(clips.cuda())
     assert torch.equal(u8, u8_pl), int((u8 != u8_pl).sum())
