@@ -339,6 +339,18 @@ int teco_farneback_flow_up_f32(const float* flow_in, int32_t P, int32_t sh, int3
 int teco_tof_reduce_f32(const float* flow_a, const float* flow_b, int32_t P, int32_t H, int32_t W, int32_t y0, int32_t x0,
                         int32_t h, int32_t w, double* partial, double* out, void* stream);
 
+/* ---------------------------------------------------------------------------------------
+ * PNG encoding of one RGB uint8 frame, byte-identical to cv2.imwrite(path.png, bgr) (libpng: filter Sub, zlib level 1,
+ * Z_RLE, 8 192-byte IDAT chunks), the file save_img writes (reference lib/ops.py:521-523).  DESIGN.md section 4.5.
+ * ------------------------------------------------------------------------------------- */
+/* Host-only size query for an H x W frame: the workspace (device, 256-byte aligned) and the output capacity in bytes.
+ * H, W >= 1 and H * (3W + 1) <= 2^30, else TECO_E_INVALID. */
+int teco_png_plan_bytes(int32_t H, int32_t W, int64_t* workspace_bytes_host, int64_t* out_capacity_host);
+/* rgb [H,W,3] uint8 -> out: the complete PNG file; *out_len (device int64) receives its length.  Buffers smaller than
+ * teco_png_plan_bytes gives -> TECO_E_INVALID.  Nothing allocates; every stage runs on `stream`. */
+int teco_png_encode_rgb8(const uint8_t* rgb, int32_t H, int32_t W, void* workspace, int64_t workspace_bytes, uint8_t* out,
+                         int64_t out_capacity, int64_t* out_len, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
