@@ -86,6 +86,10 @@ typedef struct teco_tc_desc {
   int32_t mode;                  /* 0: conv3x3 s1 SAME; 1: conv_transpose 3x3 s2 SAME (4 phases) */
   int32_t out_f32_c;             /* >0: also/only write fp32 output with this many channels  */
   float post_scale, post_shift;
+  int32_t k_live;                /* 1, 2, 4 (Cin 64): input channels from 16*k_live on are zero, their K-steps may be
+                                    skipped (same outputs); 0: all                              */
+  int32_t pool;                  /* 1: y is [N,H/2,W/2,Cout], the 2x2 max of the bf16 outputs (teco_maxpool2_bf16's
+                                    result; mode 0, Cin 64, Cout % 64 == 0, no residual / fp32 output) */
 } teco_tc_desc;
 
 /* transpose_layout bit 0: w is [3,3,cout,cin] (conv_transpose layout); bit 1: taps flipped (ky,kx) -> (2-ky,2-kx).

@@ -26,7 +26,7 @@ class ConvDesc(C.Structure):
 class TcDesc(C.Structure):
     """struct teco_tc_desc (include/teco.h)."""
     _fields_ = [(n, C.c_int32) for n in ("N", "H", "W", "Cin", "Cout", "act", "mode", "out_f32_c")] + [
-        ("post_scale", C.c_float), ("post_shift", C.c_float)]
+        ("post_scale", C.c_float), ("post_shift", C.c_float), ("k_live", C.c_int32), ("pool", C.c_int32)]
 
 
 _P, _I32, _I64, _F = C.c_void_p, C.c_int32, C.c_int64, C.c_float

@@ -76,7 +76,9 @@ __device__ __forceinline__ void tap_route(int t, int& ry, int& rx, int& ph) {
 // weights [tap][NT][64] at w_a.  Issues and commits them; mma_block() also waits for them.  ZERO_INIT: the first MMA
 // into each accumulator ignores its old contents (scale-d = 0) instead of the caller zeroing the registers.  Zeroing four
 // accumulators in registers made ptxas interleave the zeroing moves with the MMAs and serialise every wgmma.
-template <int MODE, int NT, int NACC, bool ZERO_INIT = false>
+// KL < 4 issues only K-steps 0 .. KL - 1 of each tap, in the same order: for an input whose channels from 16 KL on are
+// zero, the steps left out would add only zero products.
+template <int MODE, int NT, int NACC, bool ZERO_INIT = false, int KL = CB / 16>
 __device__ __forceinline__ void mma_issue(float (&acc)[NACC][NT / 2], uint32_t halo_a, uint32_t w_a, int wg) {
   wgmma_fence();
 #pragma unroll
@@ -93,7 +95,7 @@ __device__ __forceinline__ void mma_issue(float (&acc)[NACC][NT / 2], uint32_t h
     const uint32_t a0 = halo_a + (uint32_t)(((8 * wg + ry) * HALO_COLS + rx) * 128);
     const uint32_t b0 = w_a + (uint32_t)t * (uint32_t)NT * 128u;
 #pragma unroll
-    for (int k = 0; k < CB / 16; ++k)
+    for (int k = 0; k < KL; ++k)
       Wgmma<NT, 0, 0>::run(acc[ph], gmma_desc_sw128(a0 + 32u * k, 16u, HALO_COLS * 128u), gmma_desc_sw128(b0 + 32u * k, 16u, 1024u),
                            ZERO_INIT && first && k == 0 ? 0u : 1u);
   }
@@ -285,7 +287,8 @@ struct WsCfg {
 
 // MODE 0, one warpgroup per tile: the nine taps x four K-steps of mma_issue<0, …> with the operands swapped, A = weight
 // tap t ([64 cout][64 cin], SBO = 8 rows of 128 B), B = the halo from (ky, kx) (8-pixel groups one halo row apart).  The
-// first MMA runs with scale-d = 0.  Issues and commits them.
+// first MMA runs with scale-d = 0.  Issues and commits them.  KL: K-steps per tap, as in mma_issue.
+template <int KL>
 __device__ __forceinline__ void mma_issue_tile(float (&acc)[64], uint32_t halo_a, uint32_t w_a) {
   wgmma_fence();
 #pragma unroll
@@ -293,7 +296,7 @@ __device__ __forceinline__ void mma_issue_tile(float (&acc)[64], uint32_t halo_a
     const uint32_t a0 = w_a + (uint32_t)t * 64u * 128u;
     const uint32_t b0 = halo_a + (uint32_t)(((t / 3) * HALO_COLS + t % 3) * 128);
 #pragma unroll
-    for (int k = 0; k < CB / 16; ++k)
+    for (int k = 0; k < KL; ++k)
       Wgmma<128, 0, 0>::run(acc, gmma_desc_sw128(a0 + 32u * k, 16u, 1024u), gmma_desc_sw128(b0 + 32u * k, 16u, HALO_COLS * 128u),
                             t == 0 && k == 0 ? 0u : 1u);
   }
@@ -359,10 +362,41 @@ __device__ __forceinline__ void ws_epilogue(const float (&acc)[NACC][NR], const 
   }
 }
 
-template <int MODE>
-__global__ void __launch_bounds__(WS_THREADS, 1)
-conv3x3_ws_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ CUtensorMap ymap,
-                  const __grid_constant__ CUtensorMap rmap, const TcParams p) {
+// MODE 0 followed by a 2x2 max-pool, into an 8 x 4 pixel box of the half-resolution output.  The thread's values of tile
+// rows 2 jj, 2 jj + 1 and columns 2 (lane % 4) + {0, 1} are one pooling window for each of its channels 16 wq + lane / 4
+// + 8 i.  Each value is rounded to bf16 as ws_epilogue stores it, and the window's max is taken as maxpool2_bf16_kernel
+// takes it: max(max(TL, TR), max(BL, BR)) by __hmax2, channel i in half i of the pair.  Pooled pixel P = 4 jj + lane % 4
+// is the 128-byte row P of the staging tile, channel chunk q stored at chunk q ^ (P & 7).
+template <int ACT>
+__device__ __forceinline__ void ws_epilogue_pool(const float (&acc)[64], const float (&b)[2], uint32_t out_a, int wq, int lane) {
+#pragma unroll
+  for (int jj = 0; jj < TILE_ROWS / 2; ++jj) {
+    __nv_bfloat162 v[4];                                             // TL, TR, BL, BR
+#pragma unroll
+    for (int r = 0; r < 2; ++r)
+#pragma unroll
+      for (int c = 0; c < 2; ++c) {
+        const int j = 2 * jj + r;
+        v[2 * r + c] = __floats2bfloat162_rn(teco_act(acc[4 * j + c] + b[0], ACT), teco_act(acc[4 * j + 2 + c] + b[1], ACT));
+      }
+    const __nv_bfloat162 m = __hmax2(__hmax2(v[0], v[1]), __hmax2(v[2], v[3]));
+    const int P = 4 * jj + (lane & 3);
+    const uint32_t row = out_a + (uint32_t)(P * 128 + 2 * (lane >> 2));
+    const uint32_t m32 = *reinterpret_cast<const uint32_t*>(&m);
+    asm volatile("st.shared.b16 [%0], %1;" ::"r"(row + (uint32_t)(((2 * wq) ^ (P & 7)) << 4)), "h"((uint16_t)(m32 & 0xffffu))
+                 : "memory");
+    asm volatile("st.shared.b16 [%0], %1;" ::"r"(row + (uint32_t)(((2 * wq + 1) ^ (P & 7)) << 4)), "h"((uint16_t)(m32 >> 16))
+                 : "memory");
+  }
+}
+
+// The body of conv3x3_ws_kernel<MODE> (KL = 4, no pool) and of FNet's conv3x3_ws_live_kernel<KL, POOL> (MODE 0): KL
+// K-steps per tap (mma_issue_tile), POOL the 2x2 max-pooled epilogue (ws_epilogue_pool).  Separate instances keep the
+// generator's layers free of the variants' branches and registers.
+template <int MODE, int KL, bool POOL>
+__device__ __forceinline__ void ws_layer(const CUtensorMap& tmap, const CUtensorMap& ymap, const CUtensorMap& rmap,
+                                         const TcParams& p) {
+  static_assert(MODE == 0 || (KL == CB / 16 && !POOL), "conv3x3_ws_kernel<1> runs the full K without a pool");
   using Cfg = WsCfg<MODE>;
   constexpr int WS_STAGES = Cfg::STAGES, WS_OUT_BUFS = Cfg::OUT_BUFS, NACC = Cfg::NACC, S = Cfg::S;
   constexpr uint32_t WS_OUT_BYTES = Cfg::OUT_BYTES;
@@ -453,7 +487,7 @@ conv3x3_ws_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constan
     mbar_wait(smem_u32(&full[st]), (uint32_t)((k / WS_STAGES) & 1));
     if (turn > 0) named_bar_sync(my_turn, 2 * 128);
     const uint32_t halo_a = smem_u32(ring + (size_t)st * HALO_STAGE);
-    if constexpr (MODE == 0) mma_issue_tile(acc[0], halo_a, smem_u32(w_s));
+    if constexpr (MODE == 0) mma_issue_tile<KL>(acc[0], halo_a, smem_u32(w_s));
     else mma_issue<MODE, 64, NACC, true>(acc, halo_a, smem_u32(w_s), wg);
     if (turn + 1 < turns) named_bar_arrive(other_turn, 2 * 128);
     if (has_res && leader && k + k_step < my_tiles) {
@@ -474,21 +508,48 @@ conv3x3_ws_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constan
       named_bar_sync(3 + wg, 128);
     }
     const uint32_t out_a = smem_u32(out_s);
-    switch (p.act) {                          // once per tile: the element loop is compiled per activation
-      case TECO_ACT_RELU: ws_epilogue<TECO_ACT_RELU, MODE>(acc, s_bias, bias_r, out_a, has_res, wq, lane); break;
-      case TECO_ACT_LRELU02: ws_epilogue<TECO_ACT_LRELU02, MODE>(acc, s_bias, bias_r, out_a, has_res, wq, lane); break;
-      case TECO_ACT_TANH24: ws_epilogue<TECO_ACT_TANH24, MODE>(acc, s_bias, bias_r, out_a, has_res, wq, lane); break;
-      case TECO_ACT_SIGMOID: ws_epilogue<TECO_ACT_SIGMOID, MODE>(acc, s_bias, bias_r, out_a, has_res, wq, lane); break;
-      default: ws_epilogue<TECO_ACT_NONE, MODE>(acc, s_bias, bias_r, out_a, has_res, wq, lane); break;
+    if constexpr (POOL) {                     // the dispatch sends no residual with it
+      switch (p.act) {
+        case TECO_ACT_RELU: ws_epilogue_pool<TECO_ACT_RELU>(acc[0], bias_r, out_a, wq, lane); break;
+        case TECO_ACT_LRELU02: ws_epilogue_pool<TECO_ACT_LRELU02>(acc[0], bias_r, out_a, wq, lane); break;
+        case TECO_ACT_TANH24: ws_epilogue_pool<TECO_ACT_TANH24>(acc[0], bias_r, out_a, wq, lane); break;
+        case TECO_ACT_SIGMOID: ws_epilogue_pool<TECO_ACT_SIGMOID>(acc[0], bias_r, out_a, wq, lane); break;
+        default: ws_epilogue_pool<TECO_ACT_NONE>(acc[0], bias_r, out_a, wq, lane); break;
+      }
+    } else {
+      switch (p.act) {                        // once per tile: the element loop is compiled per activation
+        case TECO_ACT_RELU: ws_epilogue<TECO_ACT_RELU, MODE>(acc, s_bias, bias_r, out_a, has_res, wq, lane); break;
+        case TECO_ACT_LRELU02: ws_epilogue<TECO_ACT_LRELU02, MODE>(acc, s_bias, bias_r, out_a, has_res, wq, lane); break;
+        case TECO_ACT_TANH24: ws_epilogue<TECO_ACT_TANH24, MODE>(acc, s_bias, bias_r, out_a, has_res, wq, lane); break;
+        case TECO_ACT_SIGMOID: ws_epilogue<TECO_ACT_SIGMOID, MODE>(acc, s_bias, bias_r, out_a, has_res, wq, lane); break;
+        default: ws_epilogue<TECO_ACT_NONE, MODE>(acc, s_bias, bias_r, out_a, has_res, wq, lane); break;
+      }
     }
     fence_async_smem();                       // the staging writes -> visible to the TMA store
     named_bar_sync(3 + wg, 128);
     if (leader) {
-      tma_store_4d(&ymap, out_a, n0, S * x0, S * oy0, n);
+      // pooled: the 8 x 4 box at half the tile's coordinates on the [N, H / 2, W / 2] output (even x0, y0), clipped
+      // where the odd last row or column of the input pools to nothing
+      if constexpr (POOL) tma_store_4d(&ymap, out_a, n0, x0 / 2, y0 / 2, n);
+      else tma_store_4d(&ymap, out_a, n0, S * x0, S * oy0, n);
       bulk_commit();
     }
   }
   if (leader) bulk_wait_all();
+}
+
+template <int MODE>
+__global__ void __launch_bounds__(WS_THREADS, 1)
+conv3x3_ws_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ CUtensorMap ymap,
+                  const __grid_constant__ CUtensorMap rmap, const TcParams p) {
+  ws_layer<MODE, CB / 16, false>(tmap, ymap, rmap, p);
+}
+
+template <int KL, bool POOL>
+__global__ void __launch_bounds__(WS_THREADS, 1)
+conv3x3_ws_live_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ CUtensorMap ymap,
+                       const __grid_constant__ CUtensorMap rmap, const TcParams p) {
+  ws_layer<0, KL, POOL>(tmap, ymap, rmap, p);
 }
 
 // ------------------------------------------------------------------ im2col-tiled layer (images smaller than a tile)
@@ -684,6 +745,8 @@ __device__ __forceinline__ void f32_epilogue(const float (&acc)[2][1][8], const 
     }
 }
 
+// KL: K-steps per tap (mma_issue); 4 for the generator's output stage, 2 for FNet's flow head (32 live channels)
+template <int KL>
 __global__ void __launch_bounds__(WS_THREADS, F32_CTAS_PER_SM)
 conv3x3_f32out_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ CUtensorMap omap,
                       const __grid_constant__ CUtensorMap rmap, const F32Params p) {
@@ -768,8 +831,8 @@ conv3x3_f32out_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_con
     mbar_wait(smem_u32(&full[st]), (uint32_t)((k / F32_STAGES) & 1));
     if (k > 0) named_bar_sync(my_turn, 2 * 128);
     const uint32_t halo_a = smem_u32(ring + (size_t)st * HALO_STAGE);
-    mma_issue<0, 16, 1, true>(acc[0], halo_a, w_a, 0);
-    mma_issue<0, 16, 1, true>(acc[1], halo_a, w_a, 1);
+    mma_issue<0, 16, 1, true, KL>(acc[0], halo_a, w_a, 0);
+    mma_issue<0, 16, 1, true, KL>(acc[1], halo_a, w_a, 1);
     if (k + 1 < my_tiles) named_bar_arrive(other_turn, 2 * 128);
     if (p.has_res && leader && k + 2 < my_tiles) {
       bulk_wait_read<F32_BUFS - 2>();         // the store of this warpgroup's previous tile has read box sb_next
@@ -1190,6 +1253,16 @@ KernelT pick_kernel(int mode, int nt) {
   return conv3x3_wgmma_kernel<0, 16>;
 }
 
+using WsKernelT = void (*)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const TcParams);
+
+// Mode 0 on the warp-specialised kernel: the full K without a pool on conv3x3_ws_kernel<0>, every other (k_live, pool) on
+// its conv3x3_ws_live_kernel instance
+WsKernelT pick_ws_kernel(int k_live, int pool) {
+  if (k_live == 1) return pool ? conv3x3_ws_live_kernel<1, true> : conv3x3_ws_live_kernel<1, false>;
+  if (k_live == 2) return pool ? conv3x3_ws_live_kernel<2, true> : conv3x3_ws_live_kernel<2, false>;
+  return pool ? conv3x3_ws_live_kernel<CB / 16, true> : conv3x3_ws_kernel<0>;
+}
+
 // CTAs of `kern` resident per SM at `smem` bytes of dynamic shared memory; the opt-in shared-memory attribute is set on
 // first use and the answer cached per (kernel, size), so a launch costs no extra driver calls.
 int resident_ctas(const void* kern, size_t smem, int* per_sm, int threads = NUM_THREADS) {
@@ -1238,29 +1311,30 @@ int launch_conv3x3(const teco_tc_desc* d, const void* x, const void* wpk, const 
   if (rc != TECO_OK) return rc;
   int per_sm = 0;
   // one K block, 64-channel bf16 output slices, and no residual in mode 1: the warp-specialised kernel
-  if (p.nblk == 1 && d->Cout % 64 == 0 && !out_f32 && (d->mode == 0 || !res)) {
+  const bool ws = p.nblk == 1 && d->Cout % 64 == 0 && !out_f32 && (d->mode == 0 || !res);
+  TECO_CHECK_ARG(!d->pool || (ws && d->mode == 0 && !res && d->H >= 2 && d->W >= 2),
+                 "teco_conv3x3_tc: pool needs mode 0, Cin 64, Cout a multiple of 64, H, W >= 2 and no residual or fp32 output");
+  if (ws) {
     // output and residual: one warpgroup's box of 16 rows x 8 pixels (a whole tile; 16 x 16 of the 2H x 2W output in
-    // mode 1) x 64 channels
+    // mode 1) x 64 channels; pooled, 8 rows x 4 pixels of the H / 2 x W / 2 output
     const int s = d->mode == 1 ? 2 : 1;
     CUtensorMap ymap, rmap;
-    int rc_map = encode_halo_map(&ymap, y, d->N, s * d->H, s * d->W, d->Cout, "teco_conv3x3_tc", s * TILE_COLS, TILE_ROWS);
+    int rc_map = d->pool ? encode_halo_map(&ymap, y, d->N, d->H / 2, d->W / 2, d->Cout, "teco_conv3x3_tc", TILE_COLS / 2, TILE_ROWS / 2)
+                         : encode_halo_map(&ymap, y, d->N, s * d->H, s * d->W, d->Cout, "teco_conv3x3_tc", s * TILE_COLS, TILE_ROWS);
     if (rc_map != TECO_OK) return rc_map;
     rmap = ymap;
     if (res && res != y) {
       rc_map = encode_halo_map(&rmap, res, d->N, d->H, d->W, d->Cout, "teco_conv3x3_tc", TILE_COLS, TILE_ROWS);
       if (rc_map != TECO_OK) return rc_map;
     }
-    const void* kern = d->mode == 1 ? (const void*)conv3x3_ws_kernel<1> : (const void*)conv3x3_ws_kernel<0>;
+    const WsKernelT kern = d->mode == 1 ? conv3x3_ws_kernel<1> : pick_ws_kernel(d->k_live, d->pool);
     const size_t ws_smem = d->mode == 1 ? WsCfg<1>::SMEM : WsCfg<0>::SMEM;
-    const int rc_occ = resident_ctas(kern, ws_smem, &per_sm, WS_THREADS);
+    const int rc_occ = resident_ctas((const void*)kern, ws_smem, &per_sm, WS_THREADS);
     if (rc_occ != TECO_OK) return rc_occ;
     const int nsplit_ws = d->Cout / 64;
     const long long slots = ((long long)per_sm * teco_sm_count() + nsplit_ws - 1) / nsplit_ws;
     const unsigned gx = (unsigned)(tiles < slots ? tiles : slots);
-    if (d->mode == 1)
-      conv3x3_ws_kernel<1><<<dim3(gx, (unsigned)nsplit_ws), WS_THREADS, ws_smem, stream>>>(tmap, ymap, rmap, p);
-    else
-      conv3x3_ws_kernel<0><<<dim3(gx, (unsigned)nsplit_ws), WS_THREADS, ws_smem, stream>>>(tmap, ymap, rmap, p);
+    kern<<<dim3(gx, (unsigned)nsplit_ws), WS_THREADS, ws_smem, stream>>>(tmap, ymap, rmap, p);
     TECO_CUDA_LAUNCH_CHECK("teco_conv3x3_tc");
     return TECO_OK;
   }
@@ -1343,11 +1417,12 @@ int launch_conv3x3_f32out(const teco_tc_desc* d, const void* x, const void* wpk,
     if (rc != TECO_OK) return rc;
   }
   int per_sm = 0;
-  rc = resident_ctas((const void*)conv3x3_f32out_kernel, F32_SMEM, &per_sm, WS_THREADS);
+  const auto kern = d->k_live == 1 ? conv3x3_f32out_kernel<1> : d->k_live == 2 ? conv3x3_f32out_kernel<2> : conv3x3_f32out_kernel<4>;
+  rc = resident_ctas((const void*)kern, F32_SMEM, &per_sm, WS_THREADS);
   if (rc != TECO_OK) return rc;
   const long long slots = (long long)per_sm * teco_sm_count();   // persistent: as many CTAs as are resident at once
   const unsigned gx = (unsigned)(tiles < slots ? tiles : slots);
-  conv3x3_f32out_kernel<<<gx, WS_THREADS, F32_SMEM, stream>>>(tmap, omap, rmap, p);
+  kern<<<gx, WS_THREADS, F32_SMEM, stream>>>(tmap, omap, rmap, p);
   TECO_CUDA_LAUNCH_CHECK("teco_conv3x3_f32out_tc");
   return TECO_OK;
 }
@@ -1411,6 +1486,11 @@ int launch_trunk(int N, int L, const void* x_in, void* buf_a, void* buf_b, const
   return TECO_OK;
 }
 
+// k_live 0 is every K-step; 1, 2 or 4 steps of 16 channels per tap only make sense with one 64-channel K block
+bool k_live_ok(const teco_tc_desc* d) {
+  return d->k_live == 0 || (d->Cin == CB && (d->k_live == 1 || d->k_live == 2 || d->k_live == 4));
+}
+
 }  // namespace
 
 extern "C" int64_t teco_packed_weight_bytes(int32_t cin_pad, int32_t cout_pad) {
@@ -1444,6 +1524,8 @@ extern "C" int teco_conv3x3_tc(const teco_tc_desc* d, const void* x, const void*
   TECO_CHECK_ARG((((uintptr_t)x) & 15) == 0 && (((uintptr_t)wpk) & 15) == 0 && (((uintptr_t)y) & 15) == 0 &&
                      (((uintptr_t)res) & 15) == 0,
                  "teco_conv3x3_tc: tensors must be 16-byte aligned");
+  TECO_CHECK_ARG(k_live_ok(d), "teco_conv3x3_tc: k_live must be 0, or 1, 2 or 4 with Cin 64 (got %d, Cin %d)", d->k_live, d->Cin);
+  TECO_CHECK_ARG(d->pool == 0 || d->pool == 1, "teco_conv3x3_tc: pool must be 0 or 1 (got %d)", d->pool);
   return launch_conv3x3(d, x, wpk, bias, res, y, res_f32, out_f32, (cudaStream_t)stream);
 }
 
@@ -1455,7 +1537,8 @@ extern "C" int teco_conv3x3_im2col_tc(const teco_tc_desc* d, const void* x, cons
                  "teco_conv3x3_im2col_tc: Cin must be a multiple of 64 in [64,512] (got %d)", d->Cin);
   TECO_CHECK_ARG(d->Cout >= 64 && d->Cout % 64 == 0 && d->Cout <= 512,
                  "teco_conv3x3_im2col_tc: Cout must be a multiple of 64 in [64,512] (got %d)", d->Cout);
-  TECO_CHECK_ARG(d->mode == 0 && d->out_f32_c == 0, "teco_conv3x3_im2col_tc: mode 0 with a bf16 output only");
+  TECO_CHECK_ARG(d->mode == 0 && d->out_f32_c == 0 && d->k_live == 0 && d->pool == 0,
+                 "teco_conv3x3_im2col_tc: mode 0 with a bf16 output only (k_live and pool 0)");
   TECO_CHECK_ARG(d->act >= 0 && d->act <= TECO_ACT_SIGMOID, "teco_conv3x3_im2col_tc: unknown activation %d", d->act);
   TECO_CHECK_ARG((((uintptr_t)x) & 15) == 0 && (((uintptr_t)wpk) & 15) == 0 && (((uintptr_t)y) & 15) == 0,
                  "teco_conv3x3_im2col_tc: tensors must be 16-byte aligned");
@@ -1473,6 +1556,8 @@ extern "C" int teco_conv3x3_f32out_tc(const teco_tc_desc* d, const void* x, cons
   TECO_CHECK_ARG(d->act >= 0 && d->act <= TECO_ACT_SIGMOID, "teco_conv3x3_f32out_tc: unknown activation %d", d->act);
   TECO_CHECK_ARG(d->out_f32_c == 2 || d->out_f32_c == 3, "teco_conv3x3_f32out_tc: out_f32_c must be 2 or 3 (got %d)",
                  d->out_f32_c);
+  TECO_CHECK_ARG(k_live_ok(d) && d->pool == 0, "teco_conv3x3_f32out_tc: k_live must be 0, 1, 2 or 4 and pool 0 (got %d, %d)",
+                 d->k_live, d->pool);
   TECO_CHECK_ARG(((long long)d->W * d->out_f32_c * 4) % 16 == 0,
                  "teco_conv3x3_f32out_tc: an fp32 row (W*out_f32_c*4 = %lld bytes) must be a multiple of 16 bytes",
                  (long long)d->W * d->out_f32_c * 4);

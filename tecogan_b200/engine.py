@@ -13,8 +13,6 @@ Look-ahead (bf16 mode, step(lr, next_lr=...) / run_sequence): the flow of frame 
 runs concurrently with generator_F of frame i; frame i+1 then starts directly with warp + generator.  Same kernels on
 the same inputs in the same order per buffer, hence bit-identical outputs to the serial recurrence (tested).
 """
-import os
-
 import torch
 
 from . import config
@@ -264,14 +262,10 @@ class ClipEngine:
     contiguous block) -> self.clip_u8 [T,B,4h,4w,3] uint8 (save_img quantisation, lib/ops.py:521-523); the fp32 output of
     the last frame stays in self.out01."""
 
-    def __init__(self, h, w, T, num_resblock=16, batch=1, use_graph=True, device="cuda", fnet_pairs=None):
-        """fnet_pairs: consecutive frame pairs (of all B clips) per fnet pass -- a divisor of T-1.  All pairs of a clip are
-        independent (lib/Teco.py:102-117 batches them all); more pairs per pass = fewer, larger launches (metric config,
-        296 clips: 14.46 ms per step with 1 pair per pass, 14.04 with 3, 13.87 with all 9; config 5, b=1: +19 %).  Opt-in
-        (default TECO_FNET_PAIRS or 1): the larger fnet batch makes the conv launcher pick other tile / K-split variants, so the
-        flow -- and with it the output -- differs from the streaming engine's in the last bf16 bit (1 LSB of a few uint8
-        pixels at B = 6 / 12; at 256x256 the Y-PSNR delta against the oracle moved from < 0.05 to 0.08 dB), and only the
-        one-pair configuration is held to the parity thresholds by the tests."""
+    def __init__(self, h, w, T, num_resblock=16, batch=1, use_graph=True, device="cuda"):
+        """FNet runs once per clip batch, over all B * (T - 1) consecutive frame pairs (they are independent, and
+        lib/Teco.py:102-117 batches them all too): fewer, fuller launches.  Every FNet convolution computes each output in a
+        fixed order whatever the batch size, so the flows are byte-identical to one-pair passes over the same frames."""
         if h < 8 or w < 8:
             raise ValueError("ClipEngine: LR frames must be at least 8x8")
         if T < 1:
@@ -289,24 +283,21 @@ class ClipEngine:
             self.gen = GeneratorPlan(gs, batch, h, w, num_resblock, self.device)
         with variable_scope('fnet'), variable_scope('autoencode_unit') as fs:
             _ensure_vars_fnet()
-            if fnet_pairs is None:
-                fnet_pairs = int(os.environ.get("TECO_FNET_PAIRS", "1"))
-            if T > 1 and (fnet_pairs < 1 or (T - 1) % fnet_pairs):
-                raise ValueError("ClipEngine: fnet_pairs=%d does not divide the %d frame pairs of a clip" % (fnet_pairs, T - 1))
-            self.pairs = fnet_pairs if T > 1 else 1
-            self.fnet = FNetPlan(fs, batch * self.pairs, h, w, self.device)
-        self.flows = torch.zeros((max(T - 1, 1), batch) + tuple(self.fnet.flow.shape[1:]), device=self.device, dtype=f32)
+            # pair (t - 1, t) of clip b is FNet image (t - 1) * B + b: time-major, so frames 0 .. T-2 and 1 .. T-1 of all
+            # clips are two contiguous blocks of clip_in, and the flows land in self.flows[t - 1][b]
+            self.fnet = FNetPlan(fs, batch * max(T - 1, 1), h, w, self.device)
+        self.flows = self.fnet.flow.view((max(T - 1, 1), batch) + tuple(self.fnet.flow.shape[1:]))
         self.graph = None
-        # our kernel launches per clip batch: fnet passes, then per frame warp/pack/generator/deprocess
-        self.launches = ((T - 1) // self.pairs) * (self.fnet.launches + 2) + T * (self.gen.launches + 2) + (T - 1)
+        # our kernel launches per clip batch: one fnet pass, then per frame warp/pack/generator/deprocess
+        self.launches = (self.fnet.launches + 2 if T > 1 else 0) + T * (self.gen.launches + 2) + (T - 1)
 
     def _body(self):
         g, f, T = self.gen, self.fnet, self.T
-        P, hw3 = self.pairs, (self.h, self.w, 3)
-        for t in range(1, T, P):                # pairs (t-1, t) .. (t+P-2, t+P-1): time-major, so P frames are one block
-            _f32_slice_to_bf16(self.clip_in[t - 1:t - 1 + P].view(-1, *hw3), 0, 3, f.x_in, 0)
-            _f32_slice_to_bf16(self.clip_in[t:t + P].view(-1, *hw3), 0, 3, f.x_in, 3)
-            f.run(flow_out=self.flows[t - 1:t - 1 + P].view((-1,) + tuple(self.flows.shape[2:])))
+        hw3 = (self.h, self.w, 3)
+        if T > 1:
+            _f32_slice_to_bf16(self.clip_in[:T - 1].view(-1, *hw3), 0, 3, f.x_in, 0)
+            _f32_slice_to_bf16(self.clip_in[1:].view(-1, *hw3), 0, 3, f.x_in, 3)
+            f.run()
         n = self.out01.numel()
         for t in range(T):
             if t == 0:

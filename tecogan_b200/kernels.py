@@ -507,15 +507,18 @@ def pad_bias(b, cout_pad):
     return out
 
 
-def conv3x3_tc(x, wpk, bias, y=None, *, cout, act=ACT_NONE, res=None, mode=0, out_f32=None, res_f32=None, post=(1.0, 0.0)):
+def conv3x3_tc(x, wpk, bias, y=None, *, cout, act=ACT_NONE, res=None, mode=0, out_f32=None, res_f32=None, post=(1.0, 0.0),
+               k_live=0, pool=False):
     """One launch of the wgmma kernel.  x [N,H,W,Cin] bf16; y [N,H(,x2),W(,x2),cout] bf16 (allocated if None and
-    out_f32 is None)."""
+    out_f32 is None).  k_live (Cin 64): x's channels from 16 * k_live on are zero, so their K-steps may be skipped;
+    pool: y is [N,H/2,W/2,cout], the 2x2 max-pool of the output (maxpool2_bf16's result)."""
     N, H, W, Cin = x.shape
     s = 2 if mode == 1 else 1
     if y is None and out_f32 is None:
-        y = torch.empty((N, s * H, s * W, cout), device=x.device, dtype=bf16)
+        y = torch.empty((N, H // 2, W // 2, cout) if pool else (N, s * H, s * W, cout), device=x.device, dtype=bf16)
     d = TcDesc(N=N, H=H, W=W, Cin=Cin, Cout=cout, act=act, mode=mode,
-               out_f32_c=0 if out_f32 is None else out_f32.shape[-1], post_scale=post[0], post_shift=post[1])
+               out_f32_c=0 if out_f32 is None else out_f32.shape[-1], post_scale=post[0], post_shift=post[1],
+               k_live=k_live, pool=int(pool))
     call("teco_conv3x3_tc", d, ptr(x, bf16), ptr(wpk, bf16), ptr(bias, f32), ptr(res, bf16), ptr(y, bf16), ptr(res_f32, f32),
          ptr(out_f32, f32), stream_ptr())
     return y if out_f32 is None else out_f32
@@ -538,12 +541,12 @@ def conv3x3_f32out_fits(W, C):
     return C in (2, 3) and (W * C * 4) % 16 == 0
 
 
-def conv3x3_f32out_tc(x, wpk, bias, y=None, *, cout, act=ACT_NONE, out_f32, res_f32=None, post=(1.0, 0.0)):
+def conv3x3_f32out_tc(x, wpk, bias, y=None, *, cout, act=ACT_NONE, out_f32, res_f32=None, post=(1.0, 0.0), k_live=0):
     """conv3x3_tc's fp32 output stage (Cin 64, cout 16, out_f32 [N,H,W,2 or 3]) on its pipelined kernel, bit-identical;
     called as conv3x3_tc is.  y must be None."""
     N, H, W, Cin = x.shape
     d = TcDesc(N=N, H=H, W=W, Cin=Cin, Cout=cout, act=act, mode=0, out_f32_c=out_f32.shape[-1], post_scale=post[0],
-               post_shift=post[1])
+               post_shift=post[1], k_live=k_live)
     call("teco_conv3x3_f32out_tc", d, ptr(x, bf16), ptr(wpk, bf16), ptr(bias, f32), ptr(None), ptr(y, bf16), ptr(res_f32, f32),
          ptr(out_f32, f32), stream_ptr())
     return out_f32

@@ -30,7 +30,15 @@ def pad64(c):
 
 
 class TcLayer:
-    __slots__ = ("wpk", "bias", "cin_pad", "cout_pad", "cout")
+    __slots__ = ("wpk", "bias", "cin_pad", "cout_pad", "cout", "k_live")
+
+
+def _k_live(live, cin_pad):
+    """K-steps of 16 channels per tap that cover `live` input channels of a 64-channel slab (1, 2 or 4); 0 (all) for
+    wider inputs."""
+    if cin_pad != 64:
+        return 0
+    return next(k for k in (1, 2, 4) if 16 * k >= live)
 
 
 _cache = {}
@@ -53,6 +61,7 @@ def _layer(full_name, transpose=False, cin_perm=None, cin_pad=None, f32_out=Fals
     L.cin_pad = cin_pad or pad64(cin)
     L.cout_pad = pad16(cout) if f32_out else pad64(cout)
     L.cout = cout
+    L.k_live = _k_live(cin if cin_perm is None else 1 + max(i for i, c in enumerate(cin_perm) if c >= 0), L.cin_pad)
     L.wpk = K.packed_weight(w.detach(), L.cin_pad, L.cout_pad, transpose, cin_perm)
     L.bias = K.pad_bias(b.detach(), L.cout_pad) if b is not None else None
     for k in [k for k in _cache if k[0] == store.uid and k[2] == full_name]:
@@ -174,7 +183,11 @@ class GeneratorPlan:
 
 
 class FNetPlan:
-    """Pre-allocated bf16 pipeline for fnet on [n,h,w] inputs: 14 wgmma launches + 3 max-pools + 3 resizes."""
+    """Pre-allocated bf16 pipeline for fnet on [n,h,w] inputs: 14 wgmma launches + 3 max-pools + 3 resizes, where an
+    encoder's conv_2 runs on the one-K-block warp-specialised kernel (64 input channels, a level of at least 16 x 8) its
+    max-pool is fused into the conv's epilogue, and the layers with 6 or 32 live input channels in their 64-channel slab
+    (encoder_1, encoder_2/conv_1, the flow head) run only the K-steps that carry them.  t2 of a fused level is not
+    written."""
 
     def __init__(self, scope, n, h, w, device):
         self.n, self.h, self.w = n, h, w
@@ -199,7 +212,11 @@ class FNetPlan:
         self.fh, self.fw = ch, cw
         self.o1 = z(n, ch, cw, 64)
         self.flow = torch.zeros((n, ch, cw, 2), device=device, dtype=f32)
-        self.launches = 14 + 6
+        # levels smaller than conv3x3_tc's 16 x 8 tile of one image run on 128-pixel tiles across images
+        self.small = [t2.shape[1] < 16 or t2.shape[2] < 8 for t1, t2, t3 in self.bufs]
+        self.fused_pool = [i < 3 and not small and c2.cin_pad == 64
+                           for i, ((c1, c2), small) in enumerate(zip(self.layers, self.small))]
+        self.launches = 14 + 6 - sum(self.fused_pool)
         self.head_conv = K.conv3x3_f32out_tc if K.conv3x3_f32out_fits(cw, 2) else K.conv3x3_tc
 
     def run(self, flow_out=None):
@@ -209,17 +226,21 @@ class FNetPlan:
         flow = self.flow if flow_out is None else flow_out
         for i, ((c1, c2), (t1, t2, t3)) in enumerate(zip(self.layers, self.bufs)):
             _, hh, ww, cc = t2.shape
-            # levels smaller than conv3x3_tc's 16 x 8 tile of one image: 128-pixel tiles across images
-            conv = K.conv3x3_im2col_tc if hh < 16 or ww < 8 else K.conv3x3_tc
-            conv(x, c1.wpk, c1.bias, t1, cout=c1.cout_pad, act=ACT_LRELU02)
-            conv(t1, c2.wpk, c2.bias, t2, cout=c2.cout_pad, act=ACT_LRELU02)
-            if i < 3:
-                call("teco_maxpool2_bf16", ptr(t2, bf16), ptr(t3, bf16), n, hh, ww, cc, stream_ptr())
+            if self.small[i]:
+                K.conv3x3_im2col_tc(x, c1.wpk, c1.bias, t1, cout=c1.cout_pad, act=ACT_LRELU02)
+                K.conv3x3_im2col_tc(t1, c2.wpk, c2.bias, t2, cout=c2.cout_pad, act=ACT_LRELU02)
             else:
+                K.conv3x3_tc(x, c1.wpk, c1.bias, t1, cout=c1.cout_pad, act=ACT_LRELU02, k_live=c1.k_live)
+                K.conv3x3_tc(t1, c2.wpk, c2.bias, t3 if self.fused_pool[i] else t2, cout=c2.cout_pad, act=ACT_LRELU02,
+                             k_live=c2.k_live, pool=self.fused_pool[i])
+            if i < 3 and not self.fused_pool[i]:
+                call("teco_maxpool2_bf16", ptr(t2, bf16), ptr(t3, bf16), n, hh, ww, cc, stream_ptr())
+            elif i >= 3:
                 call("teco_resize2x_bf16", ptr(t2, bf16), ptr(t3, bf16), n, hh, ww, cc, stream_ptr())
             x = t3
-        K.conv3x3_tc(x, self.l_o1.wpk, self.l_o1.bias, self.o1, cout=64, act=ACT_LRELU02)
-        self.head_conv(self.o1, self.l_o2.wpk, self.l_o2.bias, None, cout=16, act=ACT_TANH24, out_f32=flow)
+        K.conv3x3_tc(x, self.l_o1.wpk, self.l_o1.bias, self.o1, cout=64, act=ACT_LRELU02, k_live=self.l_o1.k_live)
+        self.head_conv(self.o1, self.l_o2.wpk, self.l_o2.bias, None, cout=16, act=ACT_TANH24, out_f32=flow,
+                       k_live=self.l_o2.k_live)
         return flow
 
 
