@@ -355,6 +355,19 @@ int teco_png_plan_bytes(int32_t H, int32_t W, int64_t* workspace_bytes_host, int
 int teco_png_encode_rgb8(const uint8_t* rgb, int32_t H, int32_t W, void* workspace, int64_t workspace_bytes, uint8_t* out,
                          int64_t out_capacity, int64_t* out_len, void* stream);
 
+/* ---------------------------------------------------------------------------------------
+ * JPEG encoding of one RGB uint8 frame, byte-identical to cv2.imwrite(path.jpg, bgr) with cv2's defaults (baseline,
+ * quality 95, 4:2:0, islow FDCT, the Annex K Huffman tables), the file save_img writes by default (reference
+ * lib/ops.py:521-523, main.py --output_ext jpg).  DESIGN.md section 4.6.
+ * ------------------------------------------------------------------------------------- */
+/* Host-only size query for an H x W frame: the workspace (device, 256-byte aligned) and the output capacity in bytes.
+ * 1 <= H, W <= 65500 (JPEG's limit), else TECO_E_INVALID. */
+int teco_jpeg_plan_bytes(int32_t H, int32_t W, int64_t* workspace_bytes_host, int64_t* out_capacity_host);
+/* rgb [H,W,3] uint8 -> out: the complete JPEG file; *out_len (device int64) receives its length.  Buffers smaller than
+ * teco_jpeg_plan_bytes gives -> TECO_E_INVALID.  Nothing allocates; every stage runs on `stream`. */
+int teco_jpeg_encode_rgb8(const uint8_t* rgb, int32_t H, int32_t W, void* workspace, int64_t workspace_bytes, uint8_t* out,
+                          int64_t out_capacity, int64_t* out_len, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

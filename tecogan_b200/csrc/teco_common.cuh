@@ -68,4 +68,33 @@ __device__ __forceinline__ float block_sum(float v, float* smem32) {
   return r;
 }
 
+// Exclusive scan of one int per thread over a CTA of NT threads (multiple of 32); returns the prefix, *total the sum.
+// Every thread of the CTA must call it.
+template <int NT>
+__device__ __forceinline__ int cta_exclusive_scan(int v, int* sm /* NT/32 + 1 ints */, int* total) {
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  int x = v;
+#pragma unroll
+  for (int d = 1; d < 32; d <<= 1) {
+    int y = __shfl_up_sync(0xffffffffu, x, d);
+    if (lane >= d) x += y;
+  }
+  if (lane == 31) sm[wid] = x;
+  __syncthreads();
+  if (wid == 0) {
+    int w = lane < NT / 32 ? sm[lane] : 0;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+      int y = __shfl_up_sync(0xffffffffu, w, d);
+      if (lane >= d) w += y;
+    }
+    if (lane < NT / 32) sm[lane] = w;
+  }
+  __syncthreads();
+  const int before = (wid > 0 ? sm[wid - 1] : 0) + x - v;
+  *total = sm[NT / 32 - 1];
+  __syncthreads();
+  return before;
+}
+
 int teco_sm_count();

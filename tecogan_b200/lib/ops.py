@@ -122,12 +122,19 @@ def tf_data_gaussDownby4(HRdata, sigma=1.5):
 
 def save_img(out_path, img):
     """clip(img*255) -> uint8 -> BGR imwrite (reference lib/ops.py:521-523).  img: [H,W,3] CUDA or numpy in [0,1].
-    A CUDA image saved as .png (any case, as cv2 matches extensions) is encoded on the GPU into the bytes cv2.imwrite
-    would write; a path that cannot be written is ignored, as the reference ignores imwrite's False."""
+    A CUDA image saved as .png, or as .jpg / .jpeg / .jpe (any case, as cv2 matches extensions; sides up to JPEG's
+    65 500), is encoded on the GPU into the bytes cv2.imwrite would write; a path that cannot be written is ignored, as
+    the reference ignores imwrite's False."""
     import cv2 as cv
-    if torch.is_tensor(img) and img.is_cuda and out_path.lower().endswith(".png"):
-        from ..png import encode_png
-        data = encode_png(K.to_u8(img).contiguous())
+    path = out_path.lower()
+    encode = None
+    if torch.is_tensor(img) and img.is_cuda:
+        if path.endswith(".png"):
+            from ..png import encode_png as encode
+        elif path.endswith((".jpg", ".jpeg", ".jpe")) and max(img.shape[0], img.shape[1]) <= 65500:
+            from ..jpeg import encode_jpeg as encode
+    if encode is not None:
+        data = encode(K.to_u8(img).contiguous())
         try:
             with open(out_path, "wb") as f:
                 f.write(data)
