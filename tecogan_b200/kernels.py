@@ -306,7 +306,7 @@ def space_to_depth4(x):
 class _BNTrain(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, beta, lrelu):
-        x = _cc(x)
+        x, beta = _cc(x), _cc(beta)
         C = x.shape[-1]
         npix = x.numel() // C
         y = torch.empty_like(x)
