@@ -309,6 +309,11 @@ extern "C" int teco_conv2d_wgrad_f32(const teco_conv_desc* d, const float* x, co
   TECO_CHECK_ARG(x && dy && dw, "teco_conv2d_wgrad_f32: NULL tensor");
   cudaStream_t s = (cudaStream_t)stream;
   long long M = (long long)d->N * d->OH * d->OW;
+  // Every check comes before the first write: a rejected call leaves dw and db as they were.
+  if (db) {
+    TECO_CHECK_ARG(d->Cout <= 256, "teco_conv2d_wgrad_f32: bias gradient supports Cout <= 256 (got %d)", d->Cout);
+    TECO_CHECK_ARG(M < (1LL << 31), "teco_conv2d_wgrad_f32: too many output pixels for the bias gradient");
+  }
   if (!accumulate) {
     TECO_CUDA_CALL(cudaMemsetAsync(dw, 0, sizeof(float) * (size_t)d->KH * d->KW * d->Cin * d->Cout, s));
     if (db) TECO_CUDA_CALL(cudaMemsetAsync(db, 0, sizeof(float) * (size_t)d->Cout, s));
@@ -329,8 +334,6 @@ extern "C" int teco_conv2d_wgrad_f32(const teco_conv_desc* d, const float* x, co
   conv2d_wgrad_f32_kernel<<<grid, 256, 0, s>>>(*d, x, dy, dw, ci_tiles, pps);
   TECO_CUDA_LAUNCH_CHECK("teco_conv2d_wgrad_f32");
   if (db) {
-    TECO_CHECK_ARG(d->Cout <= 256, "teco_conv2d_wgrad_f32: bias gradient supports Cout <= 256 (got %d)", d->Cout);
-    TECO_CHECK_ARG(M < (1LL << 31), "teco_conv2d_wgrad_f32: too many output pixels for the bias gradient");
     const int ppar = 256 / d->Cout;
     int ppb = 8 * ppar;                                          // eight pixels per thread
     long long blocks = (M + ppb - 1) / ppb;
