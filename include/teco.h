@@ -356,6 +356,29 @@ int teco_png_encode_rgb8(const uint8_t* rgb, int32_t H, int32_t W, void* workspa
                          int64_t out_capacity, int64_t* out_len, void* stream);
 
 /* ---------------------------------------------------------------------------------------
+ * PNG decoding of a batch of files to RGB uint8, byte-identical to cv2.imread(path, IMREAD_COLOR)[..., ::-1] on the
+ * subset the device takes (non-interlaced; grey 1/2/4/8 bits, RGB 8, palette 1/2/4/8, grey + alpha 8, RGBA 8;
+ * 1 <= H, W <= 65500).  The caller walks the chunks and checks the CRCs; the device reports per file whether its zlib
+ * stream decoded exactly.  DESIGN.md section 4.7.
+ * ------------------------------------------------------------------------------------- */
+/* Host-only size query: the workspace bytes one file of this size and format needs (its filtered rows, rounded up to
+ * 256).  Sizes or formats outside the subset -> TECO_E_INVALID. */
+int teco_png_decode_plan_bytes(int32_t H, int32_t W, int32_t colour_type, int32_t bit_depth, int64_t* workspace_bytes_host);
+/* desc: device int64 [nfiles, 11], one row per file:
+ *   0 stream offset in src, 1 stream length (the IDAT data, concatenated), 2 H, 3 W, 4 colour type, 5 bit depth,
+ *   6 palette offset in src, 7 palette entries (colour type 3; else unused), 8 destination offset in dst,
+ *   9 destination row pitch in bytes (>= 3W), 10 workspace offset (rows of the sizes teco_png_decode_plan_bytes gives,
+ *   not overlapping one another or dst).
+ * status: device int32 [nfiles], written for every file: 0 the RGB frame is at dst; otherwise nothing is promised about
+ * the file's destination rows and the caller decodes it another way.  1 zlib header, 2 block type or stored length,
+ * 3 Huffman code or code lengths, 4 symbol outside the code, 5 distance before the start or beyond the window,
+ * 6 stream ends early, 7 more bytes than H * (rowbytes + 1), 8 fewer, 9 Adler-32, 10 bytes after the Adler-32,
+ * 11 filter type above 4, 12 palette index beyond the palette, 13 descriptor outside the buffers or the subset.
+ * No file reads or writes outside its own ranges.  Nothing allocates; every stage runs on `stream`. */
+int teco_png_decode_rgb8(const uint8_t* src, int64_t src_bytes, const int64_t* desc, int32_t nfiles, void* workspace,
+                         int64_t workspace_bytes, uint8_t* dst, int64_t dst_bytes, int32_t* status, void* stream);
+
+/* ---------------------------------------------------------------------------------------
  * JPEG encoding of one RGB uint8 frame, byte-identical to cv2.imwrite(path.jpg, bgr) with cv2's defaults (baseline,
  * quality 95, 4:2:0, islow FDCT, the Annex K Huffman tables), the file save_img writes by default (reference
  * lib/ops.py:521-523, main.py --output_ext jpg).  DESIGN.md section 4.6.

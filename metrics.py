@@ -5,9 +5,9 @@ with --lpips_alexnet and --lpips_lin, LPIPS and tLP100 (tecogan_b200/lpips.py: A
 Same frame selection (cutfr = 2, metrics.py:117,131), same cut of the result to the target size (:134-135), same crop_8x8
 (:171-172), same per-frame / per-folder / total printout and metrics.csv layout (:205-242) restricted to
 keys = ["PSNR", "SSIM"], plus "LPIPS" and "tLP100" with the two LPIPS flags and "tOF" with --tof, in the reference's
-order PSNR, SSIM, LPIPS, tOF, tLP100.  Each PNG is decoded and run through AlexNet once; tLP100 reuses the previous
-frame's features.  With --tof the folder's frames are decoded up front and all its Farneback flows (tecogan_b200/tof.py)
-run as one batch; the per-frame line then carries "tOF %02.2f, " before psnr, as the reference prints it.  Without
+order PSNR, SSIM, LPIPS, tOF, tLP100.  Each folder's frames are decoded once, on the device (read_folder), and run
+through AlexNet once; tLP100 reuses the previous frame's features.  With --tof all the folder's Farneback flows
+(tecogan_b200/tof.py) run as one batch; the per-frame line then carries "tOF %02.2f, " before psnr, as the reference prints it.  Without
 --tof nothing about the output changes.  Unlike the reference, which fails there, a result smaller than its target is
 compared on the area the two share, for tOF as for the other metrics.
 
@@ -49,21 +49,24 @@ def metric_keys(lpips, tof):
     return KEYS + (["LPIPS"] if lpips else []) + (["tOF"] if tof else []) + (["tLP100"] if lpips else [])
 
 
-def folder_tof(result, target):
-    """tOF list of the frames cutfr .. n-cutfr-1 of one scene (one shorter than PSNR's): every frame decoded once, all
-    flows in one batch on the common area of result and target."""
+def read_folder(paths):
+    """[H, W, 3] uint8 RGB CUDA tensors of the PNG files at `paths`: decoded on the device in byte-bounded batches
+    (tecogan_b200/png.py::decode_png), with read_rgb for the files the device does not take."""
+    from tecogan_b200.png import decode_png
+    return decode_png(paths, host_decode=read_rgb)
+
+
+def folder_tof(tars, outs):
+    """tOF list of one scene's decoded frames cutfr .. n-cutfr-1 (one shorter than PSNR's): all flows in one batch on
+    the common area of result and target."""
     import torch
     from tecogan_b200 import tof as TOF
-    idx = range(CUTFR, len(target) - CUTFR)
-    tars, outs = [read_rgb(target[i]) for i in idx], [read_rgb(result[i]) for i in idx]
     if not tars:
         return []
     for name, frames in (("target", tars), ("result", outs)):
-        if len({f.shape for f in frames}) != 1:
+        if len({tuple(f.shape) for f in frames}) != 1:
             raise ValueError("tOF: the %s frames of one folder differ in size" % name)
-    t = torch.from_numpy(np.stack(tars)).cuda()
-    o = torch.from_numpy(np.stack(outs)).cuda()
-    return TOF.tof_sequence(t, o)
+    return TOF.tof_sequence(torch.stack(tars), torch.stack(outs))
 
 
 def evaluate_folder(result_dir, target_dir, log=print, lpips=None, tof=False):
@@ -74,17 +77,20 @@ def evaluate_folder(result_dir, target_dir, log=print, lpips=None, tof=False):
     from tecogan_b200 import metrics as M
     result, target = listPNGinDir(result_dir), listPNGinDir(target_dir)
     lists = {k: [] for k in metric_keys(lpips is not None, tof)}
-    tof_all = folder_tof(result, target) if tof else None
+    idx = list(range(CUTFR, len(target) - CUTFR))
+    frames = read_folder([target[i] for i in idx] + [result[i] for i in idx])   # every frame decoded once
+    tars, outs = frames[:len(idx)], frames[len(idx):]
+    tof_all = folder_tof(tars, outs) if tof else None
     prev = None
-    for i in range(CUTFR, len(target) - CUTFR):
-        out, tar = read_rgb(result[i]), read_rgb(target[i])
-        msg = "frame %d, tar %s, out %s, " % (i, str(tar.shape), str(out.shape))
+    for n, i in enumerate(idx):
+        t, o = tars[n], outs[n]
+        tar, out = t.shape, o.shape
+        msg = "frame %d, tar %s, out %s, " % (i, str(tuple(tar)), str(tuple(out)))
         if tof and i > CUTFR:                     # metrics.py:143-169
             lists["tOF"].append(tof_all[i - CUTFR - 1])
             msg += "tOF %02.2f, " % lists["tOF"][-1]
-        t, o = torch.from_numpy(tar).cuda(), torch.from_numpy(out).cuda()
         ps, ss = M.frame_metrics(t, o)            # window = crop_8x8 of the common area; no cropped copies
-        win = M.crop_window(min(tar.shape[0], out.shape[0]), min(tar.shape[1], out.shape[1]))
+        win = M.crop_window(min(tar[0], out[0]), min(tar[1], out[1]))
         lists["PSNR"].append(ps[0])
         lists["SSIM"].append(ss[0])
         log(result[i])

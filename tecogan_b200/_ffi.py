@@ -98,6 +98,8 @@ SIGNATURES = {
     "teco_tof_reduce_f32": [_P, _P, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _P, _P, _P],
     "teco_png_plan_bytes": [_I32, _I32, _P, _P],
     "teco_png_encode_rgb8": [_P, _I32, _I32, _P, _I64, _P, _I64, _P, _P],
+    "teco_png_decode_plan_bytes": [_I32, _I32, _I32, _I32, _P],
+    "teco_png_decode_rgb8": [_P, _I64, _P, _I32, _P, _I64, _P, _I64, _P, _P],
     "teco_jpeg_plan_bytes": [_I32, _I32, _P, _P],
     "teco_jpeg_encode_rgb8": [_P, _I32, _I32, _P, _I64, _P, _I64, _P, _P],
 }

@@ -274,8 +274,9 @@ class FrameStore:
     uint8 RGB device buffer, and the batches of those loaders cut from it on the GPU.
 
     Frame i sits at byte offsets[i] with shape sizes[i] = (H, W); sizes come from the PNG headers, so the offsets are known
-    before anything is decoded, and scenes may differ in size.  The frames are decoded on `queue_thread` host threads in
-    chunks of about `chunk_bytes` through a pinned staging buffer.  With world > 1 (an initialised torch.distributed group
+    before anything is decoded, and scenes may differ in size.  `queue_thread` host threads read the files and pack
+    their compressed streams into a pinned stage; the device decodes them in chunks of about `chunk_bytes` straight
+    into the store (tecogan_b200/png.py::decode_png_into), and a file outside its PNG subset is decoded on the host.  With world > 1 (an initialised torch.distributed group
     whose backend can broadcast `device` tensors: NCCL under torchrun) rank r decodes the r-th contiguous share of the
     frames and broadcasts it, so every rank holds the whole store after 1/world of the decoding.
 
@@ -333,29 +334,22 @@ class FrameStore:
         return total
 
     def _decode(self, paths, a, b, threads, chunk_bytes):
-        import torch
+        """Frames a..b-1 into self.buf: host threads read the files and pack their compressed streams, the device
+        decodes them in chunks of about chunk_bytes (tecogan_b200.png.decode_png_into); a file the device does not take
+        is decoded on the host by the loader and copied into its slot."""
+        from ..png import decode_png_into
         if b <= a:
             return
-        off = self.offsets
-        stage = torch.empty(int(min(off[b] - off[a], max(chunk_bytes, int((off[a + 1:b + 1] - off[a:b]).max())))),
-                            dtype=torch.uint8).pin_memory()
-        host = stage.numpy()
-        with concurrent.futures.ThreadPoolExecutor(max_workers=threads) as pool:
-            i = a
-            while i < b:
-                j = i + 1
-                while j < b and off[j + 1] - off[i] <= stage.numel():
-                    j += 1
+        expect = {paths[k]: tuple(int(v) for v in self.sizes[k]) for k in range(a, b)}
 
-                def put(k, i=i):
-                    im = self.loader.decode(paths[k])
-                    h, w = self.sizes[k]
-                    if im.shape[:2] != (h, w):
-                        raise ValueError('FrameStore: %s decodes to %dx%d, its header says %dx%d' % (paths[k], im.shape[0], im.shape[1], h, w))
-                    host[off[k] - off[i]:off[k + 1] - off[i]].reshape(h, w, 3)[...] = im
-                list(pool.map(put, range(i, j)))
-                self.buf[int(off[i]):int(off[j])].copy_(stage[:int(off[j] - off[i])])   # synchronous: the stage is reused
-                i = j
+        def host(path):
+            im = self.loader.decode(path)
+            h, w = expect[path]
+            if im.shape[:2] != (h, w):
+                raise ValueError('FrameStore: %s decodes to %dx%d, its header says %dx%d' % (path, im.shape[0], im.shape[1], h, w))
+            return im
+        decode_png_into(paths[a:b], self.buf, self.offsets[a:b], self.sizes[a:b], threads=threads,
+                        batch_bytes=chunk_bytes, host_decode=host)
 
     def view(self, loader):
         """This store serving `loader`, one of the loaders it was built from."""
