@@ -391,6 +391,25 @@ int teco_jpeg_plan_bytes(int32_t H, int32_t W, int64_t* workspace_bytes_host, in
 int teco_jpeg_encode_rgb8(const uint8_t* rgb, int32_t H, int32_t W, void* workspace, int64_t workspace_bytes, uint8_t* out,
                           int64_t out_capacity, int64_t* out_len, void* stream);
 
+/* ---------------------------------------------------------------------------------------
+ * GIF89a encoding of a batch of RGB uint8 animations, the TensorBoard image summaries of training (reference
+ * lib/Teco.py:498-503, lib/ops.py:399-431): per animation one median-cut palette of up to 256 colours over all of its
+ * frames, Sierra-2-4A error diffusion per frame, LZW at minimum code size 8, 33 cs per frame, looping.  DESIGN.md
+ * section 4.8 specifies every rule; an animation of at most 256 distinct colours is stored exactly.
+ * ------------------------------------------------------------------------------------- */
+/* tf.image.convert_image_dtype(x, uint8, saturate=True) in float32: y = trunc(clamp(x * 255.5, 0, 255)), NaN -> 0;
+   deprocess = 1 first maps x to (x + 1) / 2 (reference lib/ops.py:17-22).  n elements, any layout. */
+int teco_convert_image_u8(const float* x, uint8_t* y, int64_t n, int32_t deprocess, void* stream);
+/* Host-only size query for N animations of T frames of H x W: the workspace (device, 256-byte aligned) and the output
+ * capacity in bytes.  N, T >= 1, 1 <= H, W <= 65535 and T * H * W <= 2^28, else TECO_E_INVALID. */
+int teco_gif_plan_bytes(int32_t N, int32_t T, int32_t H, int32_t W, int64_t* workspace_bytes_host,
+                        int64_t* out_capacity_host);
+/* rgb [N,T,H,W,3] uint8 -> out: the N GIF files back to back; out_len (device int64 [N]) receives each file's length,
+ * so file i starts at the sum of the lengths before it.  Buffers smaller than teco_gif_plan_bytes gives ->
+ * TECO_E_INVALID.  Nothing allocates; every stage runs on `stream`. */
+int teco_gif_encode_rgb8(const uint8_t* rgb, int32_t N, int32_t T, int32_t H, int32_t W, void* workspace,
+                         int64_t workspace_bytes, uint8_t* out, int64_t out_capacity, int64_t* out_len, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -411,6 +411,8 @@ def train(FLAGS):
     if monitor:
         from tecogan_b200.summary import EventWriter
         writer = EventWriter(FLAGS.summary_dir)
+        # the GIF summaries go to a sibling run: readers of the scalar file see only simple values
+        gif_writer = EventWriter(os.path.join(FLAGS.summary_dir, 'gif'))
         val_hr = validation_source(FLAGS, dev)
         test_while_train(FLAGS, start_step)
     tested = {start_step}
@@ -432,6 +434,7 @@ def train(FLAGS):
             if monitor and (run_step % FLAGS.summary_freq) == 0:     # reference main.py:384-402
                 print('Run and Recording summary!!')
                 writer.add_scalars(run_step, [('learning_rate', res["lr"])] + list(zip(Net.update_list_name, Net.update_list_avg())))
+                gif_writer.add_images(run_step, Net.image_summary())
                 if val_hr is not None:
                     val = Net.train.evaluate(*frvsr_gpu_data_loader(val_hr(run_step // FLAGS.summary_freq), FLAGS))
                     writer.add_scalars(run_step, [('val_' + name, v) for name, v in val.items()])
@@ -470,6 +473,7 @@ def train(FLAGS):
             test_while_train(FLAGS, Net.global_step())
     if monitor:
         writer.close()
+        gif_writer.close()
     print('Optimization done!!!!!!!!!!!!')
     if world > 1:
         dist.destroy_process_group()

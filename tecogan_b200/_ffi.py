@@ -102,6 +102,9 @@ SIGNATURES = {
     "teco_png_decode_rgb8": [_P, _I64, _P, _I32, _P, _I64, _P, _I64, _P, _P],
     "teco_jpeg_plan_bytes": [_I32, _I32, _P, _P],
     "teco_jpeg_encode_rgb8": [_P, _I32, _I32, _P, _I64, _P, _I64, _P, _P],
+    "teco_convert_image_u8": [_P, _P, _I64, _I32, _P],
+    "teco_gif_plan_bytes": [_I32, _I32, _I32, _I32, _P, _P],
+    "teco_gif_encode_rgb8": [_P, _I32, _I32, _I32, _I32, _P, _I64, _P, _I64, _P, _P],
 }
 _RESTYPES = {"teco_packed_weight_bytes": C.c_int64, "teco_crc32c": C.c_int64}
 

@@ -124,12 +124,13 @@ class _Graph:
         s_input_warp = K.dense_image_warp(pre.reshape(B * (T - 1), crop, crop, 3).contiguous(), gen_flow_lr)  # :120-122
         # ---- recurrent generator (lib/Teco.py:125-164)
         zeros48 = torch.zeros((B, crop, crop, 48), device=r_inputs.device, dtype=torch.float32)
-        gen_outputs = []
+        gen_outputs, gen_warppre = [], []
         with variable_scope('generator'):
             gen_pre = generator_F(torch.cat((r_inputs[:, 0], zeros48), dim=-1), 3, reuse=False, FLAGS=FLAGS)
             gen_outputs.append(gen_pre)
             for t in range(T - 1):
                 warped = K.dense_image_warp(gen_pre, gen_flow[:, t].contiguous())
+                gen_warppre.append(warped)
                 s2d = K.space_to_depth4(deprocess(warped))
                 gen_pre = generator_F(torch.cat((r_inputs[:, t + 1], s2d), dim=-1), 3, reuse=True, FLAGS=FLAGS)
                 gen_outputs.append(gen_pre)
@@ -247,6 +248,7 @@ class _Graph:
         update_list += [gen_loss]
         update_list_name += ["All_loss_Gen"]
         self.gen_outputs, self.s_gen_output = gen_outputs, s_gen_output
+        self.r_inputs, self.r_targets, self.gen_warppre = r_inputs, r_targets, gen_warppre   # the image summary's (:498-503)
         self.gen_loss = gen_loss
         self.fnet_loss = FLAGS.warp_scaling * warp_loss + gen_loss    # :443
         self.update_list, self.update_list_name = update_list, update_list_name
@@ -309,6 +311,8 @@ class _TrainState:
         self.counter1 = self.counter2 = 0
         self.last = None
         self.eval_in = self.eval_tg = self.eval_graph = None   # evaluate(): buffers and graph of its own
+        self._summary_src = None
+        self._gif = None
         from .. import config
         K.tc_cache_clear()                         # packed bf16 weights of a previous trainer are not ours
         prev_precision = config.precision()
@@ -376,6 +380,7 @@ class _TrainState:
         self._scal_off, self._n_scal = o, scal.numel()
         self._names_now = g.update_list_name
         self._gen_outputs = g.gen_outputs.detach()
+        self._summary_src = (g.r_inputs, g.r_targets, self._gen_outputs, [w.detach() for w in g.gen_warppre])
 
     def __call__(self, r_inputs=None, r_targets=None):
         F = self.FLAGS
@@ -465,6 +470,36 @@ class _TrainState:
         else:
             self._evaluate_compute()
         return dict(zip(self._eval_names, self._eval_scal.tolist()))
+
+    # ---- GIF image summaries (reference lib/Teco.py:498-503, lib/ops.py:434-484) -------------------------------------
+    def image_summary(self):
+        """The reference's four GIF summaries of the last training step's own batch and forward pass (the weights before
+        that step's update): [(tag, height, width, GIF bytes)] for LR = r_inputs, HR = deprocess(r_targets), Generated =
+        deprocess(gen_outputs) and WarpPreGen = deprocess(the T - 1 warped previous outputs), each the first
+        min(4, batch_size) clips of the step (ping-pong extended with --pingpang), quantised as
+        tf.image.convert_image_dtype(saturate=True).  Tags image_summaries/<name>/gif/<i>, or .../gif when one clip is
+        written.  Quantisation and the four encodes run on the device; the host waits for them together."""
+        if self._summary_src is None:
+            raise RuntimeError("image_summary: no training step has run yet")
+        from ..gif import GifEncoder, convert_image_u8
+        from .._encode import collect
+        lr, hr, gen, warppre = self._summary_src
+        k = min(4, self.FLAGS.batch_size)
+        if self._gif is None:
+            self._gif = {name: GifEncoder("image_summary " + name) for name in ("LR", "HR", "Generated", "WarpPreGen")}
+        srcs = (("LR", lr[:k], False), ("HR", hr[:k], True), ("Generated", gen[:k], True),
+                ("WarpPreGen", torch.stack([w[:k] for w in warppre], dim=1), True))
+        pending, shapes = [], []
+        for name, x, dep in srcs:
+            u8 = convert_image_u8(x, deprocess=dep)
+            pending.append(self._gif[name].launch(u8))
+            shapes.append((name, int(u8.shape[2]), int(u8.shape[3])))
+        out = []
+        for (name, h, w), files in zip(shapes, collect(pending)):
+            for i, data in enumerate(files):
+                tag = "image_summaries/%s/gif" % name + ("" if k == 1 else "/%d" % i)
+                out.append((tag, h, w, data))
+        return out
 
     # ---- checkpoint / resume (reference: tf.train.Saver over GLOBAL_VARIABLES, main.py:307,346-349) -------------------
     def state_tensors(self):
@@ -575,7 +610,7 @@ def TecoGAN(r_inputs, r_targets, FLAGS, GAN_Flag=True):
         update_list=[float(v) for v in g0.update_list],
         update_list_name=names_avg,
         update_list_avg=state.update_list_avg,
-        image_summary=None,          # gif summaries are observability only (SURVEY section 2 row 13)
+        image_summary=state.image_summary,
         global_step=lambda: state.global_step,
     )
 

@@ -5,7 +5,9 @@ An event file `events.out.tfevents.<unix time>.<hostname>` is a TFRecord stream:
 length, the masked CRC32C of those 8 bytes, the payload, the masked CRC32C of the payload.  Each payload is an `Event`
 proto (tensorflow/core/util/event.proto): the first carries file_version = "brain.Event:2"; every later one wall_time
 (field 1, double), step (2, int64) and a Summary (5) whose repeated Value (1) holds tag (1, string) and simple_value
-(2, float) -- what tf.summary.scalar + FileWriter.add_summary write.  CRC and protobuf encoding are tf_bundle's."""
+(2, float) -- what tf.summary.scalar + FileWriter.add_summary write -- or an image (4): Summary.Image with height (1,
+int32), width (2), colorspace (3) and encoded_image_string (4), what the reference's GIF summaries write
+(lib/ops.py:434-484).  CRC and protobuf encoding are tf_bundle's."""
 import os
 import socket
 import struct
@@ -37,8 +39,14 @@ def _scalar_summary(pairs):
                     for tag, v in pairs)
 
 
+def _image_summary(items):
+    return b"".join(_pb_bytes(1, _pb_bytes(1, str(tag).encode()) + _pb_bytes(4, _pb_varint(1, int(h)) + _pb_varint(2, int(w))
+                                                                             + _pb_varint(3, 3) + _pb_bytes(4, bytes(data))))
+                    for tag, h, w, data in items)
+
+
 class EventWriter:
-    """Scalar summaries for TensorBoard in `logdir` (tf.summary.FileWriter's file naming and record format)."""
+    """Scalar and image summaries for TensorBoard in `logdir` (tf.summary.FileWriter's file naming and record format)."""
 
     def __init__(self, logdir):
         os.makedirs(logdir, exist_ok=True)
@@ -53,6 +61,10 @@ class EventWriter:
     def add_scalars(self, step, pairs):
         """One Event at `step` holding a simple_value per (tag, value) of `pairs`."""
         self._write(_event(time.time(), step=step, summary=_scalar_summary(pairs)))
+
+    def add_images(self, step, items):
+        """One Event at `step` holding an RGB image (colorspace 3) per (tag, height, width, encoded bytes) of `items`."""
+        self._write(_event(time.time(), step=step, summary=_image_summary(items)))
 
     def close(self):
         self._f.close()
