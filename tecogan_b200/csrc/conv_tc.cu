@@ -870,42 +870,69 @@ conv3x3_f32out_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_con
 // A chain of 3x3 64 -> 64 layers on 32 x 32 images in one launch, the activations never leaving shared memory.  A cluster
 // of two CTAs (one per SM, persistent) owns clips c, c + G, ... (G clusters); CTA r of the cluster owns image rows
 // 16 r .. 16 r + 15 for every layer.
-//   - Two activation slots per CTA, each [18 rows][34 px][64 ch] bf16 in the SW128 image: the own rows, one halo row above
-//     and below, a zero column either side.  Slot 0 holds the plan's buffer 0 (x_in, read by layer 0 only) and then
-//     buffer 2; slot 1 holds buffer 1.  Layer l reads slot l & 1 and writes the other.  x_in arrives as one 4-D TMA box
-//     {64, 34, 18} at (0, -1, 16 r - 1, n), whose out-of-bounds zero fill is the padding; slot 1 is zeroed once, and rows and
-//     columns no layer writes stay zero.
+//   - Shared memory: the weight ring (9 taps x 8 KB, one whole layer), two activation slots and the mbarriers.  Each slot
+//     is [18 rows][34 px][64 ch] bf16 in the SW128 image: the own rows, one halo row above and below, a zero column
+//     either side.  Slot 0 holds the plan's buffer 0 (x_in, read by layer 0 only) and then buffer 2; slot 1 holds buffer
+//     1.  Layer l reads slot l & 1 and writes the other.  x_in arrives as one 4-D TMA box {64, 34, 18} at
+//     (0, -1, 16 r - 1, n), whose out-of-bounds zero fill is the padding; slot 1 is zeroed once, and rows and columns no
+//     layer writes stay zero.
 //   - The MMAs and the epilogue arithmetic are those of conv3x3_ws_kernel<0>, so the results are bit-identical to it: per
 //     16 x 8 tile one m64n128k16 accumulator, the weight tap as A and the slot at the tap's offset as B (8-pixel groups one
-//     34-pixel row apart), taps 0..8 x K-steps 0..3, scale-d = 0 first; bias -> activation -> (+ bf16 residual) -> bf16.
-//     Consumer warpgroup g owns column strips 2 g and 2 g + 1 (two accumulators) and issues tap-outer, alternating
-//     between them, one commit group per tap.
-//   - One producer warp streams the taps of every layer through a ring of TR_WSLOTS 8 KB slots; a slot is released once
-//     wgmma.wait_group shows its tap's MMAs complete in both warpgroups (one arrival per consumer warp).
+//     34-pixel row apart), taps 0..8 x K-steps 0..3, scale-d = 0 first, one commit group per tap; bias -> activation ->
+//     (+ bf16 residual) -> bf16.
+//   - Strip s (0..3) is the 16 x 8 tile at columns 8 s .. 8 s + 7.  Consumer warpgroup 0 owns strips 0 and 1 and works on
+//     them in that order, warpgroup 1 strips 3 and 2; write M(l, s) for the MMAs of strip s at layer l and E(l, s) for
+//     its epilogue.  The warpgroups take turns to issue a whole strip (named barriers 1 and 2, as in conv3x3_ws_kernel):
+//     W0 M(l, 0), W1 M(l, 3), W0 M(l, 1), W1 M(l, 2), W0 M(l + 1, 0), ...  A warpgroup waits for its first strip and
+//     runs its epilogue under the other warpgroup's strip before it issues its second, and runs the epilogue of its
+//     second strip under the other warpgroup's second one, so the tensor pipe has a strip queued across the layer
+//     boundary as long as an epilogue takes less than a strip's 36 MMAs.
+//   - Weights: one producer warp loads tap t of every layer into ring slot t.  A slot is released (8 arrivals, one per
+//     consumer warp) once the warp has seen the tap complete in both of its warpgroup's strips: by wgmma.wait_group per
+//     tap of its second strip, with no epilogue in between, so layer l + 1's tap t reloads while layer l's later taps
+//     still run.
 //   - The epilogue stmatrix-es the bf16 outputs straight into the other slot (an in-place residual is ldmatrix-ed from the
-//     same place first); the 128-byte swizzle chunk is taken from the address, as the TMA and the MMAs apply it.  After
-//     a generic -> async proxy fence and a barrier over the consumers, one thread bulk-copies the CTA's boundary row into
-//     the partner's halo row of the same slot (16 rows x 4352 B is a multiple of 1024: the swizzled bytes copy unchanged),
-//     completing on the partner's row_full[slot] mbarrier.
+//     same place first); the 128-byte swizzle chunk is taken from the address, as the TMA and the MMAs apply it.  After a
+//     generic -> async proxy fence and a barrier over the warpgroup, one of its threads bulk-copies the strip's 1 KB of
+//     the CTA's boundary row into the partner's halo row of the same slot (16 x 4352 B and 1024 s are multiples of
+//     1024: the swizzled bytes copy unchanged), completing on the partner's row_full[slot][s].
 //   - After a clip's last layer the consumers copy the CTA's own 16 rows of each slot the plan wrote to global memory with
 //     16-byte stores (un-swizzling the address); after a barrier one thread loads the next clip's x_in into slot 0.
-// Lock step: a CTA's layer l reads the partner's layer l - 1 row, which the partner sends only after all of its layer
-// l - 1 MMAs (both warpgroups waited for them before their epilogues) -- and those needed this CTA's layer l - 2 row.
-// Hence (a) when this CTA's layer-l row lands in the partner's slot, the partner has finished reading that slot (its layer
-// l - 1 input); (b) the source row of this CTA's layer-l copy is rewritten at layer l + 2 only after the partner received
-// it, so the copy has read it; (c) row_full[s] completes one phase per two layers, the next copy into slot s needing the
-// row this CTA sends after waiting for the current one.  Across clips the partner's first copy (layer 0, slot 1) waits on
-// peer_free, which this CTA arrives on remotely once it has waited for the partner's last row of the clip.
+// Dependencies (si = l & 1 is layer l's input slot, so = si ^ 1 its output slot).  M(l + 1, s) reads the columns of
+// strips s - 1 .. s + 1 of slot so, in the own rows and in the partner's halo row.
+//   - RAW, own rows: M(l + 1, s) follows E(l, s - 1 .. s + 1).  Within a warpgroup by program order; across the strip 1 |
+//     strip 2 boundary through mid[g][so], on which every thread of warpgroup g arrives after E(l, 1 + g) and its
+//     fence.proxy.async.  Each warpgroup runs its boundary epilogue before it next waits for the other one.
+//   - RAW, partner rows: M(l + 1, s) waits on row_full[so][s - 1 .. s + 1].
+//   - WAR, own rows: E(l + 1, s) overwrites in slot si what M(l, s - 1 .. s + 1) read.  The warpgroup waited for its own
+//     M(l, .) before its epilogues, and the other warpgroup's boundary strip M(l, .) completed before that warpgroup's
+//     E(l, .) arrived on mid[.][so], which M(l + 1, s) -- before E(l + 1, s) in program order -- waited for.
+//   - WAR, the partner's halo row: this CTA sends row (l, s) after its M(l, s), which needed the partner's rows
+//     (l - 1, s - 1 .. s + 1); the partner sent each after its E(l - 1, .), i.e. after its M(l - 1, .) that read the
+//     halo columns of strip s in slot so had completed.  So the copy lands in columns the partner has finished reading.
+//   - WAR, the source row: this CTA's row (l, s) in slot so is next rewritten by E(l + 2, s), after M(l + 2, s), which
+//     needed the partner's row (l + 1, s), sent after the partner's M(l + 1, s), which waited for row (l, s) to land:
+//     the copy has read its source.
+//   - row_full[i][s] and mid[g][i] complete one phase per layer that writes slot i.  The next phase's bytes or arrivals
+//     come from a layer two later, which needs the current phase's waiters to have moved on (the same chains as above),
+//     and this CTA's expect_tx for a phase follows its wait for the previous one in program order.
+//   - Clips: the first wait of a clip is on x_in in slot 0.  Before loading it, thread 0 has waited (a) for the
+//     partner's last-layer rows (every consumer did) and (b) on peer_free, on which the partner arrives remotely once
+//     it has waited for this CTA's last-layer rows.  So the next clip's TMA, epilogues and copies find every copy of the
+//     previous clip landed and every source read.
 constexpr int TR_COLS = LIN_W + 2;                                        // 34: a zero column either side
 constexpr int TR_ROWS = 16 + 2;                                           // own rows + a halo row above and below
 constexpr uint32_t TR_ROW_BYTES = TR_COLS * 128u;                         // 4352: wgmma SBO between tile rows
-constexpr uint32_t TR_SLOT = (TR_ROWS * TR_ROW_BYTES + 1023u) & ~1023u;   // 78848: slots start on the swizzle period
-constexpr int TR_WSLOTS = 8;                                              // weight ring depth (taps)
+constexpr uint32_t TR_SLOT_BYTES = TR_ROWS * TR_ROW_BYTES;                // 78336
 constexpr uint32_t TR_TAP = 64u * 128u;                                   // one packed tap [64 cout][64 cin]
-constexpr uint32_t TR_EDGE_BYTES = LIN_W * 128u;                          // one boundary row without its zero columns
-constexpr int TR_BARS = 2 * TR_WSLOTS + 4;                                // full[], empty[], row_full[2], x_full, peer_free
-constexpr size_t TR_SMEM = 1024 + 2 * (size_t)TR_SLOT + TR_WSLOTS * (size_t)TR_TAP + TR_BARS * sizeof(uint64_t);
+constexpr uint32_t TR_SLOT0 = LAYER_W_BYTES;                              // 73728: after the nine-tap weight ring
+constexpr uint32_t TR_SLOT1 = (TR_SLOT0 + TR_SLOT_BYTES + 1023u) & ~1023u;   // 152576: slots start on the swizzle period
+constexpr uint32_t TR_BAR_OFF = TR_SLOT1 + TR_SLOT_BYTES;                 // 230912
+constexpr uint32_t TR_STRIP_EDGE = TILE_COLS * 128u;                      // one strip's part of a boundary row: 1024
+constexpr int TR_BARS = 9 + 9 + 2 * 4 + 2 * 2 + 2;                        // full, empty, row_full, mid, x_full, peer_free
+constexpr size_t TR_SMEM = 1024 + TR_BAR_OFF + TR_BARS * sizeof(uint64_t);
 static_assert(TR_SMEM <= SMEM_MAX, "conv3x3_trunk_cluster_kernel: shared memory budget");
+static_assert(TR_SLOT0 % 1024 == 0 && TR_SLOT1 % 1024 == 0, "slots start on the swizzle period");
 static_assert((16 * TR_ROW_BYTES) % 1024 == 0, "a boundary row and the partner's halo row share their swizzle phase");
 
 struct TrunkParams {
@@ -964,23 +991,44 @@ __device__ __forceinline__ void trunk_epilogue(const float (&acc)[64], const flo
   }
 }
 
-template <int ACT>
-__device__ __forceinline__ void trunk_epilogue2(const float (&acc0)[64], const float (&acc1)[64], const float (&b)[2],
-                                                uint32_t slot, int x0, bool res, int wq, int lane) {
-  trunk_epilogue<ACT>(acc0, b, slot, x0, res, wq, lane);
-  trunk_epilogue<ACT>(acc1, b, slot, x0 + TILE_COLS, res, wq, lane);
+// M(l, s): the 9 taps x 4 K-steps of one strip into acc, B from the input slot at the strip's column (b_a), tap t from
+// ring slot t once full[t] shows it loaded (parity wpar); one commit group per tap.
+__device__ __forceinline__ void trunk_issue_strip(float (&acc)[64], uint32_t wring_a, const uint64_t* full, uint32_t wpar,
+                                                  uint32_t b_a) {
+#pragma unroll
+  for (int t = 0; t < 9; ++t) {
+    mbar_wait(smem_u32(&full[t]), wpar);
+    wgmma_fence();
+    const uint32_t a0 = wring_a + (uint32_t)t * TR_TAP;
+    const uint32_t b0 = b_a + (uint32_t)(((t / 3) * TR_COLS + t % 3) * 128);
+#pragma unroll
+    for (int kk = 0; kk < CB / 16; ++kk)
+      Wgmma<128, 0, 0>::run(acc, gmma_desc_sw128(a0 + 32u * kk, 16u, 1024u), gmma_desc_sw128(b0 + 32u * kk, 16u, TR_ROW_BYTES),
+                            t == 0 && kk == 0 ? 0u : 1u);
+    wgmma_commit();
+  }
+}
+
+// With the second strip's 9 commit groups issued and the first strip's complete: release ring slot T, T + 1, .. 8 as the
+// second strip's tap completes.  ptxas encodes a wait for at most 8 pending groups as one for at most 7, so slot 0 goes
+// with slot 1.
+template <int T>
+__device__ __forceinline__ void trunk_release_taps(const uint64_t* empty, bool lane0) {
+  wgmma_wait<8 - T>();
+  mbar_arrive_if(smem_u32(&empty[T]), lane0);
+  if constexpr (T < 8) trunk_release_taps<T + 1>(empty, lane0);
 }
 
 __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(WS_THREADS, 1)
 conv3x3_trunk_cluster_kernel(const __grid_constant__ CUtensorMap xmap, const TrunkParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint8_t* wring = smem + 2 * (size_t)TR_SLOT;
-  uint64_t* full = reinterpret_cast<uint64_t*>(wring + TR_WSLOTS * (size_t)TR_TAP);   // [TR_WSLOTS]
-  uint64_t* empty = full + TR_WSLOTS;                                                 // [TR_WSLOTS]
-  uint64_t* row_full = empty + TR_WSLOTS;        // [2]: the partner's boundary row has landed in slot s
-  uint64_t* x_full = row_full + 2;               // x_in of the clip has landed in slot 0
-  uint64_t* peer_free = x_full + 1;              // the partner has taken this CTA's last row of the previous clip
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + TR_BAR_OFF);   // [9]: tap t of the current layer is in ring slot t
+  uint64_t* empty = full + 9;                    // [9]: every consumer warp is done with ring slot t
+  uint64_t* row_full = empty + 9;                // [2][4]: strip s of the partner's boundary row has landed in slot i
+  uint64_t* mid = row_full + 8;                  // [2][2]: warpgroup g's strip 1 + g is in slot i
+  uint64_t* x_full = mid + 4;                    // x_in of the clip has landed in slot 0
+  uint64_t* peer_free = x_full + 1;              // the partner has taken this CTA's last rows of the previous clip
 
   const int tid = threadIdx.x, wg = tid >> 7;
   const uint32_t rank = cluster_ctarank(), peer = rank ^ 1u;
@@ -988,26 +1036,30 @@ conv3x3_trunk_cluster_kernel(const __grid_constant__ CUtensorMap xmap, const Tru
   const int my_clips = cl < p.N ? (p.N - cl + G - 1) / G : 0;
 
   if (tid == 0) {
-    for (int s = 0; s < TR_WSLOTS; ++s) {
-      mbar_init(smem_u32(&full[s]), 1);
-      mbar_init(smem_u32(&empty[s]), 8);         // one arrival per consumer warp
+    for (int t = 0; t < 9; ++t) {
+      mbar_init(smem_u32(&full[t]), 1);
+      mbar_init(smem_u32(&empty[t]), 8);         // one arrival per consumer warp
     }
-    for (int i = 0; i < 4; ++i) mbar_init(smem_u32(&row_full[i]), 1);   // row_full[2], x_full, peer_free
+    for (int i = 0; i < 8; ++i) mbar_init(smem_u32(&row_full[i]), 1);
+    for (int i = 0; i < 4; ++i) mbar_init(smem_u32(&mid[i]), 128);   // every thread of the warpgroup
+    mbar_init(smem_u32(x_full), 1);
+    mbar_init(smem_u32(peer_free), 1);
     fence_mbar_init();
   }
-  for (uint32_t i = tid; i < TR_SLOT / 16; i += WS_THREADS)    // slot 1 is never TMA-loaded: its padding is zeroed here
-    asm volatile("st.shared.v4.u32 [%0], {%1, %1, %1, %1};" ::"r"(smem_u32(smem + TR_SLOT) + 16 * i), "r"(0) : "memory");
+  for (uint32_t i = tid; i < TR_SLOT_BYTES / 16; i += WS_THREADS)   // slot 1 is never TMA-loaded: its padding is zeroed here
+    asm volatile("st.shared.v4.u32 [%0], {%1, %1, %1, %1};" ::"r"(smem_u32(smem + TR_SLOT1) + 16 * i), "r"(0) : "memory");
   fence_async_smem();
   cluster_sync();                                // both CTAs' barriers are initialised before any remote access
 
-  if (wg == 2) {                                 // producer warp: one lane streams every tap of every layer and clip
+  if (wg == 2) {                                 // producer warp: one lane loads every tap of every layer and clip
     if (tid == NUM_THREADS) {
-      const int per_clip = 9 * p.L, total = my_clips * per_clip;
-      for (int q = 0, lt = 0; q < total; ++q, lt = lt + 1 == per_clip ? 0 : lt + 1) {
-        const int s = q % TR_WSLOTS;
-        if (q >= TR_WSLOTS) mbar_wait(smem_u32(&empty[s]), (uint32_t)((q / TR_WSLOTS - 1) & 1));
-        mbar_expect_tx(smem_u32(&full[s]), TR_TAP);
-        bulk_load_1d(smem_u32(wring + s * TR_TAP), p.wpk + (size_t)lt * TR_TAP, TR_TAP, smem_u32(&full[s]));
+      for (int u = 0; u < my_clips * p.L; ++u) {   // u: layers loaded so far; tap t of each goes to ring slot t
+        const int l = u % p.L;
+        for (int t = 0; t < 9; ++t) {
+          if (u > 0) mbar_wait(smem_u32(&empty[t]), (uint32_t)(u - 1) & 1u);
+          mbar_expect_tx(smem_u32(&full[t]), TR_TAP);
+          bulk_load_1d(smem_u32(smem + t * TR_TAP), p.wpk + ((size_t)l * 9 + t) * TR_TAP, TR_TAP, smem_u32(&full[t]));
+        }
       }
     }
     __syncwarp();
@@ -1016,87 +1068,89 @@ conv3x3_trunk_cluster_kernel(const __grid_constant__ CUtensorMap xmap, const Tru
   }
 
   const int wq = (tid >> 5) & 3, lane = tid & 31;
-  const uint32_t slot0 = smem_u32(smem), wring_a = smem_u32(wring);
+  const bool leader = (tid & 127) == 0;          // issues this warpgroup's boundary-row copies
+  const uint32_t wring_a = smem_u32(smem);
+  auto slot_a = [&](uint32_t i) { return wring_a + (i ? TR_SLOT1 : TR_SLOT0); };
   const int y0 = 16 * (int)rank;                 // first image row of this CTA
   // this CTA's boundary row (buffer row 16 for r = 0, 1 for r = 1) -> the partner's halo row (0, resp. 17); column 1 on
   const uint32_t edge_src = (rank == 0 ? 16u : 1u) * TR_ROW_BYTES + 128u;
   const uint32_t edge_dst = (rank == 0 ? 0u : 17u) * TR_ROW_BYTES + 128u;
-  const int xa = 2 * TILE_COLS * wg;             // strips 2 wg and 2 wg + 1 start at columns xa and xa + 8
+  const int sa = wg == 0 ? 0 : 3, sb = wg == 0 ? 1 : 2;   // this warpgroup's first and second strip
+  const int my_turn = 1 + wg, other_turn = 2 - wg;        // named barrier 1 + g: warpgroup g may issue a strip
   auto load_x = [&](int n) {
-    mbar_expect_tx(smem_u32(x_full), TR_ROWS * TR_ROW_BYTES);
-    tma_load_4d(slot0, &xmap, smem_u32(x_full), 0, -1, y0 - 1, n);
+    mbar_expect_tx(smem_u32(x_full), TR_SLOT_BYTES);
+    tma_load_4d(slot_a(0), &xmap, smem_u32(x_full), 0, -1, y0 - 1, n);
+  };
+  // wait for the partner's rows of strips s - 1 .. s + 1 in slot i
+  auto wait_rows = [&](uint32_t i, int s, uint32_t par) {
+    for (int x = s > 0 ? s - 1 : 0; x <= (s < 3 ? s + 1 : 3); ++x) mbar_wait(smem_u32(&row_full[4 * i + x]), par);
   };
   if (tid == 0 && my_clips > 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(&xmap) : "memory");
     load_x(cl);
   }
 
-  float acc0[64], acc1[64];
-  uint32_t q = 0;                                // taps consumed
-  uint32_t row_par = 0;                          // bit s: phase parity of row_full[s]
+  float acc0[64], acc1[64];                      // strips sa and sb
+  uint32_t ph = 0;                               // bit i: parity of the next phase of row_full[i][.] and mid[.][i]
   for (int k = 0; k < my_clips; ++k) {
     const int n = cl + k * G;
     for (int l = 0; l < p.L; ++l) {
-      const uint32_t si = (uint32_t)l & 1u, so = si ^ 1u;
-      if (l == 0) {
-        mbar_wait(smem_u32(x_full), (uint32_t)k & 1u);
-      } else {
-        mbar_wait(smem_u32(&row_full[si]), (row_par >> si) & 1u);
-        row_par ^= 1u << si;
-      }
+      const uint32_t si = (uint32_t)l & 1u, so = si ^ 1u, par = (ph >> si) & 1u;
+      const uint32_t wpar = (uint32_t)(k * p.L + l) & 1u;   // parity of full[.] for this layer's taps
+      const uint32_t in_a = slot_a(si), out_a = slot_a(so);
+      const bool last_turn = k + 1 == my_clips && l + 1 == p.L;
+
+      if (l == 0) mbar_wait(smem_u32(x_full), (uint32_t)k & 1u);
+      else wait_rows(si, sa, par);
+      if (wg == 1 || k > 0 || l > 0) named_bar_sync(my_turn, 2 * 128);
+      trunk_issue_strip(acc0, wring_a, full, wpar, in_a + (uint32_t)(TILE_COLS * sa) * 128u);
+      named_bar_arrive(other_turn, 2 * 128);
+
       const float* bl = p.bias + 64 * l;
       const float b[2] = {bl[16 * wq + (lane >> 2)], bl[16 * wq + 8 + (lane >> 2)]};
-      const uint32_t in_a = slot0 + si * TR_SLOT + (uint32_t)xa * 128u;
-#pragma unroll
-      for (int t = 0; t < 9; ++t, ++q) {
-        const uint32_t s = q % TR_WSLOTS;
-        mbar_wait(smem_u32(&full[s]), (q / TR_WSLOTS) & 1u);
-        wgmma_fence();
-        const uint32_t a0 = wring_a + s * TR_TAP;
-        const uint32_t b0 = in_a + (uint32_t)(((t / 3) * TR_COLS + t % 3) * 128);
-#pragma unroll
-        for (int kk = 0; kk < CB / 16; ++kk)
-          Wgmma<128, 0, 0>::run(acc0, gmma_desc_sw128(a0 + 32u * kk, 16u, 1024u), gmma_desc_sw128(b0 + 32u * kk, 16u, TR_ROW_BYTES),
-                                t == 0 && kk == 0 ? 0u : 1u);
-#pragma unroll
-        for (int kk = 0; kk < CB / 16; ++kk)
-          Wgmma<128, 0, 0>::run(acc1, gmma_desc_sw128(a0 + 32u * kk, 16u, 1024u),
-                                gmma_desc_sw128(b0 + TILE_COLS * 128u + 32u * kk, 16u, TR_ROW_BYTES), t == 0 && kk == 0 ? 0u : 1u);
-        wgmma_commit();
-        if (t > 0) {
-          wgmma_wait<1>();                       // tap t - 1 has completed in this warpgroup
-          mbar_arrive_if(smem_u32(&empty[(q - 1) % TR_WSLOTS]), lane == 0);
-        }
-      }
-      wgmma_wait_all_fence(acc0);
-      wgmma_wait_all_fence(acc1);
-      if (lane == 0) mbar_arrive(smem_u32(&empty[(q - 1) % TR_WSLOTS]));
-
-      const uint32_t out_a = slot0 + so * TR_SLOT;
       const bool res = (p.res_mask >> l) & 1u;
-      // once per layer: the element loop is compiled per activation
-      if ((p.relu_mask >> l) & 1u) trunk_epilogue2<TECO_ACT_RELU>(acc0, acc1, b, out_a, xa, res, wq, lane);
-      else if ((p.lrelu_mask >> l) & 1u) trunk_epilogue2<TECO_ACT_LRELU02>(acc0, acc1, b, out_a, xa, res, wq, lane);
-      else trunk_epilogue2<TECO_ACT_NONE>(acc0, acc1, b, out_a, xa, res, wq, lane);
-      fence_async_smem();                        // the stmatrix writes -> visible to the MMAs and the bulk copies
-      named_bar_sync(1, NUM_THREADS);            // the whole layer is in slot so (and every MMA on slot si is done)
-      if (tid == 0) {
-        mbar_expect_tx(smem_u32(&row_full[so]), TR_EDGE_BYTES);   // the partner's row of this layer
-        if (l == 0 && k > 0) mbar_wait(smem_u32(peer_free), (uint32_t)(k - 1) & 1u);
-        bulk_copy_to_peer(mapa_shared(out_a + edge_dst, peer), out_a + edge_src, TR_EDGE_BYTES,
-                          mapa_shared(smem_u32(&row_full[so]), peer));
+      auto epilogue = [&](const float (&acc)[64], int s) {   // E(l, s), then its boundary-row copy
+        // once per strip: the element loop is compiled per activation
+        if ((p.relu_mask >> l) & 1u) trunk_epilogue<TECO_ACT_RELU>(acc, b, out_a, TILE_COLS * s, res, wq, lane);
+        else if ((p.lrelu_mask >> l) & 1u) trunk_epilogue<TECO_ACT_LRELU02>(acc, b, out_a, TILE_COLS * s, res, wq, lane);
+        else trunk_epilogue<TECO_ACT_NONE>(acc, b, out_a, TILE_COLS * s, res, wq, lane);
+        fence_async_smem();                      // the stmatrix writes -> visible to the MMAs and the bulk copy
+        if (s == sb) mbar_arrive(smem_u32(&mid[2 * wg + so]));
+        named_bar_sync(3 + wg, 128);
+        if (leader) {
+          const uint32_t e = (uint32_t)s * TR_STRIP_EDGE, bar = smem_u32(&row_full[4 * so + s]);
+          mbar_expect_tx(bar, TR_STRIP_EDGE);    // the partner's row of this strip and layer
+          bulk_copy_to_peer(mapa_shared(out_a + edge_dst + e, peer), out_a + edge_src + e, TR_STRIP_EDGE, mapa_shared(bar, peer));
+        }
+      };
+      wgmma_wait_all_fence(acc0);                // the first strip has completed: its epilogue runs under the other
+      epilogue(acc0, sa);                        // warpgroup's strip
+
+      if (l > 0) {
+        wait_rows(si, sb, par);
+        mbar_wait(smem_u32(&mid[2 * (wg ^ 1) + si]), par);   // the other warpgroup's E(l - 1, 2 - wg)
+        ph ^= 1u << si;
       }
+      named_bar_sync(my_turn, 2 * 128);
+      trunk_issue_strip(acc1, wring_a, full, wpar, in_a + (uint32_t)(TILE_COLS * sb) * 128u);
+      if (!(wg == 1 && last_turn)) named_bar_arrive(other_turn, 2 * 128);
+      trunk_release_taps<0>(empty, lane == 0);   // ring slot t as the second strip's tap t completes
+      wgmma_wait_all_fence(acc1);
+      epilogue(acc1, sb);
     }
-    // the partner's row of the last layer: no layer reads it, but its copy must have landed before the slot is reused
+    // the partner's rows of the last layer: no layer reads them, but their copies must have landed before the slot is
+    // reused
     const uint32_t sf = (uint32_t)((p.L - 1) & 1) ^ 1u;
-    mbar_wait(smem_u32(&row_full[sf]), (row_par >> sf) & 1u);
-    row_par ^= 1u << sf;
-    trunk_store_rows(slot0 + TR_SLOT, p.a, n, y0, tid);
-    if (p.L > 1) trunk_store_rows(slot0, p.b, n, y0, tid);
+    for (int x = 0; x < 4; ++x) mbar_wait(smem_u32(&row_full[4 * sf + x]), (ph >> sf) & 1u);
+    ph ^= 1u << sf;
+    named_bar_sync(5, NUM_THREADS);              // both warpgroups' last epilogues are in place
+    trunk_store_rows(slot_a(1), p.a, n, y0, tid);
+    if (p.L > 1) trunk_store_rows(slot_a(0), p.b, n, y0, tid);
     fence_async_smem();                          // these generic reads before the next clip's TMA and bulk-copy writes
-    named_bar_sync(1, NUM_THREADS);
+    named_bar_sync(5, NUM_THREADS);
     if (tid == 0 && k + 1 < my_clips) {
       mbar_arrive_peer(mapa_shared(smem_u32(peer_free), peer));
+      mbar_wait(smem_u32(peer_free), (uint32_t)k & 1u);   // the partner has this CTA's last rows: their sources are free
       load_x(n + G);
     }
   }

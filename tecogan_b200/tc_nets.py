@@ -113,8 +113,9 @@ def _ensure_vars_fnet():
 
 
 # A round of the one-launch trunk takes about as long whether it holds 1 or G clips, while the per-layer launches scale
-# with the batch: on an H100 SXM (700 W) the one launch was 1.20-1.32x faster at 66, 132, 198 and 264 clips (full rounds)
-# and 0.71-0.81x at 8 and 67 (1 / 8 and 1 / 2 of a round used); see tools/ab_trunk.py and DESIGN 4.1b.
+# with the batch: on an H100 80GB HBM3 (700 W limit) the one launch was 1.35-1.60x faster at 66, 132, 198 and 264 clips
+# (full rounds), 1.18x at 33 and 0.83-0.94x at 8 and 67 (1 / 8 and 1 / 2 of a round used); see tools/ab_trunk.py and
+# DESIGN 4.1b.  At three and four rounds the two paths cross near a fill of 0.75.
 LIN_TRUNK_MIN_FILL = 0.8
 
 
