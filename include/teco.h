@@ -214,6 +214,16 @@ int teco_gauss_down4_f32(const float* hr, float* lr, int32_t N, int32_t H, int32
  * out: [n, S, S, 3] fp32.  The caller keeps every crop inside its frame; 0 < n <= 65535. */
 int teco_gather_clips_u8(const uint8_t* store, const int64_t* table, int32_t n, int32_t S, float* out, void* stream);
 
+/* Inference input (reference lib/dataloader.py:38-43).  frames: device int64 [N], the device address of each of N
+ * packed [H, W, 3] RGB frames of uint8 (bits 8) or uint16 (bits 16); 0 < N <= 65535.
+ * teco_frames_to_f32:    out [N, H, W, 3] fp32 = frame / 255 (correctly rounded), the LR input.
+ * teco_gauss_blur_down4: out [N, ceil(H/4), ceil(W/4), 3] fp32 = cv2.GaussianBlur(frame, (0, 0), sigmaX=1.5)[::4, ::4]
+ *   / 255, bit for bit with cv2 4.13's float32 filter (13 taps, BORDER_REFLECT_101; DESIGN.md section 4.9), the LR
+ *   input made from HR frames.  2 <= H, W <= 65535: a 1-pixel side -> TECO_E_INVALID. */
+int teco_frames_to_f32(const int64_t* frames, int32_t bits, int32_t N, int32_t H, int32_t W, float* out, void* stream);
+int teco_gauss_blur_down4(const int64_t* frames, int32_t bits, int32_t N, int32_t H, int32_t W, float* out,
+                          void* stream);
+
 /* generic elementwise y = f(a*x + b) with f in TECO_ACT_*; n elements. preprocess/deprocess lib/ops.py:13-22 */
 int teco_affine_act_f32(const float* x, float* y, int64_t n, float a, float b, int32_t act, void* stream);
 /* dx = dy * act'(pre) expressed on the activation OUTPUT y (relu/lrelu/tanh24/sigmoid are invertible enough). */

@@ -205,18 +205,16 @@ def inference(FLAGS):
 def super_resolve_frames(eng, inference_data, image_dir, output_name, output_ext):
     """The per-frame loop of reference main.py:253-268: every frame through `eng`, the 5 warm-up frames discarded, the
     rest saved as <output_name>_<frame name>.<output_ext>."""
-    import numpy as np
     import torch
     from tecogan_b200.lib.ops import save_img
-    max_iter = len(inference_data.inputs)
+    inputs = inference_data.inputs             # [h, w, 3] float32 CUDA tensors, resident for the whole sequence
+    max_iter = len(inputs)
     srtime = 0
     print('Frame evaluation starts!!')
-    to_dev = lambda k: torch.from_numpy(np.array([inference_data.inputs[k]]).astype(np.float32)).cuda()
-    nxt = to_dev(0)
     for i in range(max_iter):
-        input_im, nxt = nxt, (to_dev(i + 1) if i + 1 < max_iter else None)
         t0 = time.time()
-        out = eng.step(input_im, next_lr=nxt)     # the next frame's flow is estimated while this frame is generated
+        # the next frame's flow is estimated while this frame is generated
+        out = eng.step(inputs[i], next_lr=inputs[i + 1] if i + 1 < max_iter else None)
         torch.cuda.synchronize()
         srtime += time.time() - t0
         if i >= 5:

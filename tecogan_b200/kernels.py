@@ -464,6 +464,44 @@ def gather_clips_u8(store, table, S):
     return out
 
 
+def _frame_table(frames):
+    """(device int64 table of frame addresses, bits, N, H, W) for a uint8 / uint16 [N, H, W, 3] CUDA tensor or a list of
+    packed [H, W, 3] CUDA tensors of one shape and dtype, which may live in different buffers."""
+    if torch.is_tensor(frames):
+        frames = list(_cc(frames)) if frames.dim() == 4 else [frames]
+    if not frames:
+        raise ValueError("no frames")
+    f0 = frames[0]
+    bits = {torch.uint8: 8, torch.uint16: 16}.get(f0.dtype)
+    if bits is None or f0.dim() != 3 or f0.shape[2] != 3:
+        raise ValueError("frames must be uint8 or uint16 [H, W, 3] RGB, got %s %s" % (f0.dtype, tuple(f0.shape)))
+    for f in frames:
+        if f.shape != f0.shape or f.dtype != f0.dtype or f.device != f0.device:
+            raise ValueError("frames of one call share shape, dtype and device: %s %s vs %s %s"
+                             % (tuple(f.shape), f.dtype, tuple(f0.shape), f0.dtype))
+    addr = torch.tensor([ptr(f).value for f in frames], dtype=torch.int64).pin_memory()
+    return addr.to(f0.device, non_blocking=True), bits, len(frames), f0.shape[0], f0.shape[1]
+
+
+def frames_to_f32(frames):
+    """uint8 / uint16 RGB frames ([N, H, W, 3] tensor or list of [H, W, 3]) -> fp32 [N, H, W, 3] = frame / 255
+    (correctly rounded: numpy's float32 division of the reference's LR input)."""
+    table, bits, N, H, W = _frame_table(frames)
+    out = torch.empty((N, H, W, 3), device=table.device, dtype=f32)
+    call("teco_frames_to_f32", ptr(table), bits, N, H, W, ptr(out, f32), stream_ptr())
+    return out
+
+
+def gauss_blur_down4(frames):
+    """uint8 / uint16 RGB frames ([N, H, W, 3] tensor or list of [H, W, 3]), H, W >= 2 -> fp32 [N, ceil(H/4), ceil(W/4), 3]
+    = cv2.GaussianBlur(frame, (0, 0), sigmaX=1.5)[::4, ::4] / 255 bit for bit: the reference's LR input made from HR
+    frames (lib/dataloader.py:38-43)."""
+    table, bits, N, H, W = _frame_table(frames)
+    out = torch.empty((N, (H + 3) // 4, (W + 3) // 4, 3), device=table.device, dtype=f32)
+    call("teco_gauss_blur_down4", ptr(table), bits, N, H, W, ptr(out, f32), stream_ptr())
+    return out
+
+
 def to_u8(x01):
     y = torch.empty(x01.shape, device=x01.device, dtype=torch.uint8)
     call("teco_to_u8", ptr(_cc(x01), f32), ptr(y, torch.uint8), x01.numel(), stream_ptr())

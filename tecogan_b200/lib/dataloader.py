@@ -17,9 +17,13 @@ from .. import kernels as K
 from .ops import preprocess
 
 
+INFERENCE_THREADS = max(1, min(8, os.cpu_count() or 1))
+
+
 def inference_data_loader(FLAGS):
     """reference lib/dataloader.py:11-50: sorted PNG list -> RGB float32 /255 frames, with the hard-coded symmetric
-    warm-up padding (list indices 5,4,3,2,1 prepended)."""
+    warm-up padding (list indices 5,4,3,2,1 prepended).  inputs[k] is an [h, w, 3] float32 CUDA tensor (read_inputs);
+    the padding entries are the same tensors as the frames they repeat."""
     filedir = FLAGS.input_dir_LR
     downSP = False
     if (FLAGS.input_dir_LR is None) or (not os.path.exists(FLAGS.input_dir_LR)):
@@ -27,26 +31,75 @@ def inference_data_loader(FLAGS):
             raise ValueError('Input directory not found')
         filedir = FLAGS.input_dir_HR
         downSP = True
-    import cv2 as cv
     names = [_ for _ in os.listdir(filedir) if _.endswith(".png")]
     names = sorted(names)
     names.sort(key=lambda f: int(''.join(list(filter(str.isdigit, f))) or -1))
     if FLAGS.input_dir_len > 0:
         names = names[:FLAGS.input_dir_len]
     image_list_LR = [os.path.join(filedir, _) for _ in names]
-
-    def preprocess_test(name):
-        im = cv.imread(name, 3).astype(np.float32)[:, :, ::-1]
-        if downSP:
-            icol_blur = cv.GaussianBlur(im, (0, 0), sigmaX=1.5)
-            im = icol_blur[::4, ::4, ::]
-        return np.ascontiguousarray(im / 255.0)
-
-    image_LR = [preprocess_test(_) for _ in image_list_LR]
+    image_LR = read_inputs(image_list_LR, downSP)
     image_list_LR = image_list_LR[5:0:-1] + image_list_LR
     image_LR = image_LR[5:0:-1] + image_LR
     Data = collections.namedtuple('Data', 'paths_LR, inputs')
     return Data(paths_LR=image_list_LR, inputs=image_LR)
+
+
+def _png_head(path):
+    """(h, w, bit depth) from the file's IHDR chunk, or None when it does not start like a PNG."""
+    from ..png import SIGNATURE
+    with open(path, 'rb') as f:
+        head = f.read(25)
+    if len(head) == 25 and head[:8] == SIGNATURE and head[12:16] == b'IHDR':
+        w, h, depth = struct.unpack('>IIB', head[16:25])
+        return int(h), int(w), int(depth)
+    return None
+
+
+def _imread_any(path):
+    """The reference's cv.imread(name, 3) = IMREAD_COLOR | IMREAD_ANYDEPTH (uint16 for 16-bit files) as contiguous RGB."""
+    import cv2 as cv
+    im = cv.imread(path, cv.IMREAD_COLOR | cv.IMREAD_ANYDEPTH)
+    if im is None:
+        raise ValueError('inference_data_loader: cannot decode ' + path)
+    return np.ascontiguousarray(im[:, :, ::-1])
+
+
+def read_inputs(paths, down, device=None, threads=INFERENCE_THREADS, window_bytes=None):
+    """The frames of `paths` as the reference's inference input (lib/dataloader.py:38-43), each an [h, w, 3] float32
+    tensor on `device`: frame / 255, or with `down` the HR frame's GaussianBlur(sigma 1.5)[::4, ::4] / 255, bit for bit.
+
+    Files are taken in windows of about `window_bytes` of decoded pixels (png.BATCH_BYTES).  A window's 8-bit PNGs are
+    decoded by png.decode_png (on the device, or by cv2 where device_pays or the device's subset says so), its other
+    files -- 16-bit PNGs, which stay uint16 as cv2 reads them, and files that are not PNGs -- by cv2 on the host and
+    uploaded; then one launch per frame size and depth converts (K.frames_to_f32) or down-samples (K.gauss_blur_down4)
+    the window, and its decoded frames are released.  So at most one window of input pixels is on the device at once;
+    the float32 frames of the whole sequence stay there, views of one tensor per launch."""
+    import torch
+    from .. import png
+    device = torch.device('cuda') if device is None else torch.device(device)
+    window_bytes = png.BATCH_BYTES if window_bytes is None else int(window_bytes)
+    heads = [_png_head(p) for p in paths]
+    cost = [hd[0] * hd[1] * 3 * (2 if hd[2] > 8 else 1) if hd else os.path.getsize(p) for p, hd in zip(paths, heads)]
+    convert = K.gauss_blur_down4 if down else K.frames_to_f32
+    out = [None] * len(paths)
+    with concurrent.futures.ThreadPoolExecutor(max_workers=max(1, int(threads))) as pool:
+        for i, j in png._windows(cost, window_bytes):
+            eight = [k for k in range(i, j) if heads[k] is not None and heads[k][2] <= 8]
+            rest = [k for k in range(i, j) if heads[k] is None or heads[k][2] > 8]
+            frames = {}
+            if eight:
+                frames.update(zip(eight, png.decode_png([paths[k] for k in eight], device, threads, window_bytes)))
+            for k, im in zip(rest, pool.map(_imread_any, [paths[k] for k in rest])):
+                frames[k] = torch.from_numpy(im).to(device)
+            groups = {}
+            for k in range(i, j):
+                groups.setdefault((tuple(frames[k].shape), frames[k].dtype), []).append(k)
+            for ks in groups.values():
+                for a in range(0, len(ks), 65535):               # frames per launch
+                    for k, im in zip(ks[a:a + 65535], convert([frames[k] for k in ks[a:a + 65535]])):
+                        out[k] = im
+            del frames
+    return out
 
 
 def frvsr_gpu_data_loader(HR_frames, FLAGS):
