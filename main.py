@@ -24,6 +24,7 @@ Differences forced by the environment, stated once:
     un-awaited subprocess.
 """
 import argparse
+import itertools
 import math
 import os
 import sys
@@ -185,45 +186,161 @@ def restore_train_state(train_state, spec):
 def inference(FLAGS):
     from tecogan_b200 import config, variables as V
     from tecogan_b200.engine import InferenceEngine
-    from tecogan_b200.lib.dataloader import inference_data_loader
+    from tecogan_b200.lib.dataloader import inference_paths, padded, stream_inputs
     if FLAGS.checkpoint is None:
         raise ValueError('The checkpoint file is needed to performing the test.')
-    inference_data = inference_data_loader(FLAGS)
-    h, w = inference_data.inputs[0].shape[:2]
-    print("input shape:", [1, h, w, 3])
-    print("output shape:", [1, h * 4, w * 4, 3])
-    config.set_precision(FLAGS.precision)
-    store = V.set_default_store(V.VariableStore(seed=FLAGS.rand_seed))
-    load_checkpoint(store, FLAGS.checkpoint, FLAGS.num_resblock)
-    eng = InferenceEngine(h, w, FLAGS.num_resblock)
-    print('Finish building the network')
-    image_dir = FLAGS.output_dir if FLAGS.output_pre == "" else os.path.join(FLAGS.output_dir, FLAGS.output_pre)
-    os.makedirs(image_dir, exist_ok=True)
-    super_resolve_frames(eng, inference_data, image_dir, FLAGS.output_name, FLAGS.output_ext)
+    paths, down = inference_paths(FLAGS)
+    frames = stream_inputs(paths, down)
+    try:
+        first = next(frames, None)
+        if first is None:
+            raise IndexError('no .png frame in the input directory')
+        h, w = first.shape[:2]
+        print("input shape:", [1, h, w, 3])
+        print("output shape:", [1, h * 4, w * 4, 3])
+        config.set_precision(FLAGS.precision)
+        store = V.set_default_store(V.VariableStore(seed=FLAGS.rand_seed))
+        load_checkpoint(store, FLAGS.checkpoint, FLAGS.num_resblock)
+        eng = InferenceEngine(h, w, FLAGS.num_resblock)
+        print('Finish building the network')
+        image_dir = FLAGS.output_dir if FLAGS.output_pre == "" else os.path.join(FLAGS.output_dir, FLAGS.output_pre)
+        os.makedirs(image_dir, exist_ok=True)
+        super_resolve_frames(eng, padded(paths), itertools.chain([first], frames), image_dir, FLAGS.output_name,
+                             FLAGS.output_ext)
+    finally:
+        frames.close()
 
 
-def super_resolve_frames(eng, inference_data, image_dir, output_name, output_ext):
+WRITE_SLOTS = 3           # output frames between the engine and the files: encoding, copied back, being written
+
+
+class FrameWriter:
+    """The write-behind half of super_resolve_frames.  put(out_u8, path) copies the engine's uint8 frame into a free slot
+    of a small ring on the current (the engine's) stream, then starts its encode -- on the slot's own stream, after an
+    event, with the slot's own encoder buffers -- or, for a format cv2 writes, the copy back to the host.  One writer
+    thread takes the slots in order, waits for each, writes its file (lib/ops.py::write_image, the rule save_img
+    follows) and hands the slot back; put() waits for a slot whose file is written.  An exception on the writer thread is
+    raised by the next put() and by close(); close() joins the thread on every exit."""
+
+    def __init__(self, h, w, device):
+        import queue
+        import threading
+        import types
+        import torch
+        self.h, self.w, self.device = h, w, torch.device(device)
+        if self.device.index is None:
+            self.device = torch.device('cuda', torch.cuda.current_device())
+        self.jobs, self.free = queue.Queue(), queue.Queue()
+        self.error = None
+        self.slots = [types.SimpleNamespace(u8=torch.empty((h, w, 3), dtype=torch.uint8, device=self.device),
+                                            stream=torch.cuda.Stream(device=self.device), encoders={}, host=None)
+                      for _ in range(WRITE_SLOTS)]
+        for s in self.slots:
+            self.free.put(s)
+        self.thread = threading.Thread(target=self._run, name='FrameWriter', daemon=True)
+        self.thread.start()
+
+    def put(self, out_u8, path):
+        import torch
+        from tecogan_b200.lib import ops
+        codec = ops.image_codec(path, self.h, self.w)
+        slot = self.free.get()
+        if isinstance(slot, BaseException):
+            raise slot
+        slot.u8.copy_(out_u8)
+        ready = torch.cuda.Event()
+        ready.record()
+        with torch.cuda.stream(slot.stream):
+            slot.stream.wait_event(ready)
+            if codec == 'cv2':
+                if slot.host is None:
+                    slot.host = torch.empty(slot.u8.shape, dtype=torch.uint8, pin_memory=True)
+                slot.host.copy_(slot.u8, non_blocking=True)
+                job = None
+            else:
+                if codec not in slot.encoders:
+                    slot.encoders[codec] = ops.device_encoder(codec)
+                job = slot.encoders[codec].launch(slot.u8, (self.h, self.w))
+        self.jobs.put((path, codec, slot, job))
+
+    def _run(self):
+        import torch
+        from tecogan_b200 import _encode
+        from tecogan_b200.lib import ops
+        try:
+            torch.cuda.set_device(self.device)
+            while True:
+                item = self.jobs.get()
+                if item is None:
+                    return
+                path, codec, slot, job = item
+                if job is None:
+                    slot.stream.synchronize()
+                    data = slot.host.numpy()
+                else:
+                    data = _encode.collect([job])[0][0]
+                ops.write_image(path, codec, data)
+                self.free.put(slot)
+        except BaseException as e:
+            self.error = e
+            self.free.put(e)                   # wakes a put() waiting for a slot
+
+    def close(self):
+        """Write what is queued (unless the writer failed), join the thread and wait for every slot's stream."""
+        self.jobs.put(None)
+        self.thread.join()
+        for s in self.slots:
+            s.stream.synchronize()
+
+
+def super_resolve_frames(eng, paths_LR, frames, image_dir, output_name, output_ext):
     """The per-frame loop of reference main.py:253-268: every frame through `eng`, the 5 warm-up frames discarded, the
-    rest saved as <output_name>_<frame name>.<output_ext>."""
+    rest saved as <output_name>_<frame name>.<output_ext>.  paths_LR is the padded file list and `frames` its [h, w, 3]
+    float32 frames in the same order (lib/dataloader.py::stream_inputs: decoded a window ahead on a reader thread).
+
+    The host does not wait for the device: each step's next frame is already on its way when the step is enqueued
+    (its flow is estimated while this frame is generated), and each output frame is copied to a FrameWriter slot,
+    encoded and written behind the steps that follow.  The files and the printed lines are those of the serial loop;
+    "total time" is the sum of the steps' device times (CUDA events around each step)."""
+    import collections
     import torch
-    from tecogan_b200.lib.ops import save_img
-    inputs = inference_data.inputs             # [h, w, 3] float32 CUDA tensors, resident for the whole sequence
-    max_iter = len(inputs)
-    srtime = 0
+    it = iter(frames)
+    max_iter = len(paths_LR)
+    srtime = 0.0
+    timing = collections.deque()           # (start, end) events of steps whose time is not yet counted
+    writer = None
     print('Frame evaluation starts!!')
-    for i in range(max_iter):
-        t0 = time.time()
-        # the next frame's flow is estimated while this frame is generated
-        out = eng.step(inputs[i], next_lr=inputs[i + 1] if i + 1 < max_iter else None)
-        torch.cuda.synchronize()
-        srtime += time.time() - t0
-        if i >= 5:
-            name, _ = os.path.splitext(os.path.basename(str(inference_data.paths_LR[i])))
-            filename = output_name + '_' + name
-            print('saving image %s' % filename)
-            save_img(os.path.join(image_dir, "%s.%s" % (filename, output_ext)), out[0])
-        else:   # First 5 is a hard-coded symmetric frame padding, ignored but time added!
-            print("Warming up %d" % (5 - i))
+    try:
+        cur = next(it, None)
+        for i in range(max_iter):
+            nxt = next(it, None) if i + 1 < max_iter else None
+            t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            t0.record()
+            eng.step(cur, next_lr=nxt)
+            t1.record()
+            timing.append((t0, t1))
+            while timing and timing[0][1].query():
+                a, b = timing.popleft()
+                srtime += a.elapsed_time(b) / 1000.0
+            cur = nxt
+            if i >= 5:
+                name, _ = os.path.splitext(os.path.basename(str(paths_LR[i])))
+                filename = output_name + '_' + name
+                print('saving image %s' % filename)
+                if writer is None:
+                    writer = FrameWriter(eng.out_u8.shape[1], eng.out_u8.shape[2], eng.device)
+                writer.put(eng.out_u8[0], os.path.join(image_dir, "%s.%s" % (filename, output_ext)))
+            else:   # First 5 is a hard-coded symmetric frame padding, ignored but time added!
+                print("Warming up %d" % (5 - i))
+        cur = nxt = None
+    finally:
+        if writer is not None:
+            writer.close()
+    if writer is not None and writer.error is not None:
+        raise writer.error
+    torch.cuda.synchronize()
+    for a, b in timing:
+        srtime += a.elapsed_time(b) / 1000.0
     print("total time " + str(srtime) + ", frame number " + str(max_iter))
 
 
@@ -256,24 +373,30 @@ def test_while_train(FLAGS, step):
     import torch
     from tecogan_b200 import config
     from tecogan_b200.engine import InferenceEngine
-    from tecogan_b200.lib.dataloader import inference_data_loader
+    from tecogan_b200.lib.dataloader import inference_paths, padded, stream_inputs
     print('[testWhileTrain] step %d:' % step)
     if not os.path.isdir(TEST_SEQUENCE_DIR):
         print('[testWhileTrain] %s not found, no test-sequence frames' % TEST_SEQUENCE_DIR)
         return
     tflags = argparse.Namespace(input_dir_LR=TEST_SEQUENCE_DIR, input_dir_HR=None, input_dir_len=10)
-    data = inference_data_loader(tflags)
-    h, w = data.inputs[0].shape[:2]
+    paths, down = inference_paths(tflags)
     image_dir = os.path.join(FLAGS.output_dir, 'train')
     os.makedirs(image_dir, exist_ok=True)
     prev_precision = config.precision()
+    frames = stream_inputs(paths, down)
+    eng = None
     try:
+        first = next(frames, None)
+        if first is None:
+            raise IndexError('no .png frame in ' + TEST_SEQUENCE_DIR)
         config.set_precision(FLAGS.precision)
-        eng = InferenceEngine(h, w, FLAGS.num_resblock)
-        super_resolve_frames(eng, data, image_dir, '%09d' % step, FLAGS.output_ext)
-        del eng
-        torch.cuda.synchronize()
+        eng = InferenceEngine(first.shape[0], first.shape[1], FLAGS.num_resblock)
+        super_resolve_frames(eng, padded(paths), itertools.chain([first], frames), image_dir, '%09d' % step,
+                             FLAGS.output_ext)
     finally:
+        frames.close()                    # the reader thread is joined, the writer was joined by super_resolve_frames
+        first = eng = None
+        torch.cuda.synchronize()
         config.set_precision(prev_precision)
 
 

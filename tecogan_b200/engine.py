@@ -230,7 +230,9 @@ class InferenceEngine:
             t.copy_(v)
         torch.cuda.synchronize()
         graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(graph, stream=self._crit):
+        # thread-local capture: the streaming command's reader and writer threads keep decoding, copying and
+        # synchronising their own streams while this thread captures (main.py::super_resolve_frames)
+        with torch.cuda.graph(graph, stream=self._crit, capture_error_mode="thread_local"):
             body()
         for t, v in zip(state, snap):
             t.copy_(v)

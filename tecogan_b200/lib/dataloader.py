@@ -20,10 +20,10 @@ from .ops import preprocess
 INFERENCE_THREADS = max(1, min(8, os.cpu_count() or 1))
 
 
-def inference_data_loader(FLAGS):
-    """reference lib/dataloader.py:11-50: sorted PNG list -> RGB float32 /255 frames, with the hard-coded symmetric
-    warm-up padding (list indices 5,4,3,2,1 prepended).  inputs[k] is an [h, w, 3] float32 CUDA tensor (read_inputs);
-    the padding entries are the same tensors as the frames they repeat."""
+def inference_paths(FLAGS):
+    """The files of the inference input (reference lib/dataloader.py:11-36) -> (paths, down): the .png files of
+    --input_dir_LR, or of --input_dir_HR when the LR directory is not given or missing (down = True: those frames are
+    down-sampled), sorted by the digits of their names and cut to --input_dir_len when it is positive."""
     filedir = FLAGS.input_dir_LR
     downSP = False
     if (FLAGS.input_dir_LR is None) or (not os.path.exists(FLAGS.input_dir_LR)):
@@ -36,12 +36,121 @@ def inference_data_loader(FLAGS):
     names.sort(key=lambda f: int(''.join(list(filter(str.isdigit, f))) or -1))
     if FLAGS.input_dir_len > 0:
         names = names[:FLAGS.input_dir_len]
-    image_list_LR = [os.path.join(filedir, _) for _ in names]
+    return [os.path.join(filedir, _) for _ in names], downSP
+
+
+def padded(seq):
+    """The reference's hard-coded symmetric warm-up padding: entries 5, 4, 3, 2, 1 prepended (fewer for a shorter
+    sequence)."""
+    return seq[5:0:-1] + seq
+
+
+def inference_data_loader(FLAGS):
+    """reference lib/dataloader.py:11-50: sorted PNG list -> RGB float32 /255 frames, with the hard-coded symmetric
+    warm-up padding (list indices 5,4,3,2,1 prepended).  inputs[k] is an [h, w, 3] float32 CUDA tensor (read_inputs);
+    the padding entries are the same tensors as the frames they repeat.  The whole sequence stays on the device;
+    stream_inputs gives the same frames holding about two windows of them at a time."""
+    image_list_LR, downSP = inference_paths(FLAGS)
     image_LR = read_inputs(image_list_LR, downSP)
-    image_list_LR = image_list_LR[5:0:-1] + image_list_LR
-    image_LR = image_LR[5:0:-1] + image_LR
     Data = collections.namedtuple('Data', 'paths_LR, inputs')
-    return Data(paths_LR=image_list_LR, inputs=image_LR)
+    return Data(paths_LR=padded(image_list_LR), inputs=padded(image_LR))
+
+
+def input_windows(paths, window_bytes=None):
+    """The [i, j) windows stream_inputs decodes `paths` in: consecutive files whose decoded input (8- or 16-bit RGB from
+    the PNG header, the file size for a file that is not a PNG) sums to at most `window_bytes` (png.BATCH_BYTES by
+    default); a single larger file is a window of its own."""
+    from .. import png
+    budget = png.BATCH_BYTES if window_bytes is None else int(window_bytes)
+    return list(png._windows([_input_cost(p) for p in paths], budget))
+
+
+def _input_cost(path):
+    hd = _png_head(path)
+    return hd[0] * hd[1] * 3 * (2 if hd[2] > 8 else 1) if hd else os.path.getsize(path)
+
+
+def stream_inputs(paths, down, window_bytes=None):
+    """Generator over the frames inference_data_loader(...).inputs holds, in the same padded order
+    (padded(paths) = paths[5:0:-1] + paths), without keeping the sequence on the device.
+
+    A reader thread decodes the files window by window (input_windows) with read_inputs(window_paths, down) on a CUDA
+    stream of its own, one window ahead of the consumer.  Each file is decoded once: the warm-up entries are the same
+    tensors as frames 1..5, which are kept until the sequence passes them again.  A window's frames reach the consumer
+    after its current stream has waited for the reader's event, and are recorded on that stream so that the allocator
+    reuses their memory only once the consumer's work on them is done.  A decoding error is raised by the generator at the
+    frame that needs the window.  Closing the generator (or an exception in it) stops and joins the reader."""
+    import queue
+    import threading
+    import torch
+    windows = input_windows(paths, window_bytes)
+    if not windows:
+        return
+    n = len(paths)
+    order = padded(list(range(n)))
+    last_use = {k: p for p, k in enumerate(order)}
+    window_of = [w for w, (i, j) in enumerate(windows) for _ in range(i, j)]
+    left = [j - i for i, j in windows]              # files of each window not yet past their last use
+    # the warm-up needs every window up to file min(5, n - 1), window w5, before its first frame, and one more may be
+    # decoded ahead; the windows before w5 return no slot, so past the warm-up the reader is one window ahead
+    w5 = window_of[order[0]]
+    slots = threading.Semaphore(w5 + 2)
+    ready, stop = queue.Queue(), threading.Event()
+    cuda = torch.cuda.is_available()
+    device = torch.cuda.current_device() if cuda else None
+
+    def read():
+        try:
+            if cuda:
+                torch.cuda.set_device(device)
+            stream = torch.cuda.Stream() if cuda else None
+            for i, j in windows:
+                slots.acquire()
+                if stop.is_set():
+                    return
+                with torch.cuda.stream(stream):
+                    frames = list(read_inputs(paths[i:j], down))
+                    done = torch.cuda.Event() if cuda else None
+                    if cuda:
+                        done.record()
+                ready.put((i, frames, done))
+                del frames
+        except BaseException as e:                  # handed to the consumer, raised there
+            ready.put(e)
+
+    reader = threading.Thread(target=read, name='stream_inputs', daemon=True)
+    reader.start()
+    have = {}
+    try:
+        for p, k in enumerate(order):
+            while k not in have:
+                got = ready.get()
+                if isinstance(got, BaseException):
+                    raise got
+                i, frames, done = got
+                if done is not None:
+                    consumer = torch.cuda.current_stream()
+                    consumer.wait_event(done)
+                    for t in frames:
+                        if torch.is_tensor(t) and t.is_cuda:
+                            t.record_stream(consumer)
+                have.update(zip(range(i, i + len(frames)), frames))
+                del got, frames
+            frame = have[k]
+            if last_use[k] == p:
+                del have[k]
+                w = window_of[k]
+                left[w] -= 1
+                if left[w] == 0 and w >= w5:
+                    slots.release()
+            yield frame
+            del frame
+    finally:
+        stop.set()
+        for _ in windows:
+            slots.release()
+        reader.join()
+        have.clear()
 
 
 def _png_head(path):

@@ -120,29 +120,53 @@ def tf_data_gaussDownby4(HRdata, sigma=1.5):
     return K.gauss_down4(HRdata)
 
 
+def image_codec(out_path, h, w, on_device=True):
+    """How save_img writes an h x w frame to out_path: 'png' or 'jpeg' (encoded on the GPU into the bytes cv2.imwrite
+    would write) for a frame on the device saved as .png, or as .jpg / .jpeg / .jpe with sides up to JPEG's 65 500 --
+    extensions in any case, as cv2 matches them -- and 'cv2' (cv2.imwrite of the host frame) for everything else."""
+    from ..jpeg import MAX_SIDE
+    path = out_path.lower()
+    if on_device:
+        if path.endswith(".png"):
+            return "png"
+        if path.endswith((".jpg", ".jpeg", ".jpe")) and max(h, w) <= MAX_SIDE:
+            return "jpeg"
+    return "cv2"
+
+
+def device_encoder(codec):
+    """A FrameEncoder of its own (workspace, device output, pinned host buffer) for 'png' or 'jpeg'."""
+    from .._encode import FrameEncoder
+    return FrameEncoder({"png": "teco_png", "jpeg": "teco_jpeg"}[codec], "encode_" + codec)
+
+
+def write_image(out_path, codec, data):
+    """Write one frame as image_codec chose: `data` is the encoded file for 'png' / 'jpeg', the [H, W, 3] uint8 RGB
+    numpy frame for 'cv2'.  A path that cannot be written is ignored, as the reference ignores imwrite's False."""
+    if codec == "cv2":
+        import cv2 as cv
+        cv.imwrite(out_path, data[:, :, ::-1])
+        return
+    try:
+        with open(out_path, "wb") as f:
+            f.write(data)
+    except OSError:
+        pass
+
+
 def save_img(out_path, img):
     """clip(img*255) -> uint8 -> BGR imwrite (reference lib/ops.py:521-523).  img: [H,W,3] CUDA or numpy in [0,1].
-    A CUDA image saved as .png, or as .jpg / .jpeg / .jpe (any case, as cv2 matches extensions; sides up to JPEG's
-    65 500), is encoded on the GPU into the bytes cv2.imwrite would write; a path that cannot be written is ignored, as
-    the reference ignores imwrite's False."""
-    import cv2 as cv
-    path = out_path.lower()
-    encode = None
-    if torch.is_tensor(img) and img.is_cuda:
-        if path.endswith(".png"):
-            from ..png import encode_png as encode
-        elif path.endswith((".jpg", ".jpeg", ".jpe")) and max(img.shape[0], img.shape[1]) <= 65500:
-            from ..jpeg import encode_jpeg as encode
-    if encode is not None:
-        data = encode(K.to_u8(img).contiguous())
-        try:
-            with open(out_path, "wb") as f:
-                f.write(data)
-        except OSError:
-            pass
-        return
-    if torch.is_tensor(img):
-        img = K.to_u8(img).cpu().numpy()
+    The file is written as image_codec and write_image say: .png and .jpg of a CUDA image are encoded on the GPU."""
+    on_device = torch.is_tensor(img) and img.is_cuda
+    codec = image_codec(out_path, img.shape[0], img.shape[1], on_device)
+    if codec == "png":
+        from ..png import encode_png
+        data = encode_png(K.to_u8(img).contiguous())
+    elif codec == "jpeg":
+        from ..jpeg import encode_jpeg
+        data = encode_jpeg(K.to_u8(img).contiguous())
+    elif torch.is_tensor(img):
+        data = K.to_u8(img).cpu().numpy()
     else:
-        img = np.clip(img * 255.0, 0, 255).astype(np.uint8)
-    cv.imwrite(out_path, img[:, :, ::-1])
+        data = np.clip(img * 255.0, 0, 255).astype(np.uint8)
+    write_image(out_path, codec, data)
