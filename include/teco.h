@@ -19,6 +19,7 @@
 #ifndef TECO_H_
 #define TECO_H_
 
+#include <stddef.h>
 #include <stdint.h>
 
 #ifdef __cplusplus
@@ -213,6 +214,18 @@ int teco_gauss_down4_f32(const float* hr, float* lr, int32_t N, int32_t H, int32
  *   out[i, y, x, c] = store[table[i][0] + y * table[i][1] + 3 * (flip ? S-1-x : x) + c] / 255   (fp32, correctly rounded)
  * out: [n, S, S, 3] fp32.  The caller keeps every crop inside its frame; 0 < n <= 65535. */
 int teco_gather_clips_u8(const uint8_t* store, const int64_t* table, int32_t n, int32_t S, float* out, void* stream);
+/* The same output from a store in host memory mapped into the device's address space: store_dev_addr is the device
+ * address teco_host_register gave for it.  Each source row is read as the 16-byte-aligned span covering its 3*S bytes,
+ * so the mapping must be readable from each row's start rounded down to 16 bytes to its end rounded up (a store in a
+ * page-aligned mapping whose size is a multiple of 16 is).  Same table, same limits, bit for bit the same out. */
+int teco_gather_clips_host_u8(uint64_t store_dev_addr, const int64_t* table, int32_t n, int32_t S, float* out,
+                              void* stream);
+/* Host memory for the host-placed frame store: teco_host_register page-locks `bytes` at `host` in place and maps them
+ * into every device's address space (cudaHostRegister Mapped | Portable); *dev is the current device's address of
+ * `host` (cudaHostGetDevicePointer).  teco_host_unregister undoes it; call it before the memory is unmapped, once no
+ * device work reads it any more.  A failure of either leaves no CUDA error behind for later calls to report. */
+int teco_host_register(void* host, size_t bytes, void** dev);
+int teco_host_unregister(void* host);
 
 /* Inference input (reference lib/dataloader.py:38-43).  frames: device int64 [N], the device address of each of N
  * packed [H, W, 3] RGB frames of uint8 (bits 8) or uint16 (bits 16); 0 < N <= 65535.

@@ -14,7 +14,8 @@ Differences forced by the environment, stated once:
     down-sampling, crops) is the same either way.  When every frame of the training (and held-out) scenes fits in device
     memory beside training, the frames are decoded once into a device-resident frame store and the clips are cut on the
     GPU from the same draws (FrameStore; select_training_input decides after the first step), so the batches are the host
-    loader's, bit for bit;
+    loader's, bit for bit; when they fit in host memory instead, the store is one page-locked host copy per node, mapped
+    into the device's address space and cut over PCIe;
   * --precision {bf16,fp32} selects wgmma tensor-core or fp32 CUDA-core convolutions for inference;
     --train_precision {fp32,bf16} does the same for training (default fp32, the reference's arithmetic);
   * under `torchrun` each rank trains on its own clip shard with one NCCL all-reduce per step;
@@ -417,29 +418,57 @@ def validation_source(FLAGS, dev):
     return lambda k: synthetic_hr_batch(FLAGS, k, 0, dev, validation=True)
 
 
-def frame_store_fits(store_bytes, free_bytes, reserved_bytes, peak_bytes, total_bytes):
-    """Whether the device frame store (lib/dataloader.py::FrameStore) fits beside training: (fits, message).
+def frame_store_fits(store_bytes, free_bytes, reserved_bytes, peak_bytes, total_bytes, host_room_bytes=None):
+    """Where the frame store (lib/dataloader.py::FrameStore) fits beside training: (placement, message).
 
     The reserve is a measured peak.  train() decides after the first training step, after the test-sequence pass (at the
     start, with --summary_dir) and after one validation pass, so `peak_bytes` (torch.cuda.max_memory_allocated) is the most
     those passes and the model have held at once.  The process can use `free_bytes` (cudaMemGetInfo) plus what PyTorch's
     allocator has reserved (`reserved_bytes`); the store fits when it leaves the peak and a margin of max(1 GiB, 5 % of the
-    device's `total_bytes`) -- allocator fragmentation, NCCL and library workspaces -- inside that."""
+    device's `total_bytes`) -- allocator fragmentation, NCCL and library workspaces -- inside that.
+
+    Without `host_room_bytes` the placement is True (the device) or False, as it always was.  With it (the bytes of host
+    memory the node can give the store, tecogan_b200/hostmem.py::host_room_bytes) the placement is 'device' when the
+    store fits on the device, else 'host' when it fits in `host_room_bytes`, else False (the host loader)."""
     margin = max(1 << 30, total_bytes // 20)
     room = free_bytes + reserved_bytes - peak_bytes - margin
     gib = lambda b: b / float(1 << 30)
     fits = store_bytes <= room
     msg = ('frame store %.2f GiB %s the %.2f GiB left beside a measured peak of %.2f GiB and a %.2f GiB margin'
            % (gib(store_bytes), 'fits in' if fits else 'does not fit in', gib(max(room, 0)), gib(peak_bytes), gib(margin)))
-    return fits, msg
+    if host_room_bytes is None:
+        return fits, msg
+    if fits:
+        return 'device', msg
+    host = store_bytes <= host_room_bytes
+    msg += ', and %s the %.2f GiB of host memory left beside the host margin' % ('fits in' if host else 'does not fit in',
+                                                                                 gib(max(host_room_bytes, 0)))
+    return ('host' if host else False), msg
+
+
+PLACEMENT_CODES = {'device': 2, 'host': 1}         # ranks agree on the smallest; 0 is the host loader
+
+
+def node_host_room(rank, world):
+    """host_room_bytes() as measured by the lowest rank on this rank's host (one host store serves all of them)."""
+    from tecogan_b200.hostmem import host_room_bytes, node_groups
+    if world <= 1:
+        return host_room_bytes()
+    import socket
+    import torch.distributed as dist
+    got = [None] * world
+    dist.all_gather_object(got, (socket.gethostname(), host_room_bytes()))
+    return got[node_groups([h for h, _ in got])[rank][0]][1]
 
 
 def select_training_input(FLAGS, Net, loader, val_hr, batch, next_step, dev, rank, world, monitor):
     """After the first training step from disk: read the training (and validation) clips from a FrameStore on the device
-    when it fits (frame_store_fits; under torchrun every rank must agree), otherwise from the host loader's thread pool.
-    Either way the batches are the same, bit for bit.  Returns (next_hr, val_hr)."""
+    when it fits, else from a FrameStore in host memory when that fits (frame_store_fits; under torchrun every rank takes
+    the smallest placement of any rank), otherwise -- or when the host memory cannot be set up (created, shared or
+    registered with the device) -- from the host loader's thread pool.  Either way the batches are the same, bit for bit.  Returns (next_hr, val_hr)."""
     import torch
     import torch.distributed as dist
+    from tecogan_b200.hostmem import HostStoreError
     from tecogan_b200.lib.dataloader import FrameStore, validation_loader
     val_loader = None
     if monitor and val_hr is not None:
@@ -451,20 +480,33 @@ def select_training_input(FLAGS, Net, loader, val_hr, batch, next_step, dev, ran
     torch.cuda.synchronize()
     store_bytes = FrameStore.estimate_bytes(loaders)
     free, total = torch.cuda.mem_get_info(dev)
-    fits, msg = frame_store_fits(store_bytes, free, torch.cuda.memory_reserved(dev), torch.cuda.max_memory_allocated(dev), total)
+    placement, msg = frame_store_fits(store_bytes, free, torch.cuda.memory_reserved(dev),
+                                      torch.cuda.max_memory_allocated(dev), total, node_host_room(rank, world))
+    code = PLACEMENT_CODES.get(placement, 0)
     if world > 1:
-        agree = torch.tensor([1 if fits else 0], dtype=torch.int32, device=dev)
+        agree = torch.tensor([code], dtype=torch.int32, device=dev)
         dist.all_reduce(agree, op=dist.ReduceOp.MIN)
-        if fits and not agree.item():
+        if agree.item() < code:
             msg += ' on this rank, not on every rank'
-        fits = bool(agree.item())
+        code = int(agree.item())
+    placement = {v: k for k, v in PLACEMENT_CODES.items()}.get(code)
+    host_loader = 'host loader (%d threads)' % loader.queue_thread
     if rank == 0:
-        print('[main] %s: training reads its clips from the %s' % (msg, 'frame store on the device' if fits else
-                                                                     'host loader (%d threads)' % loader.queue_thread))
-    if not fits:
+        print('[main] %s: training reads its clips from the %s' % (msg, {'device': 'frame store on the device',
+                                                                         'host': 'frame store in host memory'}.get(
+                                                                             placement, host_loader)))
+    store = None
+    if placement == 'host':
+        try:
+            store = FrameStore(loaders, dev, rank=rank, world=world, placement='host')
+        except HostStoreError as e:
+            if rank == 0:
+                print('[main] %s: training reads its clips from the %s' % (e, host_loader))
+    elif placement == 'device':
+        store = FrameStore(loaders, dev, rank=rank, world=world)
+    if store is None:
         clip_iter = loader.batches(start_step=next_step)
         return (lambda gstep: next(clip_iter).to(dev, non_blocking=True)), val_hr
-    store = FrameStore(loaders, dev, rank=rank, world=world)
     if rank == 0:
         print('[main] frame store: %d frames, %.2f GiB, built in %.1f s' % (len(store.paths), store.nbytes / float(1 << 30),
                                                                            store.build_seconds))

@@ -69,6 +69,9 @@ SIGNATURES = {
     "teco_depth_to_space4_f32": [_P, _P, _I32, _I32, _I32, _I32, _I32, _I32, _P],
     "teco_gauss_down4_f32": [_P, _P, _I32, _I32, _I32, _I32, _P],
     "teco_gather_clips_u8": [_P, _P, _I32, _I32, _P, _P],
+    "teco_gather_clips_host_u8": [C.c_uint64, _P, _I32, _I32, _P, _P],
+    "teco_host_register": [_P, C.c_size_t, C.POINTER(C.c_void_p)],
+    "teco_host_unregister": [_P],
     "teco_frames_to_f32": [_P, _I32, _I32, _I32, _I32, _P, _P],
     "teco_gauss_blur_down4": [_P, _I32, _I32, _I32, _I32, _P, _P],
     "teco_affine_act_f32": [_P, _P, _I64, _F, _F, _I32, _P],

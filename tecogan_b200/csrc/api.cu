@@ -77,4 +77,38 @@ int64_t teco_crc32c(const void* data, int64_t n, int64_t crc_in) {
   return (int64_t)(c ^ 0xFFFFFFFFu);
 }
 
+// Host memory for the frame store's host placement (tecogan_b200/lib/dataloader.py::FrameStore): page-locked in
+// place, mapped into every device's address space.
+// A failed call also leaves its error as the runtime's last error, which the next kernel launch's check would report
+// as its own; these failures are expected (a locked-memory limit, a range registered twice) and the caller goes on
+// without the host store, so each failure path clears it with cudaGetLastError.
+int teco_host_register(void* host, size_t bytes, void** dev) {
+  TECO_CHECK_ARG(host && dev && bytes > 0, "teco_host_register: NULL pointer or zero bytes");
+  cudaError_t e = cudaHostRegister(host, bytes, cudaHostRegisterMapped | cudaHostRegisterPortable);
+  if (e != cudaSuccess) {
+    cudaGetLastError();
+    teco_set_error("teco_host_register: cudaHostRegister failed: %s", cudaGetErrorString(e));
+    return TECO_E_CUDA;
+  }
+  e = cudaHostGetDevicePointer(dev, host, 0);
+  if (e != cudaSuccess) {
+    cudaHostUnregister(host);
+    cudaGetLastError();
+    teco_set_error("teco_host_register: cudaHostGetDevicePointer failed: %s", cudaGetErrorString(e));
+    return TECO_E_CUDA;
+  }
+  return TECO_OK;
+}
+
+int teco_host_unregister(void* host) {
+  TECO_CHECK_ARG(host, "teco_host_unregister: NULL pointer");
+  const cudaError_t e = cudaHostUnregister(host);
+  if (e != cudaSuccess) {
+    cudaGetLastError();
+    teco_set_error("teco_host_unregister: cudaHostUnregister failed: %s", cudaGetErrorString(e));
+    return TECO_E_CUDA;
+  }
+  return TECO_OK;
+}
+
 }  // extern "C"

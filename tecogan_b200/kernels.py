@@ -464,6 +464,16 @@ def gather_clips_u8(store, table, S):
     return out
 
 
+def gather_clips_host_u8(store_dev_addr, table, S):
+    """gather_clips_u8 from a uint8 store in mapped host memory: `store_dev_addr` is the device address
+    teco_host_register gave for it (tecogan_b200/hostmem.py::HostMapping); the output lands on the table's device."""
+    n = table.shape[0]
+    out = torch.empty((n, S, S, 3), device=table.device, dtype=f32)
+    call("teco_gather_clips_host_u8", int(store_dev_addr or 0), ptr(_cc(table), torch.int64), n, S, ptr(out, f32),
+         stream_ptr())
+    return out
+
+
 def _frame_table(frames):
     """(device int64 table of frame addresses, bits, N, H, W) for a uint8 / uint16 [N, H, W, 3] CUDA tensor or a list of
     packed [H, W, 3] CUDA tensors of one shape and dtype, which may live in different buffers."""

@@ -4,9 +4,11 @@ HR training clips (`HRClipLoader`) that follows `loadHR` + `tf.train.shuffle_bat
 directory layout, frame windows, moving-first-frame / random-crop / flip augmentation, a thread pool instead of TF queue
 runners.  The validation split (lib/dataloader.py:287-296) is a second `HRClipLoader` over the held-out scenes
 (`validation_loader`); it feeds the val_* summaries of main.py --mode train --summary_dir.  `FrameStore` is the device
-half: the frames of those scenes decoded once into device memory, the same batches cut there by teco_gather_clips_u8."""
+half: the frames of those scenes decoded once into device memory (or into host memory mapped into the device's address
+space), the same batches cut there by teco_gather_clips_u8 (teco_gather_clips_host_u8)."""
 import collections
 import concurrent.futures
+import itertools
 import os
 import struct
 import time
@@ -442,11 +444,17 @@ class FrameStore:
     whose backend can broadcast `device` tensors: NCCL under torchrun) rank r decodes the r-th contiguous share of the
     frames and broadcasts it, so every rank holds the whole store after 1/world of the decoding.
 
+    placement='host' keeps the frames in host memory instead (tecogan_b200/hostmem.py::shared_mapping): one memfd mapping
+    per node, shared by the node's ranks, page-locked and mapped into the device's address space.  Each rank of a node
+    decodes its contiguous share of the frames on its own device, `chunk_bytes` at a time, and copies each chunk into the
+    mapping; a barrier follows.  The batches are cut over PCIe by teco_gather_clips_host_u8.  close() releases the
+    mapping (unregister, then unmap).
+
     batch(step) is HRClipLoader.batch(step) of the first loader, uploaded to `device`, bit for bit: the same draws
     (HRClipLoader.draw: permutation, epochs, rank shard, salt) and the same pixels, cut by teco_gather_clips_u8.
     view(loader) is the same store serving another of the loaders it was built from (the validation scenes)."""
 
-    def __init__(self, loaders, device, rank=0, world=1, queue_thread=None, chunk_bytes=256 << 20):
+    def __init__(self, loaders, device, rank=0, world=1, queue_thread=None, chunk_bytes=256 << 20, placement='device'):
         import torch
         loaders = list(loaders)
         self.loader, self.device = loaders[0], torch.device(device)
@@ -469,9 +477,16 @@ class FrameStore:
         self.offsets = np.concatenate([[0], np.cumsum(nbytes)]).astype(np.int64)
         self.nbytes = int(self.offsets[-1])
         t0 = time.time()
+        if placement not in ('device', 'host'):
+            raise ValueError("FrameStore: placement is 'device' or 'host', got %r" % (placement,))
+        self.placement = placement
+        threads = max(1, int(self.loader.queue_thread if queue_thread is None else queue_thread))
+        if placement == 'host':
+            self._build_host(paths, rank, world, threads, chunk_bytes)
+            self.build_seconds = time.time() - t0
+            return
         self.buf = torch.empty(self.nbytes, dtype=torch.uint8, device=self.device)
         shares = frame_shares(len(paths), world)
-        threads = max(1, int(self.loader.queue_thread if queue_thread is None else queue_thread))
         self._decode(paths, *shares[rank], threads, chunk_bytes)
         if world > 1:
             import torch.distributed as dist
@@ -495,10 +510,46 @@ class FrameStore:
                     total += h * w * 3
         return total
 
-    def _decode(self, paths, a, b, threads, chunk_bytes):
-        """Frames a..b-1 into self.buf: host threads read the files and pack their compressed streams, the device
-        decodes them in chunks of about chunk_bytes (tecogan_b200.png.decode_png_into); a file the device does not take
-        is decoded on the host by the loader and copied into its slot."""
+    def _build_host(self, paths, rank, world, threads, chunk_bytes):
+        """The host placement: the node's shared mapping, this rank's share of it decoded on the device chunk by chunk
+        and copied in, then a barrier."""
+        import torch
+        from ..hostmem import shared_mapping
+        with torch.cuda.device(self.device):         # registered on, and synchronised on close with, this device
+            self._host, node = shared_mapping(self.nbytes, rank, world)
+        try:
+            self.buf = torch.from_numpy(self._host.array())
+            a, b = frame_shares(len(paths), len(node))[node.index(rank)]
+            while a < b:
+                end = a + 1
+                while end < b and self.offsets[end + 1] - self.offsets[a] <= chunk_bytes:
+                    end += 1
+                lo, hi = int(self.offsets[a]), int(self.offsets[end])
+                stage = torch.empty(hi - lo, dtype=torch.uint8, device=self.device)
+                self._decode(paths, a, end, threads, chunk_bytes, stage, self.offsets[a:end] - lo)
+                self.buf[lo:hi].copy_(stage)
+                a = end
+            torch.cuda.synchronize(self.device)
+            if world > 1:
+                import torch.distributed as dist
+                dist.barrier()
+        except BaseException:
+            self.close()
+            raise
+
+    def close(self):
+        """Releases a host placement's mapping: waits for the store's device, unregisters the mapping, then unmaps it
+        (errors are raised).  The store and its views must not be used afterwards.  A device placement's memory is freed
+        with the store."""
+        host = self.__dict__.pop('_host', None)
+        if host is not None:
+            self.buf = None
+            host.close()
+
+    def _decode(self, paths, a, b, threads, chunk_bytes, buf=None, offsets=None):
+        """Frames a..b-1 into self.buf (or into `buf` at `offsets`): host threads read the files and pack their
+        compressed streams, the device decodes them in chunks of about chunk_bytes (tecogan_b200.png.decode_png_into);
+        a file the device does not take is decoded on the host by the loader and copied into its slot."""
         from ..png import decode_png_into
         if b <= a:
             return
@@ -510,8 +561,8 @@ class FrameStore:
             if im.shape[:2] != (h, w):
                 raise ValueError('FrameStore: %s decodes to %dx%d, its header says %dx%d' % (path, im.shape[0], im.shape[1], h, w))
             return im
-        decode_png_into(paths[a:b], self.buf, self.offsets[a:b], self.sizes[a:b], threads=threads,
-                        batch_bytes=chunk_bytes, host_decode=host)
+        decode_png_into(paths[a:b], self.buf if buf is None else buf, self.offsets[a:b] if offsets is None else offsets,
+                        self.sizes[a:b], threads=threads, batch_bytes=chunk_bytes, host_decode=host)
 
     def view(self, loader):
         """This store serving `loader`, one of the loaders it was built from."""
@@ -546,7 +597,10 @@ class FrameStore:
         import torch
         L = self.loader
         t = torch.from_numpy(tbl).pin_memory().to(self.device, non_blocking=True)
-        out = K.gather_clips_u8(self.buf, t, L.tar_size)
+        if self.placement == 'host':
+            out = K.gather_clips_host_u8(self._host.dev_addr, t, L.tar_size)
+        else:
+            out = K.gather_clips_u8(self.buf, t, L.tar_size)
         return out.reshape(L.F.batch_size, L.F.RNN_N, L.tar_size, L.tar_size, 3)
 
     def batch(self, step):
@@ -555,14 +609,37 @@ class FrameStore:
 
     def batches(self, start_step=0, prefetch=4):
         """Endless iterator over batch(start_step), batch(start_step + 1), ...; the draws of the next `prefetch` steps are
-        made on a worker thread while the device works."""
+        made on a worker thread while the device works.  In host placement the gather of step k + 1 is enqueued on a
+        stream of its own as soon as batch k is handed out, so its PCIe reads overlap the caller's work on batch k; the
+        caller's stream waits for each batch, and record_stream keeps its memory from being reused while it is held."""
+        import torch
         with concurrent.futures.ThreadPoolExecutor(max_workers=1) as pool:
             pending = collections.deque(pool.submit(self.table, s) for s in range(start_step, start_step + prefetch))
             step = start_step
-            while True:
+            if self.placement != 'host':
+                while True:
+                    tbl = pending.popleft().result()
+                    pending.append(pool.submit(self.table, step + prefetch))
+                    yield self._gather(tbl)
+                    step += 1
+            side, drawn = torch.cuda.Stream(self.device), itertools.count(start_step + prefetch)
+
+            def launch():
                 tbl = pending.popleft().result()
-                pending.append(pool.submit(self.table, step + prefetch))
-                yield self._gather(tbl)
+                pending.append(pool.submit(self.table, next(drawn)))
+                with torch.cuda.stream(side):
+                    out = self._gather(tbl)
+                    done = torch.cuda.Event()
+                    done.record(side)
+                return out, done
+            ahead = launch()
+            while True:
+                out, done = ahead
+                consumer = torch.cuda.current_stream(self.device)
+                consumer.wait_event(done)
+                out.record_stream(consumer)
+                ahead = launch()
+                yield out
                 step += 1
 
     def checksum(self):
