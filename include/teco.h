@@ -236,6 +236,13 @@ int teco_host_unregister(void* host);
 int teco_frames_to_f32(const int64_t* frames, int32_t bits, int32_t N, int32_t H, int32_t W, float* out, void* stream);
 int teco_gauss_blur_down4(const int64_t* frames, int32_t bits, int32_t N, int32_t H, int32_t W, float* out,
                           void* stream);
+/* Training-data preparation (reference dataPrepare.py, lib/data/video.py:168-173).  frames: device int64 [N], the device
+ * address of each of N packed [H, W, 3] uint8 frames; 0 < N <= 65535, 2 <= H, W <= 65535 (else TECO_E_INVALID).
+ * teco_area_half_u8: out [N, cvRound(H/2), cvRound(W/2), 3] uint8 = cv2.resize(frame, (0, 0), fx=0.5, fy=0.5,
+ *   interpolation=INTER_AREA), bit for bit with cv2 4.13 (halves of the sizes round to even; DESIGN.md section 4.10);
+ *   swap_rb != 0 stores the channels reversed (BGR in, RGB out). */
+int teco_area_half_u8(const int64_t* frames, int32_t N, int32_t H, int32_t W, uint8_t* out, int32_t swap_rb,
+                      void* stream);
 
 /* generic elementwise y = f(a*x + b) with f in TECO_ACT_*; n elements. preprocess/deprocess lib/ops.py:13-22 */
 int teco_affine_act_f32(const float* x, float* y, int64_t n, float a, float b, int32_t act, void* stream);

@@ -212,88 +212,6 @@ def inference(FLAGS):
         frames.close()
 
 
-WRITE_SLOTS = 3           # output frames between the engine and the files: encoding, copied back, being written
-
-
-class FrameWriter:
-    """The write-behind half of super_resolve_frames.  put(out_u8, path) copies the engine's uint8 frame into a free slot
-    of a small ring on the current (the engine's) stream, then starts its encode -- on the slot's own stream, after an
-    event, with the slot's own encoder buffers -- or, for a format cv2 writes, the copy back to the host.  One writer
-    thread takes the slots in order, waits for each, writes its file (lib/ops.py::write_image, the rule save_img
-    follows) and hands the slot back; put() waits for a slot whose file is written.  An exception on the writer thread is
-    raised by the next put() and by close(); close() joins the thread on every exit."""
-
-    def __init__(self, h, w, device):
-        import queue
-        import threading
-        import types
-        import torch
-        self.h, self.w, self.device = h, w, torch.device(device)
-        if self.device.index is None:
-            self.device = torch.device('cuda', torch.cuda.current_device())
-        self.jobs, self.free = queue.Queue(), queue.Queue()
-        self.error = None
-        self.slots = [types.SimpleNamespace(u8=torch.empty((h, w, 3), dtype=torch.uint8, device=self.device),
-                                            stream=torch.cuda.Stream(device=self.device), encoders={}, host=None)
-                      for _ in range(WRITE_SLOTS)]
-        for s in self.slots:
-            self.free.put(s)
-        self.thread = threading.Thread(target=self._run, name='FrameWriter', daemon=True)
-        self.thread.start()
-
-    def put(self, out_u8, path):
-        import torch
-        from tecogan_b200.lib import ops
-        codec = ops.image_codec(path, self.h, self.w)
-        slot = self.free.get()
-        if isinstance(slot, BaseException):
-            raise slot
-        slot.u8.copy_(out_u8)
-        ready = torch.cuda.Event()
-        ready.record()
-        with torch.cuda.stream(slot.stream):
-            slot.stream.wait_event(ready)
-            if codec == 'cv2':
-                if slot.host is None:
-                    slot.host = torch.empty(slot.u8.shape, dtype=torch.uint8, pin_memory=True)
-                slot.host.copy_(slot.u8, non_blocking=True)
-                job = None
-            else:
-                if codec not in slot.encoders:
-                    slot.encoders[codec] = ops.device_encoder(codec)
-                job = slot.encoders[codec].launch(slot.u8, (self.h, self.w))
-        self.jobs.put((path, codec, slot, job))
-
-    def _run(self):
-        import torch
-        from tecogan_b200 import _encode
-        from tecogan_b200.lib import ops
-        try:
-            torch.cuda.set_device(self.device)
-            while True:
-                item = self.jobs.get()
-                if item is None:
-                    return
-                path, codec, slot, job = item
-                if job is None:
-                    slot.stream.synchronize()
-                    data = slot.host.numpy()
-                else:
-                    data = _encode.collect([job])[0][0]
-                ops.write_image(path, codec, data)
-                self.free.put(slot)
-        except BaseException as e:
-            self.error = e
-            self.free.put(e)                   # wakes a put() waiting for a slot
-
-    def close(self):
-        """Write what is queued (unless the writer failed), join the thread and wait for every slot's stream."""
-        self.jobs.put(None)
-        self.thread.join()
-        for s in self.slots:
-            s.stream.synchronize()
-
-
 def super_resolve_frames(eng, paths_LR, frames, image_dir, output_name, output_ext):
     """The per-frame loop of reference main.py:253-268: every frame through `eng`, the 5 warm-up frames discarded, the
     rest saved as <output_name>_<frame name>.<output_ext>.  paths_LR is the padded file list and `frames` its [h, w, 3]
@@ -305,6 +223,7 @@ def super_resolve_frames(eng, paths_LR, frames, image_dir, output_name, output_e
     "total time" is the sum of the steps' device times (CUDA events around each step)."""
     import collections
     import torch
+    from tecogan_b200.lib.writer import FrameWriter
     it = iter(frames)
     max_iter = len(paths_LR)
     srtime = 0.0

@@ -7,7 +7,8 @@ python3 runGan.py 4   # train FRVSR    (reference runGan.py:247-296)
 python3 runGan.py 2   # PSNR / SSIM, and LPIPS / tLP100 when the AlexNet and LPIPS v0.1 weights are found, of ./results/<scene>
                       # against ./HR/<scene> on the GPU (reference runGan.py:92-105; the reference's tOF column is outside
                       # the hot path, DESIGN.md section 6)
-Case 0 (download, needs network) is outside the hot path and prints why it is not run.
+Case 0 (download, needs network) is not run: it prints why.  The training scenes of cases 3 and 4 are made from local
+videos by dataPrepare.py (the reference's dataPrepare.py without its download).
 Extra arguments after the case number are appended to the main.py command line (e.g. --max_iter 100).
 '''
 import datetime
@@ -46,6 +47,7 @@ TrainingDataPath = os.environ.get("TECO_TRAINING_DATA", "/mnt/netdisk/video_data
 
 if runcase == 0:
     print("case 0 downloads models/data with wget (reference runGan.py:41-65); there is no network here.")
+    print("To make the training scenes from videos already on disk, run dataPrepare.py --disk_path <dir of <id>.<ext>>.")
 elif runcase == 1:   # inference a trained model
     dirstr = './results/'
     testpre = ['calendar']

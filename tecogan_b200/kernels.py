@@ -512,6 +512,32 @@ def gauss_blur_down4(frames):
     return out
 
 
+def area_half_size(n):
+    """cv2's output side for fx or fy = 0.5: cvRound(n * 0.5), halves to even (721 -> 360, 3 -> 2)."""
+    return int(round(n * 0.5))
+
+
+def area_half(frames, swap_rb=False, out=None):
+    """uint8 [H, W, 3] frames ([N, H, W, 3] tensor or list of [H, W, 3], which may live in different buffers),
+    2 <= H, W <= 65535 -> uint8 [N, cvRound(H/2), cvRound(W/2), 3] = cv2.resize(frame, (0, 0), fx=0.5, fy=0.5,
+    interpolation=cv2.INTER_AREA) bit for bit: the reference's training-frame down-sample (lib/data/video.py:168-173).
+    swap_rb reverses the channels on the store (BGR frames in, RGB out).  `out` may be given as a contiguous uint8 CUDA
+    tensor of that shape on the frames' device."""
+    table, bits, N, H, W = _frame_table(frames)
+    if bits != 8:
+        raise ValueError("area_half: frames must be uint8, got uint%d" % bits)
+    if not (2 <= H <= 65535 and 2 <= W <= 65535):
+        raise ValueError("area_half: frames need 2 <= H, W <= 65535, got %dx%d" % (H, W))
+    shape = (N, area_half_size(H), area_half_size(W), 3)
+    if out is None:
+        out = torch.empty(shape, device=table.device, dtype=torch.uint8)
+    elif tuple(out.shape) != shape or out.device != table.device:
+        raise ValueError("area_half: out must be %s on %s, got %s on %s" % (shape, table.device, tuple(out.shape),
+                                                                            out.device))
+    call("teco_area_half_u8", ptr(table), N, H, W, ptr(out, torch.uint8), int(bool(swap_rb)), stream_ptr())
+    return out
+
+
 def to_u8(x01):
     y = torch.empty(x01.shape, device=x01.device, dtype=torch.uint8)
     call("teco_to_u8", ptr(_cc(x01), f32), ptr(y, torch.uint8), x01.numel(), stream_ptr())
