@@ -25,7 +25,7 @@ H100_SMS = 132
 MAX_SLOTS = 4 * H100_SMS
 # conv3x3_trunk_cluster_kernel: clusters of two CTAs, one CTA per SM, so at most SMs / 2 clusters are resident at once
 MAX_CLUSTERS = H100_SMS // 2
-TR_WSLOTS = 8                                      # conv_tc.cu TR_WSLOTS: weight ring depth in 3x3 taps
+TR_WSLOTS = 9                                      # conv_tc.cu trunk kernel's weight ring: slot t holds tap t of a layer
 WG_ROWS, WG_COLS = 8, 16                           # conv_wgrad_tc.cu WG_ROWS, WG_COLS: weight-gradient tile
 ACT_NAMES = ("none", "relu", "lrelu", "tanh24", "sigmoid")
 
@@ -90,12 +90,17 @@ def features(mode, n, h, w, cin, cout, act, bias=True, res="", y=True, f32c=0, r
 
 def lin_features(n, h, plan):
     """teco_conv3x3_lin_tc on n 32x32 images (h is 32): conv3x3_trunk_cluster_kernel, one cluster per image at a time
-    over a persistent grid of clusters, every layer's nine taps streamed through a TR_WSLOTS-deep weight ring."""
-    out = {"lin L=%d" % len(plan), "lin last output in buffer %d" % plan[-1][1]}
-    if 9 * len(plan) > 2 * TR_WSLOTS:
-        out.add("lin weight ring wraps")          # the ring's barriers run through both phase parities
+    over a persistent grid of clusters, every layer's nine taps streamed through a TR_WSLOTS-slot weight ring, tap t in
+    slot t.  Layer l of a cluster's clip k waits on its slots at parity (k L + l) & 1, so with an even L every clip
+    starts on parity 0 and with an odd L the clips alternate."""
+    L = len(plan)
+    out = {"lin L=%d" % L, "lin last output in buffer %d" % plan[-1][1]}
+    if 9 * L > TR_WSLOTS:
+        out.add("lin weight ring wraps")          # every slot is refilled for the next layer, at the other parity
     if n > MAX_CLUSTERS:
         out.add("lin clips>clusters")             # a cluster runs several clips: x_in reloaded, partner handshake
+    if n > 2 * MAX_CLUSTERS:
+        out.add("lin three clips per cluster, L %s" % ("even" if L % 2 == 0 else "odd"))
     for i, o, r, act in plan:
         if r >= 0:
             out.add("lin res=inplace on buffer %d" % r)

@@ -110,9 +110,12 @@ LIN_CASES = {
     "res_block": (2, 32, [(0, 1, -1, RELU), (1, 2, -1, RELU), (2, 1, 1, NONE)]),
     "images_gt_sms": (150, 32, [(0, 1, -1, RELU), (1, 2, -1, RELU), (2, 1, 1, NONE), (1, 2, -1, RELU), (2, 1, 1, NONE)]),
     "nine_layers_weight_ring": (7, 32, [(0, 1, -1, RELU)] + [(1, 2, -1, RELU), (2, 1, 1, NONE)] * 4),
+    # even L: a cluster's later clips start on the same ring parity as its first (odd L above alternates it)
+    "three_clips_even_layers": (140, 32, [(0, 1, -1, RELU), (1, 2, -1, RELU), (2, 1, 1, NONE), (1, 2, -1, RELU)]),
 }
 LIN_REQUIRED = {"lin L=1", "lin L=9", "lin weight ring wraps", "lin clips>clusters", "lin res=inplace on buffer 1",
-                "lin res=inplace on buffer 2", "lin last output in buffer 2", "lin act=none", "lin act=relu", "lin act=lrelu"}
+                "lin res=inplace on buffer 2", "lin last output in buffer 2", "lin act=none", "lin act=relu", "lin act=lrelu",
+                "lin three clips per cluster, L odd", "lin three clips per cluster, L even"}
 
 # teco_conv3x3_wgrad_tc: the shapes of test_gpu_kernels.py::test_conv3x3_wgrad_tc_matches_autograd_on_bf16_operands
 WGRAD_CASES = [(1, 8, 16, 64, 64), (4, 32, 32, 64, 64), (2, 19, 21, 51, 64), (3, 16, 24, 128, 32), (2, 32, 32, 32, 256),
@@ -127,7 +130,8 @@ def _case_features(c):
 def test_case_tables_reach_every_required_path():
     """Host restatement of the dispatch (tests/conv_paths.py): each case reaches the paths it claims, and together the
     tables reach every kernel instance of teco_conv3x3_tc with each epilogue feature listed in REQUIRED, the chain's
-    weight-ring wrap, in-place residuals on either buffer and more clips than clusters (on plans its entry takes), and the
+    weight-ring wrap, in-place residuals on either buffer, more clips than clusters and clusters running three clips at
+    an odd and an even layer count (on plans its entry takes), and the
     weight gradient's ragged and narrow shapes."""
     from tecogan_b200 import kernels as K
     seen = set()
