@@ -275,6 +275,59 @@ int teco_bn_train_bwd_f32(const float* x, const float* y, const float* dy, const
                           float* dbeta, int64_t npix, int32_t C, float eps, int32_t lrelu02, void* stream);
 
 /* ---------------------------------------------------------------------------------------
+ * Fixed-order (deterministic) training reductions (main.py --deterministic; DESIGN.md section 4.3).
+ * Each *_det call computes what the entry point of the same name without _det computes, but every floating-point sum
+ * runs in an order fixed by the call's shapes alone (never by the device, occupancy, stream or timing): reductions split
+ * into a partition declared from the shapes, each part stores its partial into the caller's workspace `ws`, and one
+ * pass sums the partials in part order.  `ws` is caller-owned, 16-byte aligned and at least the bytes the matching
+ * *_plan_bytes call (host only, no device) writes to *ws_bytes_host; a smaller or NULL workspace -> TECO_E_INVALID.
+ * accumulate != 0 adds the fixed-order sum to the output's previous value (out + sum), else stores it.
+ *  teco_conv3x3_wgrad_tc_det: as teco_conv3x3_wgrad_tc; CTA x runs a fixed run of 8x16 tiles into one accumulator set and
+ *    stores it to ws[x][3,3,cin,cout] (fp32); dw = ws[0] + ws[1] + ... in split order.
+ *  teco_conv2d_wgrad_f32_det: as teco_conv2d_wgrad_f32 (db may be NULL); pixel splits stored to ws, then db's blocks.
+ *  teco_bias_grad_f32_det, teco_bn_train_f32_det, teco_bn_train_bwd_f32_det, teco_loss_*_f32_det: per-block partials,
+ *    then one fixed-order sum.  The loss workspace of teco_loss_det_plan_bytes serves all four losses for (npix, C)
+ *    (teco_loss_gan_f32_det: npix = n, C = 1).
+ *  teco_warp_bwd_f32_det: dimg is STORED (not added to): dimg[q] = sum of q's contributions in ascending source pixel
+ *    order (a counting sort of the contributions in ws); dflow as teco_warp_bwd_f32.  4 N H W < 2^31.
+ *  teco_resize_bilinear_bwd_f32_det: a gather, no workspace: input pixel (y, x) sums the outputs that read it in
+ *    ascending output row, column, then corner order.
+ *  teco_sum_ranks_f32: dst[e] = src[0][e] + src[1][e] + ... + src[R-1][e] in rank order (src: [R, n] fp32, gathered
+ *    per-rank buckets), so every rank that runs it on the same gather holds the same bits.
+ * ------------------------------------------------------------------------------------- */
+int teco_conv3x3_wgrad_tc_det_plan_bytes(int32_t N, int32_t H, int32_t W, int32_t cin, int32_t cout, int64_t* ws_bytes_host);
+int teco_conv3x3_wgrad_tc_det(int32_t N, int32_t H, int32_t W, int32_t cin_pad, int32_t cout_pad, int32_t cin, int32_t cout,
+                              const void* x, const void* dz, float* dw, int32_t accumulate, void* ws, int64_t ws_bytes,
+                              void* stream);
+int teco_conv2d_wgrad_f32_det_plan_bytes(const teco_conv_desc* d, int32_t with_bias, int64_t* ws_bytes_host);
+int teco_conv2d_wgrad_f32_det(const teco_conv_desc* d, const float* x, const float* dy, float* dw, float* db,
+                              int32_t accumulate, void* ws, int64_t ws_bytes, void* stream);
+int teco_bias_grad_f32_det_plan_bytes(int64_t npix, int32_t C, int64_t* ws_bytes_host);
+int teco_bias_grad_f32_det(const float* dy, float* db, int64_t npix, int32_t C, int32_t cpitch, int32_t accumulate,
+                           void* ws, int64_t ws_bytes, void* stream);
+int teco_bn_det_plan_bytes(int64_t npix, int32_t C, int64_t* ws_bytes_host);
+int teco_bn_train_f32_det(const float* x, const float* beta, float* y, float* stats, int64_t npix, int32_t C, float eps,
+                          int32_t lrelu02, void* ws, int64_t ws_bytes, void* stream);
+int teco_bn_train_bwd_f32_det(const float* x, const float* y, const float* dy, const float* stats, float* dx, float* dbeta,
+                              int64_t npix, int32_t C, float eps, int32_t lrelu02, void* ws, int64_t ws_bytes, void* stream);
+int teco_loss_det_plan_bytes(int64_t npix, int32_t C, int64_t* ws_bytes_host);
+int teco_loss_l2_f32_det(const float* a, const float* b, float* out, float* da, int64_t npix, int32_t C, float gscale,
+                         void* ws, int64_t ws_bytes, void* stream);
+int teco_loss_l1_f32_det(const float* a, const float* b, float* out, float* da, float* db, int64_t npix, int32_t C,
+                         int32_t per_pixel, float gscale, void* ws, int64_t ws_bytes, void* stream);
+int teco_loss_cosine_f32_det(const float* f, const float* g, float* out, float* df, int64_t npix, int32_t C, float gscale,
+                             void* ws, int64_t ws_bytes, void* stream);
+int teco_loss_gan_f32_det(const float* d_fake, const float* d_real, float* out, float* g_adv, float* g_dis_f,
+                          float* g_dis_r, int64_t n, float eps, float s_adv, float s_dis, void* ws, int64_t ws_bytes,
+                          void* stream);
+int teco_warp_bwd_f32_det_plan_bytes(int32_t N, int32_t H, int32_t W, int64_t* ws_bytes_host);
+int teco_warp_bwd_f32_det(const float* img, const float* flow, const float* dout, float* dimg, float* dflow, int32_t N,
+                          int32_t H, int32_t W, int32_t C, void* ws, int64_t ws_bytes, void* stream);
+int teco_resize_bilinear_bwd_f32_det(const float* dy, float* dx, int32_t N, int32_t h, int32_t w, int32_t C, int32_t oh,
+                                     int32_t ow, void* stream);
+int teco_sum_ranks_f32(const float* src, int32_t R, int64_t n, float* dst, void* stream);
+
+/* ---------------------------------------------------------------------------------------
  * Fused loss reductions (lib/Teco.py:316-413).  Each writes its scalar (fp32) to out[0] and, when the
  * gradient pointer is non-NULL, d(loss*gscale)/d(a) elementwise (same shape as a).
  * ------------------------------------------------------------------------------------- */

@@ -18,6 +18,10 @@ Differences forced by the environment, stated once:
     into the device's address space and cut over PCIe;
   * --precision {bf16,fp32} selects wgmma tensor-core or fp32 CUDA-core convolutions for inference;
     --train_precision {fp32,bf16} does the same for training (default fp32, the reference's arithmetic);
+  * --deterministic (opt-in extension: FLAGS has no `deterministic` attribute unless it is given) trains on fixed-order
+    reductions: every gradient, batch-norm and loss sum, and the gradient sum over ranks, adds in an order set by the
+    shapes alone, so two runs with the same seed, data, build, GPU model and rank count give bit-identical variables,
+    Adam moments, losses and outputs (the default atomic kernels agree only to rounding);
   * under `torchrun` each rank trains on its own clip shard with one NCCL all-reduce per step;
   * monitoring (--summary_dir: TensorBoard scalars, logfile.txt, validation scalars, test-sequence frames at every
     checkpoint) runs on rank 0 only, in process: the held-out scenes end_dir+1..end_dir_val are optional (validation is
@@ -52,6 +56,9 @@ FLAG_DEFS = [  # (name, type, default) -- reference main.py:32-103
     ('precision', str, 'bf16'),          # extension: inference arithmetic (bf16 wgmma | fp32 CUDA cores)
     ('train_precision', str, 'fp32'),    # extension: training convolutions (fp32 as the reference | bf16 wgmma)
     ('synthetic_data', bool, False),     # extension: seeded synthetic HR clips / random frozen VGG instead of raising
+    # extension: fixed-order training reductions, bit-identical reruns of one seed.  Opt-in: absent from FLAGS unless
+    # given (argparse.SUPPRESS), so the flag set of a run without it stays exactly the reference's.
+    ('deterministic', bool, argparse.SUPPRESS),
 ]
 
 
@@ -62,7 +69,7 @@ def parse_flags(argv=None):
         if typ is bool:
             ap.add_argument('--' + name, dest=name, nargs='?', const=True, default=default,
                             type=lambda s: s.lower() in ('1', 'true', 'yes'))
-            ap.add_argument('--no' + name, dest=name, action='store_false')
+            ap.add_argument('--no' + name, dest=name, action='store_false', default=default)
         else:
             ap.add_argument('--' + name, type=typ, default=default)
     return ap.parse_args(argv)
@@ -458,6 +465,7 @@ def train(FLAGS):
         dist.init_process_group('nccl', device_id=torch.device('cuda', local_rank))
     from tecogan_b200 import config
     config.set_train_precision(FLAGS.train_precision)   # fp32 as the reference; bf16: wgmma convolutions, fp32 master weights
+    config.set_deterministic(getattr(FLAGS, 'deterministic', False))
     store = V.set_default_store(V.VariableStore(seed=FLAGS.rand_seed))   # same seed on every rank -> identical init
     gan = FLAGS.ratio > 0
     if FLAGS.checkpoint is not None:

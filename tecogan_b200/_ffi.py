@@ -103,6 +103,25 @@ SIGNATURES = {
     "teco_farneback_flow_up_f32": [_P, _I32, _I32, _I32, _P, _I32, _I32, _P],
     "teco_tof_reduce_f32": [_P, _P, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _P, _P, _P],
     "teco_png_plan_bytes": [_I32, _I32, _P, _P],
+    # fixed-order (deterministic) training reductions: workspace sizes, then the entry points
+    "teco_conv3x3_wgrad_tc_det_plan_bytes": [_I32, _I32, _I32, _I32, _I32, _P],
+    "teco_conv3x3_wgrad_tc_det": [_I32, _I32, _I32, _I32, _I32, _I32, _I32, _P, _P, _P, _I32, _P, _I64, _P],
+    "teco_conv2d_wgrad_f32_det_plan_bytes": [C.POINTER(ConvDesc), _I32, _P],
+    "teco_conv2d_wgrad_f32_det": [C.POINTER(ConvDesc), _P, _P, _P, _P, _I32, _P, _I64, _P],
+    "teco_bias_grad_f32_det_plan_bytes": [_I64, _I32, _P],
+    "teco_bias_grad_f32_det": [_P, _P, _I64, _I32, _I32, _I32, _P, _I64, _P],
+    "teco_bn_det_plan_bytes": [_I64, _I32, _P],
+    "teco_bn_train_f32_det": [_P, _P, _P, _P, _I64, _I32, _F, _I32, _P, _I64, _P],
+    "teco_bn_train_bwd_f32_det": [_P, _P, _P, _P, _P, _P, _I64, _I32, _F, _I32, _P, _I64, _P],
+    "teco_loss_det_plan_bytes": [_I64, _I32, _P],
+    "teco_loss_l2_f32_det": [_P, _P, _P, _P, _I64, _I32, _F, _P, _I64, _P],
+    "teco_loss_l1_f32_det": [_P, _P, _P, _P, _P, _I64, _I32, _I32, _F, _P, _I64, _P],
+    "teco_loss_cosine_f32_det": [_P, _P, _P, _P, _I64, _I32, _F, _P, _I64, _P],
+    "teco_loss_gan_f32_det": [_P, _P, _P, _P, _P, _P, _I64, _F, _F, _F, _P, _I64, _P],
+    "teco_warp_bwd_f32_det_plan_bytes": [_I32, _I32, _I32, _P],
+    "teco_warp_bwd_f32_det": [_P, _P, _P, _P, _P, _I32, _I32, _I32, _I32, _P, _I64, _P],
+    "teco_resize_bilinear_bwd_f32_det": [_P, _P, _I32, _I32, _I32, _I32, _I32, _I32, _P],
+    "teco_sum_ranks_f32": [_P, _I32, _I64, _P, _P],
     "teco_png_encode_rgb8": [_P, _I32, _I32, _P, _I64, _P, _I64, _P, _P],
     "teco_png_decode_plan_bytes": [_I32, _I32, _I32, _I32, _P],
     "teco_png_decode_rgb8": [_P, _I64, _P, _I32, _P, _I64, _P, _I64, _P, _P],

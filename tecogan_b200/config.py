@@ -1,7 +1,7 @@
 """Run-time configuration of the compute path (not part of the reference interface)."""
 import contextlib as _contextlib
 
-_cfg = {"precision": "bf16", "train_precision": "fp32", "train_forward": False}
+_cfg = {"precision": "bf16", "train_precision": "fp32", "train_forward": False, "deterministic": False}
 
 
 def set_precision(p):
@@ -31,6 +31,18 @@ def set_train_precision(p):
 
 def train_precision():
     return _cfg["train_precision"]
+
+
+def set_deterministic(on):
+    """True: every reduction of the training path (weight, bias and batch-norm gradients, batch-norm statistics, loss
+    scalars, the warp and resize scatter gradients, the multi-GPU gradient sum) runs on the fixed-order *_det kernels,
+    whose summation order depends on the shapes alone, so one seed gives bit-identical runs on one GPU model and build.
+    False (default): the atomic kernels."""
+    _cfg["deterministic"] = bool(on)
+
+
+def deterministic():
+    return _cfg["deterministic"]
 
 
 @_contextlib.contextmanager

@@ -146,11 +146,12 @@ conv2d_f32_kernel(const teco_conv_desc d, const float* __restrict__ x, const flo
 
 // ---------------------------------------------------------------------------------------
 // Weight gradient: for one tap, GEMM [Cin x pixels] * [pixels x Cout], split over pixels
-// (blockIdx.z) with fp32 atomics into dw.  grid = (ci tiles * taps, co tiles, splits).
+// (blockIdx.z) with fp32 atomics into dw.  grid = (ci tiles * taps, co tiles, splits).  With part != NULL split z stores
+// its sums to part[z][tap][ci][co] instead (the fixed-order entry point reduces them in split order).
 // ---------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256)
 conv2d_wgrad_f32_kernel(const teco_conv_desc d, const float* __restrict__ x, const float* __restrict__ dy,
-                        float* __restrict__ dw, int ci_tiles, long long pix_per_split) {
+                        float* __restrict__ dw, int ci_tiles, long long pix_per_split, float* __restrict__ part) {
   __shared__ __align__(16) float As[BK][BM + PADM];  // [pixel][ci]
   __shared__ __align__(16) float Bs[BK][BN + PADM];  // [pixel][co]
   const int tid = threadIdx.x;
@@ -232,19 +233,23 @@ conv2d_wgrad_f32_kernel(const teco_conv_desc d, const float* __restrict__ x, con
     for (int j = 0; j < 4; ++j) {
       int co = co0 + tx * 4 + j;
       if (co >= d.Cout) continue;
-      atomicAdd(&dw[((long long)tap * d.Cin + ci) * d.Cout + co], acc[i][j]);
+      const long long e = ((long long)tap * d.Cin + ci) * d.Cout + co;
+      if (part) part[(long long)blockIdx.z * d.KH * d.KW * d.Cin * d.Cout + e] = acc[i][j];
+      else atomicAdd(&dw[e], acc[i][j]);
     }
   }
 }
 
 // db[c] += sum over pixels of dy[pixel, c] (dy addressed through the output mapping).  Threads are laid out
-// channel-fastest (coalesced), 256 / C pixel lanes per block, shared-memory reduce, one atomic per channel per block.
+// channel-fastest (coalesced), 256 / C pixel lanes per block, shared-memory reduce, one atomic per channel per block
+// (kDet: part[block][c] stored instead, every sum rounded explicitly).
 // Many small blocks (16-64 pixels each): the first version gave a 4096-pixel layer 16 blocks of 64 serial iterations with
 // two 64-bit divisions each and cost 46 us per call -- 27 % of an FRVSR training step.
-template <bool kContig>
+template <bool kContig, bool kDet = false>
 __global__ void __launch_bounds__(256)
-bias_grad_kernel(const teco_conv_desc d, const float* __restrict__ dy, float* __restrict__ db, int pix_per_block) {
-  __shared__ float part[256];
+bias_grad_kernel(const teco_conv_desc d, const float* __restrict__ dy, float* __restrict__ db, int pix_per_block,
+                 float* __restrict__ part = nullptr) {
+  __shared__ float lanes[256];
   const int M = d.N * d.OH * d.OW;
   const int p_begin = blockIdx.x * pix_per_block;
   const int p_end = min(M, p_begin + pix_per_block);
@@ -255,23 +260,53 @@ bias_grad_kernel(const teco_conv_desc d, const float* __restrict__ dy, float* __
   if (ps < ppar) {
     for (int pm = p_begin + ps; pm < p_end; pm += ppar) {
       if (kContig) {
-        s += dy[(size_t)pm * d.out_cpitch + c];
+        s = kDet ? __fadd_rn(s, dy[(size_t)pm * d.out_cpitch + c]) : s + dy[(size_t)pm * d.out_cpitch + c];
       } else {
         int t = pm;
         const int ox = t % d.OW;
         t /= d.OW;
         const int oy = t % d.OH;
         const int n = t / d.OH;
-        s += dy[(((size_t)n * d.out_H + (oy * d.out_sy + d.out_oy)) * d.out_W + (ox * d.out_sx + d.out_ox)) * d.out_cpitch + c];
+        const float v = dy[(((size_t)n * d.out_H + (oy * d.out_sy + d.out_oy)) * d.out_W + (ox * d.out_sx + d.out_ox)) * d.out_cpitch + c];
+        s = kDet ? __fadd_rn(s, v) : s + v;
       }
     }
   }
-  part[threadIdx.x] = s;
+  lanes[threadIdx.x] = s;
   __syncthreads();
   if (ps == 0) {
-    for (int k = 1; k < ppar; ++k) s += part[k * C + c];
-    atomicAdd(&db[c], s);
+    if (kDet) {
+      for (int k = 1; k < ppar; ++k) s = __fadd_rn(s, lanes[k * C + c]);
+      part[(size_t)blockIdx.x * C + c] = s;
+    } else {
+      for (int k = 1; k < ppar; ++k) s += lanes[k * C + c];
+      atomicAdd(&db[c], s);
+    }
   }
+}
+
+// Fixed-order partitions (the *_det entry points): functions of the shapes alone.  The weight gradient splits the pixels
+// as the default path does on a device of DET_SMS SMs; the bias gradient takes blocks of 8 * (256 / C) pixels, at most
+// DET_BIAS_BLOCKS of them.
+constexpr int DET_SMS = 132;
+constexpr long long DET_BIAS_BLOCKS = 16LL * DET_SMS;
+
+long long wgrad_splits(long long M, int base, int target, long long* pps) {
+  long long splits = (target + base - 1) / base;
+  long long max_splits = (M + 255) / 256;  // at least 256 pixels per split
+  if (splits > max_splits) splits = max_splits;
+  if (splits < 1) splits = 1;
+  if (splits > 65535) splits = 65535;
+  *pps = (M + splits - 1) / splits;
+  *pps = (*pps + BK - 1) / BK * BK;
+  return (M + *pps - 1) / *pps;
+}
+
+long long det_bias_blocks(long long M, int C, int* ppb) {
+  *ppb = 8 * (256 / C);
+  long long blocks = (M + *ppb - 1) / *ppb;
+  if (blocks > DET_BIAS_BLOCKS) { blocks = DET_BIAS_BLOCKS; *ppb = (int)((M + blocks - 1) / blocks); blocks = (M + *ppb - 1) / *ppb; }
+  return blocks;
 }
 
 int check_desc(const teco_conv_desc* d, const char* who) {
@@ -321,17 +356,10 @@ extern "C" int teco_conv2d_wgrad_f32(const teco_conv_desc* d, const float* x, co
   int ci_tiles = teco_ceil_div(d->Cin, BM);
   int co_tiles = teco_ceil_div(d->Cout, BN);
   int base = ci_tiles * d->KH * d->KW * co_tiles;
-  int target = 4 * teco_sm_count();
-  long long splits = (target + base - 1) / base;
-  long long max_splits = (M + 255) / 256;  // at least 256 pixels per split
-  if (splits > max_splits) splits = max_splits;
-  if (splits < 1) splits = 1;
-  if (splits > 65535) splits = 65535;
-  long long pps = (M + splits - 1) / splits;
-  pps = (pps + BK - 1) / BK * BK;
-  splits = (M + pps - 1) / pps;
+  long long pps;
+  const long long splits = wgrad_splits(M, base, 4 * teco_sm_count(), &pps);
   dim3 grid(ci_tiles * d->KH * d->KW, co_tiles, (unsigned)splits);
-  conv2d_wgrad_f32_kernel<<<grid, 256, 0, s>>>(*d, x, dy, dw, ci_tiles, pps);
+  conv2d_wgrad_f32_kernel<<<grid, 256, 0, s>>>(*d, x, dy, dw, ci_tiles, pps, nullptr);
   TECO_CUDA_LAUNCH_CHECK("teco_conv2d_wgrad_f32");
   if (db) {
     const int ppar = 256 / d->Cout;
@@ -359,4 +387,88 @@ extern "C" int teco_bias_grad_f32(const float* dy, float* db, int64_t npix, int3
   bias_grad_kernel<true><<<(unsigned)blocks, 256, 0, s>>>(d, dy, db, ppb);
   TECO_CUDA_LAUNCH_CHECK("teco_bias_grad_f32");
   return TECO_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------
+// Fixed-order weight and bias gradients.  Workspace: [splits][KH][KW][Cin][Cout] fp32 partials of the weight gradient,
+// then (db != NULL) [blocks][Cout] partials of the bias gradient; each is summed in split order into dw / db.
+namespace {
+struct WgradDetPlan {
+  long long splits, pps, bias_blocks, w_floats, bytes;
+  int ci_tiles, co_tiles, ppb;
+};
+WgradDetPlan wgrad_det_plan(const teco_conv_desc* d, bool with_bias) {
+  WgradDetPlan p;
+  const long long M = (long long)d->N * d->OH * d->OW;
+  p.ci_tiles = teco_ceil_div(d->Cin, BM);
+  p.co_tiles = teco_ceil_div(d->Cout, BN);
+  p.splits = wgrad_splits(M, p.ci_tiles * d->KH * d->KW * p.co_tiles, 4 * DET_SMS, &p.pps);
+  p.w_floats = (long long)d->KH * d->KW * d->Cin * d->Cout;
+  p.bias_blocks = with_bias ? det_bias_blocks(M, d->Cout, &p.ppb) : 0;
+  p.bytes = (p.splits * p.w_floats + p.bias_blocks * d->Cout) * (long long)sizeof(float);
+  return p;
+}
+
+int bias_grad_det_launch(const teco_conv_desc& d, const float* dy, float* db, long long blocks, int ppb, float* part,
+                         int accumulate, cudaStream_t s) {
+  const bool contig = d.out_sy == 1 && d.out_sx == 1 && d.out_oy == 0 && d.out_ox == 0 && d.out_H == d.OH && d.out_W == d.OW;
+  if (contig) bias_grad_kernel<true, true><<<(unsigned)blocks, 256, 0, s>>>(d, dy, db, ppb, part);
+  else bias_grad_kernel<false, true><<<(unsigned)blocks, 256, 0, s>>>(d, dy, db, ppb, part);
+  TECO_CUDA_LAUNCH_CHECK("bias_grad_kernel(det)");
+  return teco_reduce_splits(part, (int)blocks, d.Cout, db, accumulate, s);
+}
+}  // namespace
+
+#define DET_WS_CHECK(who, need) \
+  TECO_CHECK_ARG(ws && ws_bytes >= (int64_t)(need) && (((uintptr_t)ws) & 15) == 0, \
+                 "%s: workspace of %lld bytes (16-byte aligned) needed, got %lld", who, (long long)(need), (long long)ws_bytes)
+
+extern "C" int teco_conv2d_wgrad_f32_det_plan_bytes(const teco_conv_desc* d, int32_t with_bias, int64_t* ws_bytes_host) {
+  int rc = check_desc(d, "teco_conv2d_wgrad_f32_det_plan_bytes");
+  if (rc) return rc;
+  TECO_CHECK_ARG(ws_bytes_host, "teco_conv2d_wgrad_f32_det_plan_bytes: NULL output");
+  TECO_CHECK_ARG(!with_bias || d->Cout <= 256, "teco_conv2d_wgrad_f32_det_plan_bytes: bias gradient supports Cout <= 256");
+  *ws_bytes_host = wgrad_det_plan(d, with_bias != 0).bytes;
+  return TECO_OK;
+}
+
+extern "C" int teco_conv2d_wgrad_f32_det(const teco_conv_desc* d, const float* x, const float* dy, float* dw, float* db,
+                                         int32_t accumulate, void* ws, int64_t ws_bytes, void* stream) {
+  int rc = check_desc(d, "teco_conv2d_wgrad_f32_det");
+  if (rc) return rc;
+  TECO_CHECK_ARG(x && dy && dw, "teco_conv2d_wgrad_f32_det: NULL tensor");
+  const long long M = (long long)d->N * d->OH * d->OW;
+  if (db) {
+    TECO_CHECK_ARG(d->Cout <= 256, "teco_conv2d_wgrad_f32_det: bias gradient supports Cout <= 256 (got %d)", d->Cout);
+    TECO_CHECK_ARG(M < (1LL << 31), "teco_conv2d_wgrad_f32_det: too many output pixels for the bias gradient");
+  }
+  const WgradDetPlan p = wgrad_det_plan(d, db != nullptr);
+  DET_WS_CHECK("teco_conv2d_wgrad_f32_det", p.bytes);
+  cudaStream_t s = (cudaStream_t)stream;
+  float* part = (float*)ws;
+  dim3 grid(p.ci_tiles * d->KH * d->KW, p.co_tiles, (unsigned)p.splits);
+  conv2d_wgrad_f32_kernel<<<grid, 256, 0, s>>>(*d, x, dy, dw, p.ci_tiles, p.pps, part);
+  TECO_CUDA_LAUNCH_CHECK("teco_conv2d_wgrad_f32_det");
+  rc = teco_reduce_splits(part, (int)p.splits, p.w_floats, dw, accumulate, s);
+  if (rc || !db) return rc;
+  return bias_grad_det_launch(*d, dy, db, p.bias_blocks, p.ppb, part + p.splits * p.w_floats, accumulate, s);
+}
+
+extern "C" int teco_bias_grad_f32_det_plan_bytes(int64_t npix, int32_t C, int64_t* ws_bytes_host) {
+  TECO_CHECK_ARG(ws_bytes_host && npix > 0 && C > 0 && C <= 256 && npix < (1LL << 31), "teco_bias_grad_f32_det_plan_bytes: bad argument");
+  int ppb;
+  *ws_bytes_host = det_bias_blocks(npix, C, &ppb) * C * (int64_t)sizeof(float);
+  return TECO_OK;
+}
+
+extern "C" int teco_bias_grad_f32_det(const float* dy, float* db, int64_t npix, int32_t C, int32_t cpitch, int32_t accumulate,
+                                      void* ws, int64_t ws_bytes, void* stream) {
+  TECO_CHECK_ARG(dy && db && npix > 0 && C > 0 && C <= 256 && cpitch >= C && npix < (1LL << 31), "teco_bias_grad_f32_det: bad argument");
+  int ppb;
+  const long long blocks = det_bias_blocks(npix, C, &ppb);
+  DET_WS_CHECK("teco_bias_grad_f32_det", blocks * C * sizeof(float));
+  teco_conv_desc d = {};
+  d.N = 1; d.OH = 1; d.OW = (int)npix; d.Cout = C; d.out_cpitch = cpitch;
+  d.out_H = 1; d.out_W = (int)npix; d.out_sy = 1; d.out_sx = 1;
+  return bias_grad_det_launch(d, dy, db, blocks, ppb, (float*)ws, accumulate, (cudaStream_t)stream);
 }

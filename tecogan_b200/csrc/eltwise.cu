@@ -85,31 +85,62 @@ __global__ void deprocess_u8_kernel(const float* __restrict__ x, float* __restri
 }
 
 // ------------------------------------------------------------------ batch norm (per channel over pixels)
-// pass 1: per-block partial sums into acc[0,C) via atomics; C <= 256.
+// Thread (c = tid % C, lane ps = tid / C) of a block sums pixels p0 + ps, p0 + ps + ppar, ... of its block's range.
+// Default: each lane adds its sum into acc[c] with an atomic.  kDet: the lanes' sums meet in shared memory and lane 0 adds
+// them in lane order into part[block][c] (the fixed-order path of the *_det entry points), with every product and sum
+// rounded explicitly so the order can be restated on the host.
+template <bool kDet>
+__device__ __forceinline__ void bn_lane_out(float* sh, float v, int ppar, int C, float* acc, float* part) {
+  const int c = threadIdx.x % C, ps = threadIdx.x / C;
+  if (!kDet) {
+    if (ps < ppar) atomicAdd(&acc[c], v);
+    return;
+  }
+  sh[threadIdx.x] = v;
+  __syncthreads();
+  if (ps == 0) {
+    for (int k = 1; k < ppar; ++k) v = __fadd_rn(v, sh[k * C + c]);
+    part[c] = v;
+  }
+  __syncthreads();
+}
+
+// pass 1: per-block partial sums into acc[0,C) via atomics (or part[block][C]); C <= 256.
+template <bool kDet>
 __global__ void bn_partial_kernel(const float* __restrict__ x, float* __restrict__ acc, long long npix, int C,
-                                  long long pix_per_block) {
+                                  long long pix_per_block, float* __restrict__ part) {
+  __shared__ float sh[TPB];
   int ppar = TPB / C;
   int c = threadIdx.x % C, ps = threadIdx.x / C;
-  if (ps >= ppar) return;
+  if (!kDet && ps >= ppar) return;
   long long p0 = (long long)blockIdx.x * pix_per_block, p1 = min(npix, p0 + pix_per_block);
   float s = 0.f;
-  for (long long p = p0 + ps; p < p1; p += ppar) s += x[p * C + c];
-  atomicAdd(&acc[c], s);
+  if (ps < ppar)
+    for (long long p = p0 + ps; p < p1; p += ppar) s = kDet ? __fadd_rn(s, x[p * C + c]) : s + x[p * C + c];
+  bn_lane_out<kDet>(sh, s, ppar, C, acc, part + (kDet ? (size_t)blockIdx.x * C : 0));
 }
 // two-pass variance for accuracy: pass 2 accumulates sum (x-mean)^2
+template <bool kDet>
 __global__ void bn_var_kernel(const float* __restrict__ x, const float* __restrict__ acc, float* __restrict__ var_acc,
-                              long long npix, int C, long long pix_per_block) {
+                              long long npix, int C, long long pix_per_block, float* __restrict__ part) {
+  __shared__ float sh[TPB];
   int ppar = TPB / C;
   int c = threadIdx.x % C, ps = threadIdx.x / C;
-  if (ps >= ppar) return;
-  float mean = acc[c] / (float)npix;
+  if (!kDet && ps >= ppar) return;
+  float mean = kDet ? __fdiv_rn(acc[c], (float)npix) : acc[c] / (float)npix;
   long long p0 = (long long)blockIdx.x * pix_per_block, p1 = min(npix, p0 + pix_per_block);
   float q = 0.f;
-  for (long long p = p0 + ps; p < p1; p += ppar) {
-    float v = x[p * C + c] - mean;
-    q += v * v;
-  }
-  atomicAdd(&var_acc[c], q);
+  if (ps < ppar)
+    for (long long p = p0 + ps; p < p1; p += ppar) {
+      if (kDet) {
+        const float v = __fsub_rn(x[p * C + c], mean);
+        q = __fadd_rn(q, __fmul_rn(v, v));
+      } else {
+        float v = x[p * C + c] - mean;
+        q += v * v;
+      }
+    }
+  bn_lane_out<kDet>(sh, q, ppar, C, var_acc, part + (kDet ? (size_t)blockIdx.x * C : 0));
 }
 __global__ void bn_finalize_kernel(const float* __restrict__ acc, const float* __restrict__ var_acc,
                                    float* __restrict__ stats, long long npix, int C) {
@@ -130,23 +161,32 @@ __global__ void bn_apply_kernel(const float* __restrict__ x, const float* __rest
   }
 }
 // backward: g = dy * lrelu'(y); dbeta = sum g; dx = rstd * (g - mean(g) - xhat * mean(g*xhat))
+template <bool kDet>
 __global__ void bn_bwd_partial_kernel(const float* __restrict__ x, const float* __restrict__ y, const float* __restrict__ dy,
                                       const float* __restrict__ stats, float* __restrict__ acc, long long npix, int C,
-                                      float eps, int lrelu02, long long pix_per_block) {
+                                      float eps, int lrelu02, long long pix_per_block, float* __restrict__ part) {
+  __shared__ float sh[TPB];
   int ppar = TPB / C;
   int c = threadIdx.x % C, ps = threadIdx.x / C;
-  if (ps >= ppar) return;
+  if (!kDet && ps >= ppar) return;
   float mean = stats[c], rstd = rsqrtf(stats[C + c] + eps);
   long long p0 = (long long)blockIdx.x * pix_per_block, p1 = min(npix, p0 + pix_per_block);
   float s = 0.f, q = 0.f;
-  for (long long p = p0 + ps; p < p1; p += ppar) {
-    float g = dy[p * C + c];
-    if (lrelu02 && y[p * C + c] < 0.f) g *= 0.2f;
-    s += g;
-    q += g * (x[p * C + c] - mean) * rstd;
-  }
-  atomicAdd(&acc[c], s);
-  atomicAdd(&acc[C + c], q);
+  if (ps < ppar)
+    for (long long p = p0 + ps; p < p1; p += ppar) {
+      float g = dy[p * C + c];
+      if (lrelu02 && y[p * C + c] < 0.f) g *= 0.2f;
+      if (kDet) {
+        s = __fadd_rn(s, g);
+        q = __fadd_rn(q, __fmul_rn(__fmul_rn(g, __fsub_rn(x[p * C + c], mean)), rstd));
+      } else {
+        s += g;
+        q += g * (x[p * C + c] - mean) * rstd;
+      }
+    }
+  float* pb = part + (kDet ? (size_t)blockIdx.x * 2 * C : 0);
+  bn_lane_out<kDet>(sh, s, ppar, C, acc, pb);
+  bn_lane_out<kDet>(sh, q, ppar, C, acc + C, pb + C);
 }
 __global__ void bn_bwd_apply_kernel(const float* __restrict__ x, const float* __restrict__ y, const float* __restrict__ dy,
                                     const float* __restrict__ stats, const float* __restrict__ acc, float* __restrict__ dx,
@@ -164,22 +204,30 @@ __global__ void bn_bwd_apply_kernel(const float* __restrict__ x, const float* __
 }
 
 // ------------------------------------------------------------------ loss reductions
-// warp-shuffle -> block -> one atomic per block into out[k]
+// warp-shuffle -> block -> one atomic per block into out[k].  With part != NULL (the *_det entry points) block b stores
+// its value to part[b * K + k] instead, and the per-thread sums round every product and sum explicitly.
+__device__ __forceinline__ void loss_block_out(float* out, float* part, int K, int k, float v) {
+  if (part) part[(size_t)blockIdx.x * K + k] = v;
+  else atomicAdd(out + k, v);
+}
+
 __global__ void loss_l2_kernel(const float* __restrict__ a, const float* __restrict__ b, float* __restrict__ out,
-                               float* __restrict__ da, long long n, float inv_npix, float gscale) {
+                               float* __restrict__ da, long long n, float inv_npix, float gscale, float* __restrict__ part) {
   __shared__ float sm[32];
   float s = 0.f;
   GRID_STRIDE(i, n) {
     float d = a[i] - b[i];
-    s += d * d;
+    if (part) s = __fadd_rn(s, __fmul_rn(d, d));
+    else s += d * d;
     if (da) da[i] = 2.f * d * inv_npix * gscale;
   }
   s = block_sum(s, sm);
-  if (threadIdx.x == 0) atomicAdd(out, s * inv_npix);
+  if (threadIdx.x == 0) loss_block_out(out, part, 1, 0, s * inv_npix);
 }
 
 __global__ void loss_l1_kernel(const float* __restrict__ a, const float* __restrict__ b, float* __restrict__ out,
-                               float* __restrict__ da, float* __restrict__ db, long long n, float inv_den, float gscale) {
+                               float* __restrict__ da, float* __restrict__ db, long long n, float inv_den, float gscale,
+                               float* __restrict__ part) {
   __shared__ float sm[32];
   float s = 0.f;
   GRID_STRIDE(i, n) {
@@ -190,12 +238,12 @@ __global__ void loss_l1_kernel(const float* __restrict__ a, const float* __restr
     if (db) db[i] = -g;
   }
   s = block_sum(s, sm);
-  if (threadIdx.x == 0) atomicAdd(out, s * inv_den);
+  if (threadIdx.x == 0) loss_block_out(out, part, 1, 0, s * inv_den);
 }
 
 // one warp per pixel: cos = <f,g> / (sqrt(|f|^2+eps) sqrt(|g|^2+eps)), eps=1e-12 (reference lib/Teco.py:20)
 __global__ void loss_cosine_kernel(const float* __restrict__ f, const float* __restrict__ g, float* __restrict__ out,
-                                   float* __restrict__ df, long long npix, int C, float gscale) {
+                                   float* __restrict__ df, long long npix, int C, float gscale, float* __restrict__ part) {
   __shared__ float sm[32];
   int lane = threadIdx.x & 31;
   long long warp = (blockIdx.x * (long long)blockDim.x + threadIdx.x) >> 5;
@@ -208,16 +256,22 @@ __global__ void loss_cosine_kernel(const float* __restrict__ f, const float* __r
     float ff = 0.f, gg = 0.f, fg = 0.f;
     for (int c = lane; c < C; c += 32) {
       float x = fp[c], y = gp[c];
-      ff += x * x;
-      gg += y * y;
-      fg += x * y;
+      if (part) {
+        ff = __fadd_rn(ff, __fmul_rn(x, x));
+        gg = __fadd_rn(gg, __fmul_rn(y, y));
+        fg = __fadd_rn(fg, __fmul_rn(x, y));
+      } else {
+        ff += x * x;
+        gg += y * y;
+        fg += x * y;
+      }
     }
     ff = warp_sum(ff);
     gg = warp_sum(gg);
     fg = warp_sum(fg);
     float nf = sqrtf(ff + 1e-12f), ng = sqrtf(gg + 1e-12f);
     float cosv = fg / (nf * ng);
-    if (lane == 0) local += cosv;
+    if (lane == 0) local = part ? __fadd_rn(local, cosv) : local + cosv;
     if (df) {
       // d(1 - mean cos)/df = -(1/npix) * ( g/(nf ng) - cos * f / nf^2 )
       float k1 = -inv * gscale / (nf * ng), k2 = inv * gscale * cosv / (nf * nf);
@@ -225,24 +279,32 @@ __global__ void loss_cosine_kernel(const float* __restrict__ f, const float* __r
     }
   }
   float s = block_sum(local, sm);
-  if (threadIdx.x == 0) atomicAdd(out, -s * inv);
+  if (threadIdx.x == 0) loss_block_out(out, part, 1, 0, -s * inv);
 }
 __global__ void add_const_kernel(float* p, float v) { p[0] += v; }
 
 __global__ void loss_gan_kernel(const float* __restrict__ dfk, const float* __restrict__ drl, float* __restrict__ out,
                                 float* __restrict__ g_adv, float* __restrict__ g_dis_f, float* __restrict__ g_dis_r,
-                                long long n, float eps, float s_adv, float s_dis) {
+                                long long n, float eps, float s_adv, float s_dis, float* __restrict__ part) {
   __shared__ float sm[32];
   float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f, a4 = 0.f;
   float inv = 1.0f / (float)n;
   GRID_STRIDE(i, n) {
     float f = dfk[i], r = drl[i];
     float lf = logf(f + eps), l1f = logf(1.f - f + eps), lr = logf(r + eps);
-    a0 += -lf;
-    a1 += -(l1f + lr);
-    a2 += lr;
-    a3 += r;
-    a4 += f;
+    if (part) {
+      a0 = __fadd_rn(a0, -lf);
+      a1 = __fadd_rn(a1, -__fadd_rn(l1f, lr));
+      a2 = __fadd_rn(a2, lr);
+      a3 = __fadd_rn(a3, r);
+      a4 = __fadd_rn(a4, f);
+    } else {
+      a0 += -lf;
+      a1 += -(l1f + lr);
+      a2 += lr;
+      a3 += r;
+      a4 += f;
+    }
     if (g_adv) g_adv[i] = -inv * s_adv / (f + eps);
     if (g_dis_f) g_dis_f[i] = inv * s_dis / (1.f - f + eps);
     if (g_dis_r) g_dis_r[i] = -inv * s_dis / (r + eps);
@@ -253,11 +315,20 @@ __global__ void loss_gan_kernel(const float* __restrict__ dfk, const float* __re
   a3 = block_sum(a3, sm);
   a4 = block_sum(a4, sm);
   if (threadIdx.x == 0) {
-    atomicAdd(out + 0, a0 * inv);
-    atomicAdd(out + 1, a1 * inv);
-    atomicAdd(out + 2, a2 * inv);
-    atomicAdd(out + 3, a3 * inv);
-    atomicAdd(out + 4, a4 * inv);
+    loss_block_out(out, part, 5, 0, a0 * inv);
+    loss_block_out(out, part, 5, 1, a1 * inv);
+    loss_block_out(out, part, 5, 2, a2 * inv);
+    loss_block_out(out, part, 5, 3, a3 * inv);
+    loss_block_out(out, part, 5, 4, a4 * inv);
+  }
+}
+
+// out[e] (+)= part[0][e] + part[1][e] + ... + part[S-1][e], summed in split order (the fixed-order reductions).
+__global__ void reduce_splits_kernel(const float* __restrict__ part, int S, long long E, float* __restrict__ out, int accumulate) {
+  GRID_STRIDE(e, E) {
+    float t = part[e];
+    for (int s = 1; s < S; ++s) t = __fadd_rn(t, part[(long long)s * E + e]);
+    out[e] = accumulate ? __fadd_rn(out[e], t) : t;
   }
 }
 
@@ -340,8 +411,8 @@ int teco_bn_train_f32(const float* x, const float* beta, float* y, float* stats,
   if (blocks > 2 * teco_sm_count()) blocks = 2 * teco_sm_count();
   long long ppb = (npix + blocks - 1) / blocks;
   blocks = (npix + ppb - 1) / ppb;
-  bn_partial_kernel<<<(unsigned)blocks, TPB, 0, ST>>>(x, acc, npix, C, ppb);
-  bn_var_kernel<<<(unsigned)blocks, TPB, 0, ST>>>(x, acc, acc + C, npix, C, ppb);
+  bn_partial_kernel<false><<<(unsigned)blocks, TPB, 0, ST>>>(x, acc, npix, C, ppb, nullptr);
+  bn_var_kernel<false><<<(unsigned)blocks, TPB, 0, ST>>>(x, acc, acc + C, npix, C, ppb, nullptr);
   TECO_CUDA_LAUNCH_CHECK("teco_bn_train_f32(stats)");
   bn_finalize_kernel<<<teco_ceil_div(C, 128), 128, 0, ST>>>(acc, acc + C, stats, npix, C);
   bn_apply_kernel<<<grid_for(npix * C), TPB, 0, ST>>>(x, beta, stats, y, npix, C, eps, lrelu02);
@@ -359,7 +430,7 @@ int teco_bn_train_bwd_f32(const float* x, const float* y, const float* dy, const
   if (blocks > 2 * teco_sm_count()) blocks = 2 * teco_sm_count();
   long long ppb = (npix + blocks - 1) / blocks;
   blocks = (npix + ppb - 1) / ppb;
-  bn_bwd_partial_kernel<<<(unsigned)blocks, TPB, 0, ST>>>(x, y, dy, stats, dbeta, npix, C, eps, lrelu02, ppb);
+  bn_bwd_partial_kernel<false><<<(unsigned)blocks, TPB, 0, ST>>>(x, y, dy, stats, dbeta, npix, C, eps, lrelu02, ppb, nullptr);
   bn_bwd_apply_kernel<<<grid_for(npix * C), TPB, 0, ST>>>(x, y, dy, stats, dbeta, dx, npix, C, eps, lrelu02);
   TECO_CUDA_LAUNCH_CHECK("teco_bn_train_bwd_f32");
   return TECO_OK;
@@ -369,7 +440,7 @@ int teco_loss_l2_f32(const float* a, const float* b, float* out, float* da, int6
                      void* stream) {
   TECO_CHECK_ARG(a && b && out && npix > 0 && C > 0, "teco_loss_l2_f32: bad argument");
   TECO_CUDA_CALL(cudaMemsetAsync(out, 0, sizeof(float), ST));
-  loss_l2_kernel<<<grid_for(npix * C, TPB * 4), TPB, 0, ST>>>(a, b, out, da, npix * C, 1.0f / (float)npix, gscale);
+  loss_l2_kernel<<<grid_for(npix * C, TPB * 4), TPB, 0, ST>>>(a, b, out, da, npix * C, 1.0f / (float)npix, gscale, nullptr);
   TECO_CUDA_LAUNCH_CHECK("teco_loss_l2_f32");
   return TECO_OK;
 }
@@ -379,7 +450,7 @@ int teco_loss_l1_f32(const float* a, const float* b, float* out, float* da, floa
   TECO_CHECK_ARG(a && b && out && npix > 0 && C > 0, "teco_loss_l1_f32: bad argument");
   TECO_CUDA_CALL(cudaMemsetAsync(out, 0, sizeof(float), ST));
   float inv_den = per_pixel ? 1.0f / (float)npix : 1.0f / ((float)npix * (float)C);
-  loss_l1_kernel<<<grid_for(npix * C, TPB * 4), TPB, 0, ST>>>(a, b, out, da, db, npix * C, inv_den, gscale);
+  loss_l1_kernel<<<grid_for(npix * C, TPB * 4), TPB, 0, ST>>>(a, b, out, da, db, npix * C, inv_den, gscale, nullptr);
   TECO_CUDA_LAUNCH_CHECK("teco_loss_l1_f32");
   return TECO_OK;
 }
@@ -388,7 +459,7 @@ int teco_loss_cosine_f32(const float* f, const float* g, float* out, float* df, 
                          void* stream) {
   TECO_CHECK_ARG(f && g && out && npix > 0 && C > 0, "teco_loss_cosine_f32: bad argument");
   TECO_CUDA_CALL(cudaMemsetAsync(out, 0, sizeof(float), ST));
-  loss_cosine_kernel<<<grid_for(npix * 32), TPB, 0, ST>>>(f, g, out, df, npix, C, gscale);
+  loss_cosine_kernel<<<grid_for(npix * 32), TPB, 0, ST>>>(f, g, out, df, npix, C, gscale, nullptr);
   add_const_kernel<<<1, 1, 0, ST>>>(out, 1.0f);
   TECO_CUDA_LAUNCH_CHECK("teco_loss_cosine_f32");
   return TECO_OK;
@@ -398,7 +469,7 @@ int teco_loss_gan_f32(const float* d_fake, const float* d_real, float* out, floa
                       float* g_dis_r, int64_t n, float eps, float s_adv, float s_dis, void* stream) {
   TECO_CHECK_ARG(d_fake && d_real && out && n > 0, "teco_loss_gan_f32: bad argument");
   TECO_CUDA_CALL(cudaMemsetAsync(out, 0, sizeof(float) * 5, ST));
-  loss_gan_kernel<<<grid_for(n, TPB * 4), TPB, 0, ST>>>(d_fake, d_real, out, g_adv, g_dis_f, g_dis_r, n, eps, s_adv, s_dis);
+  loss_gan_kernel<<<grid_for(n, TPB * 4), TPB, 0, ST>>>(d_fake, d_real, out, g_adv, g_dis_f, g_dis_r, n, eps, s_adv, s_dis, nullptr);
   TECO_CUDA_LAUNCH_CHECK("teco_loss_gan_f32");
   return TECO_OK;
 }
@@ -409,6 +480,159 @@ int teco_adam_f32(float* p, float* m, float* v, const float* g, int64_t n, float
   adam_kernel<<<grid_for(n), TPB, 0, ST>>>(p, m, v, g, n, lr_t, b1, b2, eps, gscale);
   TECO_CUDA_LAUNCH_CHECK("teco_adam_f32");
   return TECO_OK;
+}
+
+}  // extern "C"
+
+// ---------------------------------------------------------------------------------------------------
+// Fixed-order (deterministic) variants.  Every partition below is a function of the call's shapes alone, never of the
+// device: block b of a reduction writes its partial to the caller's workspace and reduce_splits_kernel sums the partials
+// in block order.  DESIGN.md section 4.3 gives the orders and the workspace sizes.
+namespace {
+constexpr long long DET_BN_BLOCKS = 264;     // batch-norm statistics: at most this many blocks of >= 1024 pixels
+constexpr long long DET_LOSS_BLOCKS = 2112;  // loss reductions: at most this many blocks
+
+long long det_bn_blocks(long long npix, long long* ppb) {
+  long long blocks = (npix + 1023) / 1024;
+  if (blocks > DET_BN_BLOCKS) blocks = DET_BN_BLOCKS;
+  *ppb = (npix + blocks - 1) / blocks;
+  return (npix + *ppb - 1) / *ppb;
+}
+
+unsigned det_grid(long long n, int per_block) {
+  long long b = (n + per_block - 1) / per_block;
+  if (b > DET_LOSS_BLOCKS) b = DET_LOSS_BLOCKS;
+  if (b < 1) b = 1;
+  return (unsigned)b;
+}
+
+// blocks of each loss: l2 / l1 (kind 0 / 1) over npix * C elements, cosine (2) one warp per pixel, gan (3) over npix values
+unsigned det_loss_blocks(int kind, long long npix, int C) {
+  if (kind == 2) return det_grid(npix * 32, TPB);
+  if (kind == 3) return det_grid(npix, TPB * 4);
+  return det_grid(npix * C, TPB * 4);
+}
+}  // namespace
+
+int teco_reduce_splits(const float* part, int S, long long E, float* out, int accumulate, cudaStream_t stream) {
+  reduce_splits_kernel<<<grid_for(E), TPB, 0, stream>>>(part, S, E, out, accumulate);
+  TECO_CUDA_LAUNCH_CHECK("reduce_splits_kernel");
+  return TECO_OK;
+}
+
+#define DET_WS_CHECK(who, need) \
+  TECO_CHECK_ARG(ws && ws_bytes >= (int64_t)(need) && (((uintptr_t)ws) & 15) == 0, \
+                 "%s: workspace of %lld bytes (16-byte aligned) needed, got %lld", who, (long long)(need), (long long)ws_bytes)
+
+extern "C" {
+
+int teco_bn_det_plan_bytes(int64_t npix, int32_t C, int64_t* ws_bytes_host) {
+  TECO_CHECK_ARG(ws_bytes_host && npix > 0 && C > 0 && C <= 256, "teco_bn_det_plan_bytes: bad argument");
+  long long ppb;
+  *ws_bytes_host = (int64_t)det_bn_blocks(npix, &ppb) * 2 * C * (int64_t)sizeof(float);
+  return TECO_OK;
+}
+
+int teco_bn_train_f32_det(const float* x, const float* beta, float* y, float* stats, int64_t npix, int32_t C, float eps,
+                          int32_t lrelu02, void* ws, int64_t ws_bytes, void* stream) {
+  TECO_CHECK_ARG(x && beta && y && stats && npix > 0, "teco_bn_train_f32_det: bad argument");
+  TECO_CHECK_ARG(C > 0 && C <= 256, "teco_bn_train_f32_det: C must be in [1,256] (got %d)", C);
+  long long ppb;
+  const long long blocks = det_bn_blocks(npix, &ppb);
+  DET_WS_CHECK("teco_bn_train_f32_det", blocks * 2 * C * sizeof(float));
+  float* acc = stats + 2 * C;
+  float* part = (float*)ws;
+  bn_partial_kernel<true><<<(unsigned)blocks, TPB, 0, ST>>>(x, nullptr, npix, C, ppb, part);
+  TECO_CUDA_LAUNCH_CHECK("teco_bn_train_f32_det(sum)");
+  int rc = teco_reduce_splits(part, (int)blocks, C, acc, 0, ST);
+  if (rc) return rc;
+  bn_var_kernel<true><<<(unsigned)blocks, TPB, 0, ST>>>(x, acc, nullptr, npix, C, ppb, part);
+  TECO_CUDA_LAUNCH_CHECK("teco_bn_train_f32_det(var)");
+  rc = teco_reduce_splits(part, (int)blocks, C, acc + C, 0, ST);
+  if (rc) return rc;
+  bn_finalize_kernel<<<teco_ceil_div(C, 128), 128, 0, ST>>>(acc, acc + C, stats, npix, C);
+  bn_apply_kernel<<<grid_for(npix * C), TPB, 0, ST>>>(x, beta, stats, y, npix, C, eps, lrelu02);
+  TECO_CUDA_LAUNCH_CHECK("teco_bn_train_f32_det");
+  return TECO_OK;
+}
+
+int teco_bn_train_bwd_f32_det(const float* x, const float* y, const float* dy, const float* stats, float* dx, float* dbeta,
+                              int64_t npix, int32_t C, float eps, int32_t lrelu02, void* ws, int64_t ws_bytes, void* stream) {
+  TECO_CHECK_ARG(x && y && dy && stats && dx && dbeta && npix > 0, "teco_bn_train_bwd_f32_det: bad argument");
+  TECO_CHECK_ARG(C > 0 && C <= 256, "teco_bn_train_bwd_f32_det: C must be in [1,256] (got %d)", C);
+  long long ppb;
+  const long long blocks = det_bn_blocks(npix, &ppb);
+  DET_WS_CHECK("teco_bn_train_bwd_f32_det", blocks * 2 * C * sizeof(float));
+  float* part = (float*)ws;
+  bn_bwd_partial_kernel<true><<<(unsigned)blocks, TPB, 0, ST>>>(x, y, dy, stats, nullptr, npix, C, eps, lrelu02, ppb, part);
+  TECO_CUDA_LAUNCH_CHECK("teco_bn_train_bwd_f32_det(partial)");
+  const int rc = teco_reduce_splits(part, (int)blocks, 2 * C, dbeta, 0, ST);
+  if (rc) return rc;
+  bn_bwd_apply_kernel<<<grid_for(npix * C), TPB, 0, ST>>>(x, y, dy, stats, dbeta, dx, npix, C, eps, lrelu02);
+  TECO_CUDA_LAUNCH_CHECK("teco_bn_train_bwd_f32_det");
+  return TECO_OK;
+}
+
+int teco_loss_det_plan_bytes(int64_t npix, int32_t C, int64_t* ws_bytes_host) {
+  TECO_CHECK_ARG(ws_bytes_host && npix > 0 && C > 0, "teco_loss_det_plan_bytes: bad argument");
+  unsigned most = 0;
+  for (int kind = 0; kind < 4; ++kind) {
+    const unsigned b = det_loss_blocks(kind, npix, C) * (kind == 3 ? 5 : 1);
+    if (b > most) most = b;
+  }
+  *ws_bytes_host = (int64_t)most * (int64_t)sizeof(float);
+  return TECO_OK;
+}
+
+int teco_loss_l2_f32_det(const float* a, const float* b, float* out, float* da, int64_t npix, int32_t C, float gscale,
+                         void* ws, int64_t ws_bytes, void* stream) {
+  TECO_CHECK_ARG(a && b && out && npix > 0 && C > 0, "teco_loss_l2_f32_det: bad argument");
+  const unsigned blocks = det_loss_blocks(0, npix, C);
+  DET_WS_CHECK("teco_loss_l2_f32_det", blocks * sizeof(float));
+  loss_l2_kernel<<<blocks, TPB, 0, ST>>>(a, b, out, da, npix * C, 1.0f / (float)npix, gscale, (float*)ws);
+  TECO_CUDA_LAUNCH_CHECK("teco_loss_l2_f32_det");
+  return teco_reduce_splits((float*)ws, (int)blocks, 1, out, 0, ST);
+}
+
+int teco_loss_l1_f32_det(const float* a, const float* b, float* out, float* da, float* db, int64_t npix, int32_t C,
+                         int32_t per_pixel, float gscale, void* ws, int64_t ws_bytes, void* stream) {
+  TECO_CHECK_ARG(a && b && out && npix > 0 && C > 0, "teco_loss_l1_f32_det: bad argument");
+  const unsigned blocks = det_loss_blocks(1, npix, C);
+  DET_WS_CHECK("teco_loss_l1_f32_det", blocks * sizeof(float));
+  float inv_den = per_pixel ? 1.0f / (float)npix : 1.0f / ((float)npix * (float)C);
+  loss_l1_kernel<<<blocks, TPB, 0, ST>>>(a, b, out, da, db, npix * C, inv_den, gscale, (float*)ws);
+  TECO_CUDA_LAUNCH_CHECK("teco_loss_l1_f32_det");
+  return teco_reduce_splits((float*)ws, (int)blocks, 1, out, 0, ST);
+}
+
+int teco_loss_cosine_f32_det(const float* f, const float* g, float* out, float* df, int64_t npix, int32_t C, float gscale,
+                             void* ws, int64_t ws_bytes, void* stream) {
+  TECO_CHECK_ARG(f && g && out && npix > 0 && C > 0, "teco_loss_cosine_f32_det: bad argument");
+  const unsigned blocks = det_loss_blocks(2, npix, C);
+  DET_WS_CHECK("teco_loss_cosine_f32_det", blocks * sizeof(float));
+  loss_cosine_kernel<<<blocks, TPB, 0, ST>>>(f, g, out, df, npix, C, gscale, (float*)ws);
+  TECO_CUDA_LAUNCH_CHECK("teco_loss_cosine_f32_det");
+  const int rc = teco_reduce_splits((float*)ws, (int)blocks, 1, out, 0, ST);
+  if (rc) return rc;
+  add_const_kernel<<<1, 1, 0, ST>>>(out, 1.0f);
+  TECO_CUDA_LAUNCH_CHECK("teco_loss_cosine_f32_det");
+  return TECO_OK;
+}
+
+int teco_loss_gan_f32_det(const float* d_fake, const float* d_real, float* out, float* g_adv, float* g_dis_f,
+                          float* g_dis_r, int64_t n, float eps, float s_adv, float s_dis, void* ws, int64_t ws_bytes,
+                          void* stream) {
+  TECO_CHECK_ARG(d_fake && d_real && out && n > 0, "teco_loss_gan_f32_det: bad argument");
+  const unsigned blocks = det_loss_blocks(3, n, 1);
+  DET_WS_CHECK("teco_loss_gan_f32_det", blocks * 5 * sizeof(float));
+  loss_gan_kernel<<<blocks, TPB, 0, ST>>>(d_fake, d_real, out, g_adv, g_dis_f, g_dis_r, n, eps, s_adv, s_dis, (float*)ws);
+  TECO_CUDA_LAUNCH_CHECK("teco_loss_gan_f32_det");
+  return teco_reduce_splits((float*)ws, (int)blocks, 5, out, 0, ST);
+}
+
+int teco_sum_ranks_f32(const float* src, int32_t R, int64_t n, float* dst, void* stream) {
+  TECO_CHECK_ARG(src && dst && R > 0 && n > 0, "teco_sum_ranks_f32: bad argument");
+  return teco_reduce_splits(src, R, n, dst, 0, ST);
 }
 
 }  // extern "C"

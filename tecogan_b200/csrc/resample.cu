@@ -95,6 +95,150 @@ __global__ void warp_bwd_f32_kernel(const float* __restrict__ img, const float* 
   }
 }
 
+// ---- fixed-order gradient of dense_image_warp with respect to the image.  Source pixel i reads the four destinations
+// (y0, x0), (y0, x0 + 1), (y0 + 1, x0), (y0 + 1, x0 + 1) of bil_setup (distinct: the clamp keeps y0 <= H - 2, x0 <= W - 2).
+// A counting sort lists, for every destination q, the entries 4 i + corner that reach it; each list is put in ascending
+// order and dimg[q][c] = (((0 + g_1) + g_2) + ...) with g_k = dout[i_k][c] * w_y * w_x rounded as the atomic kernel
+// rounds it.  The integer atomics of the count and the placement are the only unordered steps, and the sort undoes them.
+constexpr int WD_SCAN = 1024;
+
+__device__ __forceinline__ long long warp_dst(const Bil& b, int n, int H, int W, int corner) {
+  return ((long long)n * H + b.y0 + (corner >> 1)) * W + b.x0 + (corner & 1);
+}
+
+__device__ __forceinline__ Bil warp_src(const float* __restrict__ flow, long long i, int H, int W, int* n) {
+  const int x = (int)(i % W);
+  const long long t = i / W;
+  const int y = (int)(t % H);
+  *n = (int)(t / H);
+  const float2 f = *reinterpret_cast<const float2*>(flow + i * 2);
+  return bil_setup((float)y - f.x, (float)x - f.y, H, W);
+}
+
+__global__ void warp_det_count_kernel(const float* __restrict__ flow, int* __restrict__ cnt, int N, int H, int W) {
+  const long long total = (long long)N * H * W;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    int n;
+    const Bil b = warp_src(flow, i, H, W, &n);
+    for (int k = 0; k < 4; ++k) atomicAdd(&cnt[warp_dst(b, n, H, W, k)], 1);
+  }
+}
+
+// off[q] = exclusive prefix of cnt inside q's chunk of WD_SCAN; bsum[chunk] = the chunk's total
+__global__ void __launch_bounds__(WD_SCAN) warp_det_scan_chunks_kernel(const int* __restrict__ cnt, int* __restrict__ off,
+                                                                      int* __restrict__ bsum, long long P) {
+  __shared__ int sm[WD_SCAN / 32 + 1];
+  const long long q = (long long)blockIdx.x * WD_SCAN + threadIdx.x;
+  int total;
+  const int before = cta_exclusive_scan<WD_SCAN>(q < P ? cnt[q] : 0, sm, &total);
+  if (q < P) off[q] = before;
+  if (threadIdx.x == 0) bsum[blockIdx.x] = total;
+}
+
+// bsum -> exclusive prefix over chunks, in place (one CTA walking the chunks in order)
+__global__ void __launch_bounds__(WD_SCAN) warp_det_scan_totals_kernel(int* __restrict__ bsum, int chunks) {
+  __shared__ int sm[WD_SCAN / 32 + 1];
+  int carry = 0;
+  for (int c0 = 0; c0 < chunks; c0 += WD_SCAN) {
+    const int c = c0 + threadIdx.x;
+    int total;
+    const int before = cta_exclusive_scan<WD_SCAN>(c < chunks ? bsum[c] : 0, sm, &total);
+    if (c < chunks) bsum[c] = carry + before;
+    carry += total;
+  }
+}
+
+__device__ __forceinline__ int warp_det_start(const int* off, const int* bsum, long long q) {
+  return off[q] + bsum[q / WD_SCAN];
+}
+
+__global__ void warp_det_place_kernel(const float* __restrict__ flow, int* __restrict__ cnt, const int* __restrict__ off,
+                                      const int* __restrict__ bsum, int* __restrict__ list, int N, int H, int W) {
+  const long long total = (long long)N * H * W;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    int n;
+    const Bil b = warp_src(flow, i, H, W, &n);
+    for (int k = 0; k < 4; ++k) {
+      const long long q = warp_dst(b, n, H, W, k);
+      list[warp_det_start(off, bsum, q) + atomicSub(&cnt[q], 1) - 1] = (int)(4 * i + k);
+    }
+  }
+}
+
+__global__ void warp_det_gather_kernel(const float* __restrict__ flow, const float* __restrict__ dout, const int* __restrict__ off,
+                                       const int* __restrict__ bsum, int* __restrict__ list, float* __restrict__ dimg,
+                                       int N, int H, int W, int C) {
+  const long long P = (long long)N * H * W;
+  for (long long q = blockIdx.x * (long long)blockDim.x + threadIdx.x; q < P; q += (long long)gridDim.x * blockDim.x) {
+    const int beg = warp_det_start(off, bsum, q);
+    const int end = q + 1 < P ? warp_det_start(off, bsum, q + 1) : (int)(4 * P);
+    for (int a = beg + 1; a < end; ++a) {   // insertion sort: lists are short except where a flow converges
+      const int v = list[a];
+      int b = a - 1;
+      while (b >= beg && list[b] > v) { list[b + 1] = list[b]; --b; }
+      list[b + 1] = v;
+    }
+    float* d = dimg + q * C;
+    for (int c = 0; c < C; ++c) d[c] = 0.f;
+    for (int a = beg; a < end; ++a) {
+      const int e = list[a];
+      const long long i = e >> 2;
+      const int k = e & 3;
+      int n;
+      const Bil b = warp_src(flow, i, H, W, &n);
+      const float wy = (k >> 1) ? b.ay : 1.f - b.ay, wx = (k & 1) ? b.ax : 1.f - b.ax;
+      for (int c = 0; c < C; ++c) d[c] = __fadd_rn(d[c], __fmul_rn(__fmul_rn(dout[i * C + c], wy), wx));
+    }
+  }
+}
+
+// ---- fixed-order gradient of the legacy bilinear resize, as a gather: input pixel (y, x) sums the outputs (Y, X) that
+// read it in ascending Y, then X, then corner order (top-left, top-right, bottom-left, bottom-right), each product rounded
+// as the atomic kernel rounds it.  The outputs that read row y are those with y0(Y) in {y - 1, y}; y0 is monotone in Y.
+__device__ __forceinline__ int resize_first(int target, int n_out, float scale) {   // first Y with floor(Y * scale) >= target
+  int lo = 0, hi = n_out;
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if ((int)floorf(__fmul_rn((float)mid, scale)) >= target) hi = mid;
+    else lo = mid + 1;
+  }
+  return lo;
+}
+
+__global__ void resize_bilinear_bwd_gather_kernel(const float* __restrict__ dy, float* __restrict__ dx, int N, int h, int w,
+                                                  int C, int oh, int ow) {
+  long long total = (long long)N * h * w * C;
+  float sy = (float)h / (float)oh, sx = (float)w / (float)ow;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const int c = (int)(i % C);
+    long long t = i / C;
+    const int x = (int)(t % w);
+    t /= w;
+    const int y = (int)(t % h);
+    const int n = (int)(t / h);
+    const int Y0 = resize_first(y - 1, oh, sy), Y1 = resize_first(y + 1, oh, sy);
+    const int X0 = resize_first(x - 1, ow, sx), X1 = resize_first(x + 1, ow, sx);
+    const float* g0 = dy + (long long)n * oh * ow * C + c;
+    float s = 0.f;
+    for (int Y = Y0; Y < Y1; ++Y) {
+      const float fy = __fmul_rn((float)Y, sy);
+      const int y0 = (int)floorf(fy), y1 = min(y0 + 1, h - 1);
+      const float wy = __fsub_rn(fy, (float)y0);
+      for (int X = X0; X < X1; ++X) {
+        const float fx = __fmul_rn((float)X, sx);
+        const int x0 = (int)floorf(fx), x1 = min(x0 + 1, w - 1);
+        const float wx = __fsub_rn(fx, (float)x0);
+        const float g = g0[((long long)Y * ow + X) * C];
+        if (y0 == y && x0 == x) s = __fadd_rn(s, __fmul_rn(__fmul_rn(g, 1.f - wy), 1.f - wx));
+        if (y0 == y && x1 == x) s = __fadd_rn(s, __fmul_rn(__fmul_rn(g, 1.f - wy), wx));
+        if (y1 == y && x0 == x) s = __fadd_rn(s, __fmul_rn(__fmul_rn(g, wy), 1.f - wx));
+        if (y1 == y && x1 == x) s = __fadd_rn(s, __fmul_rn(__fmul_rn(g, wy), wx));
+      }
+    }
+    dx[i] = s;
+  }
+}
+
 // ---- fused feedback: flow_lr -> (symmetric pad, x4, upscale_four) -> warp(pre_gen) -> s2d into dst.
 // CTA tile = 2 LR rows x 32 LR columns (8 x 128 HR pixels); one thread per (LR pixel, dy): 4 HR pixels x 3 channels
 // = 12 contiguous destination values.  The HR flow inside the tile is a convex combination of the 3 x 33 LR flow
@@ -652,6 +796,54 @@ int teco_warp_bwd_f32(const float* img, const float* flow, const float* dout, fl
   TECO_CHECK_ARG(img && flow && dout, "teco_warp_bwd_f32: NULL tensor");
   TECO_CHECK_ARG(N > 0 && H >= 2 && W >= 2 && C > 0, "teco_warp_bwd_f32: bad shape");
   LAUNCH1D(warp_bwd_f32_kernel, (long long)N * H * W, img, flow, dout, dimg, dflow, N, H, W, C);
+  return TECO_OK;
+}
+
+}  // extern "C"
+// Fixed-order gradients (DESIGN.md section 4.3).  Workspace of teco_warp_bwd_f32_det: int32 cnt[P], off[P], list[4P] and
+// bsum[ceil(P / 1024)] for P = N * H * W pixels.
+namespace {
+long long warp_det_ints(long long P) { return 6 * P + (P + WD_SCAN - 1) / WD_SCAN; }
+}  // namespace
+
+extern "C" {
+
+int teco_warp_bwd_f32_det_plan_bytes(int32_t N, int32_t H, int32_t W, int64_t* ws_bytes_host) {
+  TECO_CHECK_ARG(ws_bytes_host && N > 0 && H >= 2 && W >= 2 && 4LL * N * H * W < (1LL << 31),
+                 "teco_warp_bwd_f32_det_plan_bytes: bad shape");
+  *ws_bytes_host = warp_det_ints((long long)N * H * W) * (int64_t)sizeof(int);
+  return TECO_OK;
+}
+
+int teco_warp_bwd_f32_det(const float* img, const float* flow, const float* dout, float* dimg, float* dflow, int32_t N,
+                          int32_t H, int32_t W, int32_t C, void* ws, int64_t ws_bytes, void* stream) {
+  TECO_CHECK_ARG(img && flow && dout, "teco_warp_bwd_f32_det: NULL tensor");
+  TECO_CHECK_ARG(N > 0 && H >= 2 && W >= 2 && C > 0 && 4LL * N * H * W < (1LL << 31), "teco_warp_bwd_f32_det: bad shape");
+  const long long P = (long long)N * H * W;
+  TECO_CHECK_ARG(!dimg || (ws && ws_bytes >= warp_det_ints(P) * (long long)sizeof(int) && (((uintptr_t)ws) & 15) == 0),
+                 "teco_warp_bwd_f32_det: workspace of %lld bytes (16-byte aligned) needed, got %lld",
+                 warp_det_ints(P) * (long long)sizeof(int), (long long)ws_bytes);
+  if (dflow) { LAUNCH1D(warp_bwd_f32_kernel, P, img, flow, dout, nullptr, dflow, N, H, W, C); }
+  if (!dimg) return TECO_OK;
+  int* cnt = (int*)ws;
+  int* off = cnt + P;
+  int* list = off + P;
+  int* bsum = list + 4 * P;
+  const int chunks = (int)((P + WD_SCAN - 1) / WD_SCAN);
+  TECO_CUDA_CALL(cudaMemsetAsync(cnt, 0, sizeof(int) * (size_t)P, (cudaStream_t)stream));
+  LAUNCH1D(warp_det_count_kernel, P, flow, cnt, N, H, W);
+  warp_det_scan_chunks_kernel<<<chunks, WD_SCAN, 0, (cudaStream_t)stream>>>(cnt, off, bsum, P);
+  warp_det_scan_totals_kernel<<<1, WD_SCAN, 0, (cudaStream_t)stream>>>(bsum, chunks);
+  TECO_CUDA_LAUNCH_CHECK("teco_warp_bwd_f32_det(scan)");
+  LAUNCH1D(warp_det_place_kernel, P, flow, cnt, off, bsum, list, N, H, W);
+  LAUNCH1D(warp_det_gather_kernel, P, flow, dout, off, bsum, list, dimg, N, H, W, C);
+  return TECO_OK;
+}
+
+int teco_resize_bilinear_bwd_f32_det(const float* dy, float* dx, int32_t N, int32_t h, int32_t w, int32_t C, int32_t oh,
+                                     int32_t ow, void* stream) {
+  TECO_CHECK_ARG(dy && dx && N > 0 && h > 0 && w > 0 && C > 0 && oh > 0 && ow > 0, "teco_resize_bilinear_bwd_f32_det: bad argument");
+  LAUNCH1D(resize_bilinear_bwd_gather_kernel, (long long)N * h * w * C, dy, dx, N, h, w, C, oh, ow);
   return TECO_OK;
 }
 

@@ -98,3 +98,5 @@ __device__ __forceinline__ int cta_exclusive_scan(int v, int* sm /* NT/32 + 1 in
 }
 
 int teco_sm_count();
+// out[e] (+)= part[0][e] + ... + part[S-1][e] for e < E, summed in split order (eltwise.cu).  S >= 1.
+int teco_reduce_splits(const float* part, int S, long long E, float* out, int accumulate, cudaStream_t stream);

@@ -2,9 +2,12 @@
 hand-written kernels; torch.autograd.Function is used only as the tape that strings them together for
 BPTT (plumbing).  All tensors are contiguous NHWC fp32 CUDA tensors unless stated otherwise.
 """
+import ctypes
+
 import torch
 
 from . import _ffi as F
+from . import config
 from ._ffi import ACT_NONE, ACT_RELU, ACT_LRELU02, ACT_TANH24, ACT_SIGMOID, ConvDesc, TcDesc, call, ptr, stream_ptr
 
 f32 = torch.float32
@@ -20,6 +23,26 @@ def same_pad(n, k, s):
 
 def _cc(t):
     return t if t.is_contiguous() else t.contiguous()
+
+
+# ------------------------------------------------------------------------------------------ fixed-order mode
+def plan_bytes(name, *args):
+    """Workspace bytes of fixed-order entry points: `name`_plan_bytes(*args, &bytes), host only."""
+    n = ctypes.c_int64(0)
+    call(name + "_plan_bytes", *args, ctypes.byref(n))
+    return n.value
+
+
+def det_workspace(nbytes, device):
+    """Workspace of a *_det call from the caching allocator (so CUDA-graph capture keeps working); 16-byte aligned."""
+    return torch.empty(max(int(nbytes), 16), device=device, dtype=torch.uint8)
+
+
+def _det_call(name, plan, device, *args):
+    """name(*args, ws, ws_bytes, stream) with a workspace of the size plan_bytes(*plan) gives."""
+    nb = plan_bytes(*plan)
+    ws = det_workspace(nb, device)
+    call(name, *args, ptr(ws), nb, stream_ptr())
 
 
 # ------------------------------------------------------------------------------------------ raw launches
@@ -46,6 +69,10 @@ def conv2d_wgrad_raw(x, dy, dw, db, *, stride, pad_t, pad_l, OH, OW, out_map=(1,
     d = ConvDesc(N=N, H=H, W=W, Cin=Cin, OH=OH, OW=OW, Cout=Cout, KH=KH, KW=KW, stride=stride, pad_t=pad_t, pad_l=pad_l,
                  out_H=dy.shape[1], out_W=dy.shape[2], out_sy=out_map[0], out_oy=out_map[1], out_sx=out_map[2],
                  out_ox=out_map[3], in_cpitch=Cp, out_cpitch=dy.shape[3], act=0, post_scale=1.0, post_shift=0.0)
+    if config.deterministic():
+        _det_call("teco_conv2d_wgrad_f32_det", ("teco_conv2d_wgrad_f32_det", d, int(db is not None)), x.device, d,
+                  ptr(x, f32), ptr(dy, f32), ptr(dw, f32), ptr(db, f32), int(accumulate))
+        return
     call("teco_conv2d_wgrad_f32", d, ptr(x, f32), ptr(dy, f32), ptr(dw, f32), ptr(db, f32), int(accumulate), stream_ptr())
 
 
@@ -240,7 +267,8 @@ class _ResizeBilinear(torch.autograd.Function):
     def backward(ctx, dy):
         N, h, w, C, oh, ow = ctx.shape
         dx = torch.empty((N, h, w, C), device=dy.device, dtype=f32)
-        call("teco_resize_bilinear_bwd_f32", ptr(_cc(dy), f32), ptr(dx, f32), N, h, w, C, oh, ow, stream_ptr())
+        name = "teco_resize_bilinear_bwd_f32_det" if config.deterministic() else "teco_resize_bilinear_bwd_f32"
+        call(name, ptr(_cc(dy), f32), ptr(dx, f32), N, h, w, C, oh, ow, stream_ptr())
         return dx, None, None
 
 
@@ -265,8 +293,13 @@ class _Warp(torch.autograd.Function):
     def backward(ctx, dout):
         img, flow = ctx.saved_tensors
         N, H, W, C = img.shape
-        dimg = torch.zeros_like(img) if ctx.needs_input_grad[0] else None
         dflow = torch.empty_like(flow) if ctx.needs_input_grad[1] else None
+        if config.deterministic():     # dimg is stored, not added to
+            dimg = torch.empty_like(img) if ctx.needs_input_grad[0] else None
+            _det_call("teco_warp_bwd_f32_det", ("teco_warp_bwd_f32_det", N, H, W), img.device, ptr(img, f32),
+                      ptr(flow, f32), ptr(_cc(dout), f32), ptr(dimg, f32), ptr(dflow, f32), N, H, W, C)
+            return dimg, dflow
+        dimg = torch.zeros_like(img) if ctx.needs_input_grad[0] else None
         call("teco_warp_bwd_f32", ptr(img, f32), ptr(flow, f32), ptr(_cc(dout), f32), ptr(dimg, f32), ptr(dflow, f32),
              N, H, W, C, stream_ptr())
         return dimg, dflow
@@ -311,7 +344,12 @@ class _BNTrain(torch.autograd.Function):
         npix = x.numel() // C
         y = torch.empty_like(x)
         stats = torch.empty(4 * C, device=x.device, dtype=f32)
-        call("teco_bn_train_f32", ptr(x, f32), ptr(beta, f32), ptr(y, f32), ptr(stats, f32), npix, C, 1e-3, int(lrelu), stream_ptr())
+        if config.deterministic():
+            _det_call("teco_bn_train_f32_det", ("teco_bn_det", npix, C), x.device, ptr(x, f32), ptr(beta, f32), ptr(y, f32),
+                      ptr(stats, f32), npix, C, 1e-3, int(lrelu))
+        else:
+            call("teco_bn_train_f32", ptr(x, f32), ptr(beta, f32), ptr(y, f32), ptr(stats, f32), npix, C, 1e-3, int(lrelu),
+                 stream_ptr())
         ctx.lrelu = lrelu
         ctx.save_for_backward(x, y, stats)
         return y
@@ -323,8 +361,12 @@ class _BNTrain(torch.autograd.Function):
         npix = x.numel() // C
         dx = torch.empty_like(x)
         dbeta2 = torch.empty(2 * C, device=x.device, dtype=f32)
-        call("teco_bn_train_bwd_f32", ptr(x, f32), ptr(y, f32), ptr(_cc(dy), f32), ptr(stats, f32), ptr(dx, f32),
-             ptr(dbeta2, f32), npix, C, 1e-3, int(ctx.lrelu), stream_ptr())
+        if config.deterministic():
+            _det_call("teco_bn_train_bwd_f32_det", ("teco_bn_det", npix, C), x.device, ptr(x, f32), ptr(y, f32),
+                      ptr(_cc(dy), f32), ptr(stats, f32), ptr(dx, f32), ptr(dbeta2, f32), npix, C, 1e-3, int(ctx.lrelu))
+        else:
+            call("teco_bn_train_bwd_f32", ptr(x, f32), ptr(y, f32), ptr(_cc(dy), f32), ptr(stats, f32), ptr(dx, f32),
+                 ptr(dbeta2, f32), npix, C, 1e-3, int(ctx.lrelu), stream_ptr())
         return dx, dbeta2[:C].clone(), None
 
 
@@ -334,6 +376,13 @@ def batchnorm_train(x, beta, lrelu=False):
 
 
 # ------------------------------------------------------------------------------------------ losses (value + fused grad)
+def _loss_call(name, npix, C, device, *args):
+    if config.deterministic():
+        _det_call(name + "_det", ("teco_loss_det", npix, C), device, *args)
+    else:
+        call(name, *args, stream_ptr())
+
+
 class _LossL2(torch.autograd.Function):
     @staticmethod
     def forward(ctx, a, b):
@@ -341,7 +390,8 @@ class _LossL2(torch.autograd.Function):
         C = a.shape[-1]
         out = torch.empty(1, device=a.device, dtype=f32)
         da = torch.empty_like(a) if (ctx.needs_input_grad[0] or ctx.needs_input_grad[1]) else None
-        call("teco_loss_l2_f32", ptr(a, f32), ptr(b, f32), ptr(out, f32), ptr(da, f32), a.numel() // C, C, 1.0, stream_ptr())
+        _loss_call("teco_loss_l2_f32", a.numel() // C, C, a.device, ptr(a, f32), ptr(b, f32), ptr(out, f32), ptr(da, f32),
+                   a.numel() // C, C, 1.0)
         ctx.save_for_backward(da)
         return out[0]
 
@@ -364,8 +414,8 @@ class _LossL1(torch.autograd.Function):
         C = a.shape[-1]
         out = torch.empty(1, device=a.device, dtype=f32)
         da = torch.empty_like(a) if (ctx.needs_input_grad[0] or ctx.needs_input_grad[1]) else None
-        call("teco_loss_l1_f32", ptr(a, f32), ptr(b, f32), ptr(out, f32), ptr(da, f32), ptr(None), a.numel() // C, C,
-             int(per_pixel), 1.0, stream_ptr())
+        _loss_call("teco_loss_l1_f32", a.numel() // C, C, a.device, ptr(a, f32), ptr(b, f32), ptr(out, f32), ptr(da, f32),
+                   ptr(None), a.numel() // C, C, int(per_pixel), 1.0)
         ctx.save_for_backward(da)
         return out[0]
 
@@ -388,7 +438,8 @@ class _LossCos(torch.autograd.Function):
         C = f.shape[-1]
         out = torch.empty(1, device=f.device, dtype=f32)
         df = torch.empty_like(f) if ctx.needs_input_grad[0] else None
-        call("teco_loss_cosine_f32", ptr(f, f32), ptr(g, f32), ptr(out, f32), ptr(df, f32), f.numel() // C, C, 1.0, stream_ptr())
+        _loss_call("teco_loss_cosine_f32", f.numel() // C, C, f.device, ptr(f, f32), ptr(g, f32), ptr(out, f32), ptr(df, f32),
+                   f.numel() // C, C, 1.0)
         ctx.save_for_backward(df)
         return out[0]
 
@@ -410,8 +461,8 @@ class _LossGAN(torch.autograd.Function):
         d_fake, d_real = _cc(d_fake), _cc(d_real)
         out = torch.empty(5, device=d_fake.device, dtype=f32)
         g_adv, g_f, g_r = torch.empty_like(d_fake), torch.empty_like(d_fake), torch.empty_like(d_real)
-        call("teco_loss_gan_f32", ptr(d_fake, f32), ptr(d_real, f32), ptr(out, f32), ptr(g_adv, f32), ptr(g_f, f32),
-             ptr(g_r, f32), d_fake.numel(), eps, 1.0, 1.0, stream_ptr())
+        _loss_call("teco_loss_gan_f32", d_fake.numel(), 1, d_fake.device, ptr(d_fake, f32), ptr(d_real, f32), ptr(out, f32),
+                   ptr(g_adv, f32), ptr(g_f, f32), ptr(g_r, f32), d_fake.numel(), eps, 1.0, 1.0)
         ctx.save_for_backward(g_adv, g_f, g_r)
         return out
 
@@ -542,6 +593,16 @@ def to_u8(x01):
     y = torch.empty(x01.shape, device=x01.device, dtype=torch.uint8)
     call("teco_to_u8", ptr(_cc(x01), f32), ptr(y, torch.uint8), x01.numel(), stream_ptr())
     return y
+
+
+def sum_ranks(src, out=None):
+    """out[e] = src[0][e] + src[1][e] + ... in row order (teco_sum_ranks_f32): the fixed-order sum over ranks."""
+    src = _cc(src)
+    R = src.shape[0]
+    if out is None:
+        out = torch.empty(src.shape[1:], device=src.device, dtype=f32)
+    call("teco_sum_ranks_f32", ptr(src, f32), R, out.numel(), ptr(out, f32), stream_ptr())
+    return out
 
 
 def l2norm_channels(f):
@@ -753,6 +814,10 @@ def conv3x3_wgrad_tc(xb, dzb, dw, cin, cout, accumulate=False):
     """dw[3,3,cin,cout] fp32 (+)= sum_p xb[p+tap][ci] dzb[p][co] on wgmma (teco_conv3x3_wgrad_tc); xb / dzb: NHWC bf16 with
     channel counts padded to multiples of 64."""
     N, H, W, cp = xb.shape
+    if config.deterministic():
+        _det_call("teco_conv3x3_wgrad_tc_det", ("teco_conv3x3_wgrad_tc_det", N, H, W, cin, cout), xb.device, N, H, W, cp,
+                  dzb.shape[-1], cin, cout, ptr(xb, bf16), ptr(dzb, bf16), ptr(dw, f32), int(accumulate))
+        return dw
     call("teco_conv3x3_wgrad_tc", N, H, W, cp, dzb.shape[-1], cin, cout, ptr(xb, bf16), ptr(dzb, bf16), ptr(dw, f32),
          int(accumulate), stream_ptr())
     return dw
@@ -762,7 +827,12 @@ def bias_grad(dz, C=None):
     """db[c] = sum over pixels of dz[..., c] (fp32)."""
     C = dz.shape[-1] if C is None else C
     db = torch.empty(C, device=dz.device, dtype=f32)
-    call("teco_bias_grad_f32", ptr(dz, f32), ptr(db, f32), dz.numel() // dz.shape[-1], C, dz.shape[-1], 0, stream_ptr())
+    npix = dz.numel() // dz.shape[-1]
+    if config.deterministic():
+        _det_call("teco_bias_grad_f32_det", ("teco_bias_grad_f32_det", npix, C), dz.device, ptr(dz, f32), ptr(db, f32), npix,
+                  C, dz.shape[-1], 0)
+    else:
+        call("teco_bias_grad_f32", ptr(dz, f32), ptr(db, f32), npix, C, dz.shape[-1], 0, stream_ptr())
     return db
 
 

@@ -20,12 +20,27 @@ def shard_clips(n_clips, rank=None, world_size=None):
     return begin, begin + base + (1 if rank < rem else 0)
 
 
+def gather_ranks(bucket):
+    """[world, n] tensor whose row r is rank r's `bucket` (the same on every rank)."""
+    _, w = world()
+    out = torch.empty((w,) + tuple(bucket.shape), device=bucket.device, dtype=bucket.dtype)
+    dist.all_gather(list(out.unbind(0)), bucket)
+    return out
+
+
 def allreduce_bucket(bucket):
     """Sum `bucket` over all ranks in place (the single collective of a training step).  Returns 1/world, the scale that
-    turns the sums into means (applied inside the fused Adam kernel and to the scalars)."""
+    turns the sums into means (applied inside the fused Adam kernel and to the scalars).  In deterministic mode
+    (config.set_deterministic) the ranks' buckets are gathered and summed in rank order (teco_sum_ranks_f32), so every
+    rank holds the same bits and a rerun at the same rank count reproduces them; otherwise NCCL sums in its own order."""
     _, w = world()
     if w > 1:
-        dist.all_reduce(bucket, op=dist.ReduceOp.SUM)
+        from . import config
+        if config.deterministic():
+            from . import kernels as K
+            K.sum_ranks(gather_ranks(bucket), out=bucket)
+        else:
+            dist.all_reduce(bucket, op=dist.ReduceOp.SUM)
     return 1.0 / w
 
 
