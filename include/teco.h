@@ -178,7 +178,8 @@ int teco_warp_bwd_f32(const float* img, const float* flow, const float* dout, fl
  *   warped  = dense_image_warp(pre_gen, flow_hr)              main.py:215
  *   dst[n,y,x, ch_off + (dy*4+dx)*3 + c] = warped[n,4y+dy,4x+dx,c] * in_scale + in_shift   (space-to-depth 4)
  * pre_gen: [N,4h,4w,3] fp32.  flow_lr: [N,fh,fw,2] fp32 with fh<=h, fw<=w (symmetric-padded to h,w).
- * dst: [N,h,w,dst_cpitch] fp32 (dst_bf16==0) or bf16 (dst_bf16!=0).  warped_out (optional): fp32 [N,4h,4w,3]. */
+ * dst: [N,h,w,dst_cpitch] fp32 (dst_bf16==0) or bf16 (dst_bf16!=0).  warped_out (optional): fp32 [N,4h,4w,3].
+ * A bf16 dst needs ch_off and dst_cpitch multiples of 8, a 16-byte-aligned dst and no warped_out (else TECO_E_INVALID). */
 int teco_warp_s2d_fused(const float* pre_gen, const float* flow_lr, void* dst, float* warped_out,
                         int32_t N, int32_t h, int32_t w, int32_t fh, int32_t fw, int32_t dst_cpitch,
                         int32_t ch_off, int32_t dst_bf16, float in_scale, float in_shift, void* stream);

@@ -239,7 +239,8 @@ __global__ void resize_bilinear_bwd_gather_kernel(const float* __restrict__ dy, 
   }
 }
 
-// ---- fused feedback: flow_lr -> (symmetric pad, x4, upscale_four) -> warp(pre_gen) -> s2d into dst.
+// ---- fused feedback: flow_lr -> (symmetric pad, x4, upscale_four) -> warp(pre_gen) -> s2d into an fp32 dst, optionally
+// with the fp32 warped frame (bf16 destinations run warp_s2d_v2_kernel, warp_s2d_v2.cu).
 // CTA tile = 2 LR rows x 32 LR columns (8 x 128 HR pixels); one thread per (LR pixel, dy): 4 HR pixels x 3 channels
 // = 12 contiguous destination values.  The HR flow inside the tile is a convex combination of the 3 x 33 LR flow
 // samples around it, so their min/max bound every query of the tile: the CTA stages that source window of the
@@ -272,9 +273,8 @@ __device__ __forceinline__ FlowQ load_flow_quad(const float* __restrict__ fb, in
 // Round-2 ncu of the first versions: 227 thread instructions per HR pixel at IPC 2.2 -- the kernel was instruction- and
 // latency-bound, not memory-bound: generic loads through a run-time selected pointer, 64-bit index arithmetic and integer
 // divisions.  This version keeps each address space in its own code path and all per-pixel index arithmetic in 32 bits.
-template <bool kBf16>
 __global__ void __launch_bounds__(TPB, 5)
-warp_s2d_fused_kernel(const float* __restrict__ pre_gen, const float* __restrict__ flow_lr, void* __restrict__ dst,
+warp_s2d_fused_kernel(const float* __restrict__ pre_gen, const float* __restrict__ flow_lr, float* __restrict__ dst,
                       float* __restrict__ warped_out, int N, int h, int w, int fh, int fw, int dst_cpitch, int ch_off,
                       float in_scale, float in_shift) {
   extern __shared__ __align__(16) float win[];
@@ -429,34 +429,8 @@ warp_s2d_fused_kernel(const float* __restrict__ pre_gen, const float* __restrict
   }
   // space-to-depth: element (dy*4 + dx)*3 + c of the 48 channels of LR pixel (ly, lx)
   const size_t o = (((size_t)n * h + min(ly, h - 1)) * w + min(lx, w - 1)) * dst_cpitch + ch_off;
-  if (kBf16) {
-    __nv_bfloat16* d = reinterpret_cast<__nv_bfloat16*>(dst) + o;
-    const bool vec = ((o & 3) == 0);                 // warp-uniform per LR row except through lx; all lanes shuffle anyway
-#pragma unroll
-    for (int dy = 0; dy < 4; ++dy) {
-      const float v0 = vals[dy][0] * in_scale + in_shift, v1 = vals[dy][1] * in_scale + in_shift, v2 = vals[dy][2] * in_scale + in_shift;
-      // the 12 values of (LR pixel, dy) sit in four neighbouring lanes (dx = 0..3): lanes dx = 0,1,2 each write 8 bytes
-      const float n0 = __shfl_down_sync(0xffffffffu, v0, 1), n1 = __shfl_down_sync(0xffffffffu, v1, 1),
-                  n2 = __shfl_down_sync(0xffffffffu, v2, 1);
-      if (!valid) continue;
-      if (vec) {
-        if (dx < 3) {
-          const float e0 = dx == 0 ? v0 : (dx == 1 ? v1 : v2), e1 = dx == 0 ? v1 : (dx == 1 ? v2 : n0),
-                      e2 = dx == 0 ? v2 : (dx == 1 ? n0 : n1), e3 = dx == 0 ? n0 : (dx == 1 ? n1 : n2);
-          __nv_bfloat162 a = __floats2bfloat162_rn(e0, e1), c = __floats2bfloat162_rn(e2, e3);
-          uint2 u;
-          u.x = *reinterpret_cast<uint32_t*>(&a);
-          u.y = *reinterpret_cast<uint32_t*>(&c);
-          *reinterpret_cast<uint2*>(d + dy * 12 + dx * 4) = u;
-        }
-      } else {
-        d[dy * 12 + dx * 3 + 0] = __float2bfloat16_rn(v0);
-        d[dy * 12 + dx * 3 + 1] = __float2bfloat16_rn(v1);
-        d[dy * 12 + dx * 3 + 2] = __float2bfloat16_rn(v2);
-      }
-    }
-  } else if (valid) {
-    float* d = reinterpret_cast<float*>(dst) + o;
+  if (valid) {
+    float* d = dst + o;
 #pragma unroll
     for (int dy = 0; dy < 4; ++dy) {
       d[dy * 12 + dx * 3 + 0] = vals[dy][0] * in_scale + in_shift;
@@ -848,8 +822,7 @@ int teco_resize_bilinear_bwd_f32_det(const float* dy, float* dx, int32_t N, int3
 }
 
 }  // extern "C"
-// warp_s2d_v2.cu: the low-instruction-count version for the inference layout (bf16 destination, aligned channel offset)
-bool teco_warp_s2d_v2_applicable(const void* dst, int dst_cpitch, int ch_off, int dst_bf16, const float* warped_out);
+// warp_s2d_v2.cu: the kernel for bf16 destinations
 int teco_warp_s2d_v2_launch(const float* pre_gen, const float* flow_lr, void* dst, int N, int h, int w, int fh, int fw,
                             int dst_cpitch, int ch_off, float in_scale, float in_shift, cudaStream_t stream);
 extern "C" {
@@ -863,29 +836,28 @@ int teco_warp_s2d_fused(const float* pre_gen, const float* flow_lr, void* dst, f
   TECO_CHECK_ARG(ch_off >= 0 && ch_off + 48 <= dst_cpitch, "teco_warp_s2d_fused: 48 channels do not fit at ch_off=%d in pitch %d",
                  ch_off, dst_cpitch);
   TECO_CHECK_ARG((((uintptr_t)pre_gen) & 15) == 0, "teco_warp_s2d_fused: pre_gen must be 16-byte aligned");
-  const char* v2_env = getenv("TECO_WARP_V2");                 // A/B switch, read per call: "0" selects the first version
-  if ((!v2_env || v2_env[0] != '0') && teco_warp_s2d_v2_applicable(dst, dst_cpitch, ch_off, dst_bf16, warped_out))
+  if (dst_bf16) {
+    // warp_s2d_v2_kernel writes the 48 channels of each LR pixel as six 16-byte stores
+    TECO_CHECK_ARG(!warped_out, "teco_warp_s2d_fused: warped_out needs an fp32 dst");
+    TECO_CHECK_ARG(ch_off % 8 == 0, "teco_warp_s2d_fused: a bf16 dst needs ch_off %% 8 == 0, got %d", ch_off);
+    TECO_CHECK_ARG(dst_cpitch % 8 == 0, "teco_warp_s2d_fused: a bf16 dst needs dst_cpitch %% 8 == 0, got %d", dst_cpitch);
+    TECO_CHECK_ARG((((uintptr_t)dst) & 15) == 0, "teco_warp_s2d_fused: a bf16 dst must be 16-byte aligned");
     return teco_warp_s2d_v2_launch(pre_gen, flow_lr, dst, N, h, w, fh, fw, dst_cpitch, ch_off, in_scale, in_shift,
                                    (cudaStream_t)stream);
+  }
   const int tiles_x = teco_ceil_div(w, WS_TLW), tiles_y = teco_ceil_div(h, WS_TLH);
   TECO_CHECK_ARG(tiles_y <= 65535 && N <= 65535, "teco_warp_s2d_fused: more than 65535 row bands or images");
   const size_t smem = WS_SMEM_FLOATS * sizeof(float);
   static bool attr = false;
   if (!attr) {
-    TECO_CUDA_CALL(cudaFuncSetAttribute(warp_s2d_fused_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    TECO_CUDA_CALL(cudaFuncSetAttribute(warp_s2d_fused_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    TECO_CUDA_CALL(cudaFuncSetAttribute(warp_s2d_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     attr = true;
   }
   // the 4-float stores of warped_out need 16-byte alignment of every (row, 4*lx) start: W*3 floats per row, 4*lx*3 = 12 lx
   TECO_CHECK_ARG(!warped_out || ((((uintptr_t)warped_out) & 15) == 0), "teco_warp_s2d_fused: warped_out must be 16-byte aligned");
-  TECO_CHECK_ARG((((uintptr_t)pre_gen) & 15) == 0, "teco_warp_s2d_fused: pre_gen must be 16-byte aligned");
   const dim3 grid((unsigned)tiles_x, (unsigned)tiles_y, (unsigned)N);
-  if (dst_bf16)
-    warp_s2d_fused_kernel<true><<<grid, TPB, smem, (cudaStream_t)stream>>>(pre_gen, flow_lr, dst, warped_out, N, h, w, fh, fw, dst_cpitch,
-                                                                          ch_off, in_scale, in_shift);
-  else
-    warp_s2d_fused_kernel<false><<<grid, TPB, smem, (cudaStream_t)stream>>>(pre_gen, flow_lr, dst, warped_out, N, h, w, fh, fw, dst_cpitch,
-                                                                           ch_off, in_scale, in_shift);
+  warp_s2d_fused_kernel<<<grid, TPB, smem, (cudaStream_t)stream>>>(pre_gen, flow_lr, (float*)dst, warped_out, N, h, w, fh, fw,
+                                                                   dst_cpitch, ch_off, in_scale, in_shift);
   TECO_CUDA_LAUNCH_CHECK("teco_warp_s2d_fused");
   return TECO_OK;
 }

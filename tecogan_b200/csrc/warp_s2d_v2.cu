@@ -1,10 +1,9 @@
-// warp_s2d_v2.cu -- second version of the fused feedback kernel for the inference layout (bf16 destination inside the packed
-// 64-channel generator input, no fp32 copy of the warped frame):
+// warp_s2d_v2.cu -- second version of the fused feedback kernel, the one for bf16 destinations (the packed 64-channel
+// generator input: channel offset and pitch multiples of 8, no fp32 copy of the warped frame):
 //   flow_lr -> symmetric pad, x4, upscale_four -> dense_image_warp(previous HR output) -> space_to_depth
 // (reference main.py:201,212-215; lib/ops.py:126-163 upscale_four; tf.contrib.image.dense_image_warp).  Same arithmetic,
-// formula for formula, as warp_s2d_fused_kernel in resample.cu (which keeps every other layout: fp32 destinations,
-// warped_out, unaligned channel offsets); what changes is the instruction count per HR pixel (the first version is
-// issue-bound, not memory-bound).  Here:
+// formula for formula, as warp_s2d_fused_kernel in resample.cu (which keeps fp32 destinations and warped_out); what
+// changes is the instruction count per HR pixel (the first version is issue-bound, not memory-bound).  Here:
 //   * CTA tile 4 x 32 LR pixels (16 x 128 HR): the per-tile work (flow bound, window set-up, barriers) is paid once per 2048
 //     HR pixels instead of 1024, and the staged source window carries 2 halo rows per 16 instead of per 8;
 //   * the 5 x 33 flow samples of the tile are parked in shared memory once (no thread repeats the symmetric-pad index
@@ -15,9 +14,9 @@
 //   * floor() is ONE add with round-toward-minus-infinity against 1.5 * 2^23 (the sum's mantissa is the integer), the index
 //     arithmetic works directly on that bit pattern (two IMADs per pixel), clamps only on the axes whose tile can touch one;
 //   * results go through a bf16 staging tile in shared memory in destination order and leave as 16-byte stores, six per LR
-//     pixel (was: three shuffles, eight selects and an 8-byte store per HR pixel with a quarter of the lanes idle);
+//     pixel;
 //   * rough motion (window larger than the 40 KB stage): the tile in two halves with their own windows, then an L1 gather.
-// The output is bit-identical to the first version's.
+// The output is the first version's fp32 output rounded to bf16 (round to nearest even), bit for bit.
 #include "teco_common.cuh"
 #include "tc_ptx.cuh"
 
@@ -282,11 +281,7 @@ warp_s2d_v2_kernel(const float* __restrict__ pre_gen, const float* __restrict__ 
 
 }  // namespace
 
-// Called by teco_warp_s2d_fused (resample.cu) for the layouts this version covers.  Returns false when it does not apply.
-bool teco_warp_s2d_v2_applicable(const void* dst, int dst_cpitch, int ch_off, int dst_bf16, const float* warped_out) {
-  return dst_bf16 && !warped_out && (ch_off & 7) == 0 && (dst_cpitch & 7) == 0 && ((uintptr_t)dst & 15) == 0;
-}
-
+// Called by teco_warp_s2d_fused (resample.cu) for bf16 destinations, after it has checked their layout.
 int teco_warp_s2d_v2_launch(const float* pre_gen, const float* flow_lr, void* dst, int N, int h, int w, int fh, int fw,
                             int dst_cpitch, int ch_off, float in_scale, float in_shift, cudaStream_t stream) {
   const size_t smem = V2_WIN_FLOATS * sizeof(float) + V2_STAGE_BYTES + sizeof(V2Smem);

@@ -753,7 +753,8 @@ def resize2x_bf16(x):
 
 def warp_s2d_fused(pre_gen, flow_lr, dst, ch_off, in_scale=1.0, in_shift=0.0, warped_out=None):
     """Fused feedback kernel (teco_warp_s2d_fused): pre_gen [N,4h,4w,3] fp32, flow_lr [N,fh,fw,2] fp32,
-    dst [N,h,w,Cp] fp32 or bf16."""
+    dst [N,h,w,Cp] fp32 or bf16.  A bf16 dst needs ch_off and Cp multiples of 8, 16-byte alignment and no warped_out;
+    other bf16 layouts raise ValueError."""
     N, h, w, Cp = dst.shape
     call("teco_warp_s2d_fused", ptr(pre_gen, f32), ptr(flow_lr, f32), ptr(dst), ptr(warped_out, f32), N, h, w,
          flow_lr.shape[1], flow_lr.shape[2], Cp, ch_off, int(dst.dtype == bf16), float(in_scale), float(in_shift), stream_ptr())

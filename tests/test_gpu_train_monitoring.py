@@ -1,7 +1,7 @@
 """GPU: training monitoring -- Network.train.evaluate (the training graph's forward on a validation batch, reference
 main.py:299-304,391-402) against the goldens, the oracle and the training step itself; evaluation leaves training
 untouched; and main.py --mode train --summary_dir end to end (event file, logfile.txt, validation block, test-sequence
-frames, and the same checkpoint as a run without monitoring).
+frames, and, with --deterministic, the same checkpoint bit for bit as a run without monitoring).
 
 The loss and BatchNorm reductions and the weight gradients accumulate with fp32 atomics, so two executions of the same
 forward agree to rounding, not necessarily to the bit: values a run COMPUTES are compared at rounding tolerances, while
@@ -219,9 +219,11 @@ def _main(cwd, *args):
 
 def test_main_train_with_summary_dir_end_to_end(tmp_path):
     _write_calendar(str(tmp_path))
-    common = ["--mode", "train", "--synthetic_data", "--max_iter", "4", "--summary_freq", "2", "--save_freq", "4",
-              "--display_freq", "2", "--crop_size", "16", "--batch_size", "1", "--RNN_N", "3", "--num_resblock", "2",
-              "--output_ext", "png"]
+    # fixed-order reductions: a run's training is a function of its inputs alone, so monitoring must leave it bit for bit
+    # as it is (in the default mode the fp32 atomics let two runs drift apart over the steps, monitored or not)
+    common = ["--mode", "train", "--deterministic", "--synthetic_data", "--max_iter", "4", "--summary_freq", "2",
+              "--save_freq", "4", "--display_freq", "2", "--crop_size", "16", "--batch_size", "1", "--RNN_N", "3",
+              "--num_resblock", "2", "--output_ext", "png"]
     out1 = _main(str(tmp_path), *common, "--output_dir", "run1", "--summary_dir", "summ")
     out2 = _main(str(tmp_path), *common, "--output_dir", "run2")
 
@@ -270,16 +272,5 @@ def test_main_train_with_summary_dir_end_to_end(tmp_path):
     m1 = torch.load(str(tmp_path / "run1" / "model-4.pt"))
     m2 = torch.load(str(tmp_path / "run2" / "model-4.pt"))
     assert set(m1) == set(m2)
-    lr = 1e-4
-    bit = True
     for k in m1:
-        a, b = m1[k], m2[k]
-        bit = bit and torch.equal(a, b)
-        if not a.is_floating_point():
-            assert torch.equal(a, b), k                       # global_step, Adam step counts, D counters
-        elif k.endswith("/Adam") or k.endswith("/Adam_1") or k.startswith("teco_b200/"):
-            torch.testing.assert_close(a, b, rtol=1e-3, atol=1e-2 * a.abs().max().item() + 1e-12)
-        else:
-            d = (a - b).abs()
-            assert d.max().item() < 5.0 * lr and (d < 0.05 * lr).float().mean().item() > 0.97, (k, d.max().item())
-    print("model-4.pt with and without monitoring bit-identical: %s" % bit)
+        assert torch.equal(m1[k], m2[k]), k

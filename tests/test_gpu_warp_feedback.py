@@ -124,19 +124,33 @@ def _run(pre, flow, shape, dtype, ch_off, scale, warped=False):
     return dst.cpu(), (wout.cpu() if warped else None)
 
 
-# bf16 layouts: (pitch, ch_off, taken by v2 unless TECO_WARP_V2=0).  v1 stores 8 bytes where the element offset is a multiple
-# of 4 (pitch 64, offset 4) and single values elsewhere (pitch 51, offset 3: both kinds from pixel to pixel).
-BF16_LAYOUTS = ((64, 0, True), (64, 8, True), (128, 16, True), (64, 4, False), (51, 3, False))
+def _refused(pre, flow, shape, dtype, ch_off, warped=False, dst_elem_off=0):
+    """teco_warp_s2d_fused refuses the layout with ValueError and writes nothing.  dst_elem_off: dst starts that many
+    elements into its buffer."""
+    from tecogan_b200 import kernels as K
+    buf = torch.full((int(np.prod(shape)) + dst_elem_off,), SENTINEL, dtype=dtype, device="cuda")
+    wout = torch.full(pre.shape, SENTINEL, device="cuda") if warped else None
+    with pytest.raises(ValueError, match="teco_warp_s2d_fused: .*(bf16 dst|warped_out)"):
+        K.warp_s2d_fused(pre, flow, buf[dst_elem_off:].view(shape), ch_off, warped_out=wout)
+    torch.cuda.synchronize()
+    sent = torch.full((1,), SENTINEL, dtype=dtype)
+    assert (_bits(buf.cpu()) == _bits(sent)).all(), (shape, ch_off, "dst written")
+    assert wout is None or (wout == SENTINEL).all(), (shape, ch_off, "warped_out written")
+
+
+# bf16 layouts (pitch, ch_off): warp_s2d_v2_kernel takes an offset and pitch that are multiples of 8; teco_warp_s2d_fused
+# refuses the others.  fp32 destinations, at any offset and with or without warped_out, run warp_s2d_fused_kernel.
+BF16_LAYOUTS = ((64, 0), (64, 8), (128, 16))
+BF16_REFUSED = ((64, 4), (51, 3), (60, 8))
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("name", list(CASES))
-def test_warp_s2d_matches_float64_reference_bit_for_bit(name, monkeypatch):
-    """v2 and v1 (TECO_WARP_V2=0, read per call) on the same dyadic inputs: each bf16 layout equals the bf16 rounding of the
-    float64 composition bit for bit, v1 equals v2 bit for bit, the fp32 destinations and warped_out equal the float64 values
-    exactly, and no channel outside [ch_off, ch_off + 48) is touched."""
+def test_warp_s2d_matches_float64_reference_and_refuses_unaligned_bf16(name):
+    """Both kernels on the same dyadic inputs: each bf16 layout (v2) equals the bf16 rounding of the float64 composition bit
+    for bit, the fp32 destinations and warped_out (v1) equal the float64 values exactly, no channel outside
+    [ch_off, ch_off + 48) is touched, and the unaligned bf16 layouts are refused without a write."""
     c = CASES[name]
-    monkeypatch.delenv("TECO_WARP_V2", raising=False)
     flow = _flows(name)
     N, fh, fw, _ = flow.shape
     grid = 2.0 ** (-7 if c.lo < 0 else -8)
@@ -150,15 +164,11 @@ def test_warp_s2d_matches_float64_reference_bit_for_bit(name, monkeypatch):
     exp32, exp16 = exp.float(), exp.float().to(torch.bfloat16)
 
     pre, fl_d = torch.from_numpy(img).cuda(), torch.from_numpy(flow).cuda()
-    for pitch, off, v2 in BF16_LAYOUTS:
-        shape = (N, c.h, c.w, pitch)
-        got, _ = _run(pre, fl_d, shape, torch.bfloat16, off, c.scale)
-        _check_dst(got, exp16, off, "%s bf16 pitch %d @%d%s" % (name, pitch, off, " (v2)" if v2 else ""))
-        if v2:
-            monkeypatch.setenv("TECO_WARP_V2", "0")
-            got1, _ = _run(pre, fl_d, shape, torch.bfloat16, off, c.scale)
-            monkeypatch.delenv("TECO_WARP_V2")
-            _assert_bits(got1, got, "%s bf16 pitch %d @%d: v1 vs v2" % (name, pitch, off))
+    for pitch, off in BF16_LAYOUTS:
+        got, _ = _run(pre, fl_d, (N, c.h, c.w, pitch), torch.bfloat16, off, c.scale)
+        _check_dst(got, exp16, off, "%s bf16 pitch %d @%d" % (name, pitch, off))
+    for pitch, off in BF16_REFUSED:
+        _refused(pre, fl_d, (N, c.h, c.w, pitch), torch.bfloat16, off)
     got, wout = _run(pre, fl_d, (N, c.h, c.w, 48), torch.float32, 0, c.scale, warped=True)
     _check_dst(got, exp32, 0, "%s fp32" % name)
     _assert_bits(wout, warped.float(), "%s warped_out" % name)
@@ -167,36 +177,43 @@ def test_warp_s2d_matches_float64_reference_bit_for_bit(name, monkeypatch):
 
 
 @pytest.mark.gpu
-def test_warp_s2d_dispatch_runs_v2_only_on_the_engine_layout(monkeypatch):
-    """The comparisons above compare two kernels: bf16 at an offset and pitch that are multiples of 8 without warped_out
-    runs warp_s2d_v2_kernel, TECO_WARP_V2=0 and every other layout run warp_s2d_fused_kernel."""
+def test_warp_s2d_dispatch_runs_v2_on_bf16_and_v1_on_fp32():
+    """The comparisons here compare two kernels: every accepted bf16 layout runs warp_s2d_v2_kernel and every fp32 one
+    warp_s2d_fused_kernel.  bf16 with warped_out, at an offset or pitch that is not a multiple of 8, or at an address that
+    is not 16-byte aligned raises ValueError and launches nothing."""
     from torch.profiler import ProfilerActivity, profile
-    monkeypatch.delenv("TECO_WARP_V2", raising=False)
     pre = torch.rand(1, 32, 32, 3, device="cuda")
     flow = torch.zeros(1, 8, 8, 2, device="cuda")
 
-    def kernel_run(dtype, pitch, off, warped=False):
+    def kernels(fn):
         with profile(activities=[ProfilerActivity.CUDA]) as prof:
-            _run(pre, flow, (1, 8, 8, pitch), dtype, off, (1.0, 0.0), warped)
-        names = [e.key for e in prof.key_averages() if "warp_s2d" in e.key]
+            fn()
+        return [e.key for e in prof.key_averages() if "warp_s2d" in e.key]
+
+    def kernel_run(dtype, pitch, off, warped=False):
+        names = kernels(lambda: _run(pre, flow, (1, 8, 8, pitch), dtype, off, (1.0, 0.0), warped))
         assert len(names) == 1, names
         return "v2" if "warp_s2d_v2_kernel" in names[0] else "v1"
 
-    for pitch, off, v2 in BF16_LAYOUTS:
-        assert kernel_run(torch.bfloat16, pitch, off) == ("v2" if v2 else "v1"), (pitch, off)
-    assert kernel_run(torch.bfloat16, 64, 0, warped=True) == "v1"
+    for pitch, off in BF16_LAYOUTS:
+        assert kernel_run(torch.bfloat16, pitch, off) == "v2", (pitch, off)
     assert kernel_run(torch.float32, 48, 0) == "v1"
-    monkeypatch.setenv("TECO_WARP_V2", "0")
-    assert kernel_run(torch.bfloat16, 64, 0) == "v1"
+    assert kernel_run(torch.float32, 48, 0, warped=True) == "v1"
+    assert kernel_run(torch.float32, 51, 3) == "v1"
+    refused = [lambda p=p, o=o: _refused(pre, flow, (1, 8, 8, p), torch.bfloat16, o) for p, o in BF16_REFUSED]
+    refused += [lambda: _refused(pre, flow, (1, 8, 8, 64), torch.bfloat16, 0, warped=True),
+                lambda: _refused(pre, flow, (1, 8, 8, 64), torch.bfloat16, 0, dst_elem_off=4)]
+    for fn in refused:
+        assert kernels(fn) == []
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("h,rough", [(256, False), (256, True), (32, False), (32, True)])
-def test_warp_s2d_v1_and_v2_agree_bit_for_bit_on_continuous_inputs(h, rough, monkeypatch):
-    """tools/ab_warp.py's workloads: torch.rand frames and the benchmark's un-rounded motion field, smooth and rough.  v1 and
-    v2 evaluate the same formulas in the same order, so their bf16 outputs are bit-identical.  Both stay within one bf16 ulp
-    of the float64 composition, and v1's fp32 destination and warped_out within the fp32 rounding of the query coordinate."""
-    monkeypatch.delenv("TECO_WARP_V2", raising=False)
+def test_warp_s2d_v1_and_v2_agree_bit_for_bit_on_continuous_inputs(h, rough):
+    """torch.rand frames and the benchmark's un-rounded motion field, smooth and rough.  v1 and v2 evaluate the same
+    formulas in the same order, so v2's bf16 output is v1's fp32 output rounded to nearest even, bit for bit.  v2 stays
+    within one bf16 ulp of the float64 composition, and v1's fp32 destination and warped_out within the fp32 rounding of
+    the query coordinate."""
     N = 2
     g = torch.Generator(device="cuda").manual_seed(h + rough)
     pre = torch.rand(N, 4 * h, 4 * h, 3, device="cuda", generator=g)
@@ -206,10 +223,10 @@ def test_warp_s2d_v1_and_v2_agree_bit_for_bit_on_continuous_inputs(h, rough, mon
         flow = flow + 3.0 * (torch.rand(N, h, h, 2, device="cuda", generator=g) - 0.5)
     flow = flow.contiguous()
     v2, _ = _run(pre, flow, (N, h, h, 64), torch.bfloat16, 0, (0.5, 0.5))
-    monkeypatch.setenv("TECO_WARP_V2", "0")
-    v1, _ = _run(pre, flow, (N, h, h, 64), torch.bfloat16, 0, (0.5, 0.5))
+    v1, _ = _run(pre, flow, (N, h, h, 48), torch.float32, 0, (0.5, 0.5))
     f32, wout = _run(pre, flow, (N, h, h, 48), torch.float32, 0, (1.0, 0.0), warped=True)
-    _assert_bits(v1, v2, "v1 vs v2")
+    _assert_bits(v2[..., :48], v1.to(torch.bfloat16), "v2 vs bf16(v1)")
+    assert (_bits(v2[..., 48:]) == _bits(torch.full((1,), SENTINEL, dtype=torch.bfloat16))).all(), "v2 wrote past 48 channels"
 
     warped = O.dense_image_warp(pre.cpu().double(), O.upscale_four(flow.cpu().double() * 4.0))
     ref = O.space_to_depth4(warped)
