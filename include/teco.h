@@ -80,6 +80,8 @@ int teco_conv2d_wgrad_f32(const teco_conv_desc* d, const float* x, const float* 
  * res (bf16, optional) is added after the activation; out_f32 (optional, [N,H,W,out_f32_c])
  * receives post_scale*(value + res_f32) + post_shift for the first out_f32_c channels
  * (used by the generator's output stage: + bicubic, *2-1  lib/frvsr.py:85-87).
+ * mode 1 (the transposed convolution, y [N,2H,2W,Cout]) takes Cin 64, Cout a multiple of 64 and a bf16 y, with no res
+ * and no out_f32; any other mode-1 launch returns TECO_E_INVALID.
  * ------------------------------------------------------------------------------------- */
 typedef struct teco_tc_desc {
   int32_t N, H, W, Cin, Cout;    /* Cin, Cout: padded channel counts (multiples of 16)       */

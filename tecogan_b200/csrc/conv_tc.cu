@@ -15,15 +15,15 @@
 //   B operand = weights pre-packed on the device as [cin/64][tap][cout][64 cin] bf16 in the same SW128 image, fetched by
 //               1-D bulk copies: once per CTA when the layer's Cout slice fits next to the halo ring (every 64 -> 64 layer),
 //               otherwise with each 64-channel block.
-//   D         = fp32 registers, NT / 2 per thread per accumulator (NT = output channels per CTA: 64, 32 or 16).
-// Transposed conv (stride 2, TF 'SAME', y[i] = sum_j x[j] w[i-2j]) is the same loop with the nine taps routed to four
-// sub-pixel phase accumulators (SURVEY.md A.3) and a 2x interleaving epilogue.
+//   D         = fp32 registers, NT / 2 per thread (NT = output channels per CTA: 64, 32 or 16).
 //
 // Persistent CTAs walk tiles c, c + G, ...; the halo (and weight) ring has two stages, so the TMA of the next 64-channel
 // block or tile is in flight while the warpgroups run the MMAs and the epilogue of the current one.  Layers with one
-// 64-channel input block and 64-channel bf16 output slices (mode 0, or mode 1 without a residual) run on
-// conv3x3_ws_kernel instead: the same MMAs and epilogue arithmetic behind a producer warp, a deeper ring and TMA-staged
-// residuals and stores.
+// 64-channel input block and 64-channel bf16 output slices run on conv3x3_ws_kernel<0> instead: the same MMAs and
+// epilogue arithmetic behind a producer warp, a deeper ring and TMA-staged residuals and stores.
+// The transposed conv (mode 1: stride 2, TF 'SAME', y[i] = sum_j x[j] w[i-2j]) runs only on conv3x3_ws_kernel<1>: the
+// same MMAs with the nine taps routed to four sub-pixel phase accumulators (SURVEY.md A.3) and a 2x interleaving
+// epilogue, for Cin = 64, 64-channel bf16 output slices and no residual.  teco_conv3x3_tc refuses any other mode-1 launch.
 // The fp32 output stage (Cin = 64, Cout = 16, two or three fp32 channels) has its own entry point,
 // teco_conv3x3_f32out_tc, on conv3x3_f32out_kernel: the same MMAs and epilogue arithmetic, pipelined the same way.
 #include <cuda.h>
@@ -102,59 +102,53 @@ __device__ __forceinline__ void mma_issue(float (&acc)[NACC][NT / 2], uint32_t h
   wgmma_commit();
 }
 
-template <int MODE, int NT, int NACC>
-__device__ __forceinline__ void mma_block(float (&acc)[NACC][NT / 2], uint32_t halo_a, uint32_t w_a, int wg) {
-  mma_issue<MODE, NT, NACC>(acc, halo_a, w_a, wg);
+template <int NT>
+__device__ __forceinline__ void mma_block(float (&acc)[1][NT / 2], uint32_t halo_a, uint32_t w_a, int wg) {
+  mma_issue<0, NT, 1>(acc, halo_a, w_a, wg);
   wgmma_wait_all();
 }
 
 // Epilogue of one tile: this thread holds pixels (row 8 wg + 2 wq + i, column lane / 4), channels 8 j + 2 (lane % 4) + {0, 1}
 // of the NT-channel slice starting at n0.  bias points at that slice.
-template <int MODE, int NT, int NACC>
-__device__ __forceinline__ void epilogue(const float (&acc)[NACC][NT / 2], const TcParams& p, const float* bias, int n0, int n,
+template <int NT>
+__device__ __forceinline__ void epilogue(const float (&acc)[NT / 2], const TcParams& p, const float* bias, int n0, int n,
                                          int y0, int x0) {
   const int tid = threadIdx.x, wg = tid >> 7, wq = (tid >> 5) & 3, lane = tid & 31;
-  const int ox_in = x0 + (lane >> 2);
+  const int ox = x0 + (lane >> 2);
 #pragma unroll
   for (int i = 0; i < 2; ++i) {
-    const int oy_in = y0 + 8 * wg + 2 * wq + i;
-    const bool in_img = oy_in < p.H && ox_in < p.W;
+    const int oy = y0 + 8 * wg + 2 * wq + i;
+    const bool in_img = oy < p.H && ox < p.W;
+    const size_t pix = ((size_t)n * p.H + oy) * p.W + ox;
 #pragma unroll
-    for (int ph = 0; ph < NACC; ++ph) {
-      const int OH = MODE == 1 ? 2 * p.H : p.H, OW = MODE == 1 ? 2 * p.W : p.W;
-      const int oy = MODE == 1 ? 2 * oy_in + (ph >> 1) : oy_in, ox = MODE == 1 ? 2 * ox_in + (ph & 1) : ox_in;
-      const size_t pix = ((size_t)n * OH + oy) * OW + ox;
-#pragma unroll
-      for (int j = 0; j < NT / 8; ++j) {
-        const int c = 8 * j + 2 * (lane & 3);
-        float v0 = teco_act(acc[ph][4 * j + 2 * i] + bias[c], p.act);
-        float v1 = teco_act(acc[ph][4 * j + 2 * i + 1] + bias[c + 1], p.act);
-        if (!in_img) continue;
-        if (p.out_f32) {
-          const int C = p.out_f32_c, ch = n0 + c;
-          if (ch < C)
-            p.out_f32[pix * C + ch] = (v0 + (p.res_f32 ? p.res_f32[pix * C + ch] : 0.f)) * p.post_scale + p.post_shift;
-          if (ch + 1 < C)
-            p.out_f32[pix * C + ch + 1] = (v1 + (p.res_f32 ? p.res_f32[pix * C + ch + 1] : 0.f)) * p.post_scale + p.post_shift;
+    for (int j = 0; j < NT / 8; ++j) {
+      const int c = 8 * j + 2 * (lane & 3);
+      float v0 = teco_act(acc[4 * j + 2 * i] + bias[c], p.act);
+      float v1 = teco_act(acc[4 * j + 2 * i + 1] + bias[c + 1], p.act);
+      if (!in_img) continue;
+      if (p.out_f32) {
+        const int C = p.out_f32_c, ch = n0 + c;
+        if (ch < C)
+          p.out_f32[pix * C + ch] = (v0 + (p.res_f32 ? p.res_f32[pix * C + ch] : 0.f)) * p.post_scale + p.post_shift;
+        if (ch + 1 < C)
+          p.out_f32[pix * C + ch + 1] = (v1 + (p.res_f32 ? p.res_f32[pix * C + ch + 1] : 0.f)) * p.post_scale + p.post_shift;
+      }
+      if (p.y) {
+        const size_t o = pix * p.Cout + n0 + c;
+        if (p.res) {   // in-place residual (res == y) is safe: this thread reads the element before it writes it
+          const float2 r = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(p.res + o));
+          v0 += r.x;
+          v1 += r.y;
         }
-        if (p.y) {
-          const size_t o = pix * p.Cout + n0 + c;
-          if (p.res) {   // in-place residual (res == y) is safe: this thread reads the element before it writes it
-            const float2 r = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(p.res + o));
-            v0 += r.x;
-            v1 += r.y;
-          }
-          *reinterpret_cast<__nv_bfloat162*>(p.y + o) = __floats2bfloat162_rn(v0, v1);
-        }
+        *reinterpret_cast<__nv_bfloat162*>(p.y + o) = __floats2bfloat162_rn(v0, v1);
       }
     }
   }
 }
 
-template <int MODE, int NT>
-__global__ void __launch_bounds__(NUM_THREADS, MODE == 1 ? 1 : 2)
+template <int NT>
+__global__ void __launch_bounds__(NUM_THREADS, 2)
 conv3x3_wgmma_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
-  constexpr int NACC = MODE == 1 ? 4 : 1;
   constexpr int NR = NT / 2;                    // accumulator registers per thread
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
@@ -214,25 +208,23 @@ conv3x3_wgmma_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p)
   }
   if (p.resident && nsteps > 0) mbar_wait(smem_u32(w_full), 0);
 
-  float acc[NACC][NR];
+  float acc[1][NR];
   for (int s = 0; s < nsteps; ++s) {
     const int it = s / p.nblk, b = s - it * p.nblk;
     if (tid == 0 && s + 1 < nsteps) issue(s + 1);   // its stage was released by the __syncthreads() closing step s - 1
     if (b == 0) {
 #pragma unroll
-      for (int a = 0; a < NACC; ++a)
-#pragma unroll
-        for (int r = 0; r < NR; ++r) acc[a][r] = 0.f;
+      for (int r = 0; r < NR; ++r) acc[0][r] = 0.f;
     }
     mbar_wait(smem_u32(&full[s & 1]), (uint32_t)((s >> 1) & 1));
     uint8_t* base = ring + (size_t)(s & 1) * p.stage_bytes;
     const uint32_t halo_a = smem_u32(base);
     const uint32_t w_a = p.resident ? smem_u32(w_res + (size_t)b * p.w_blk_bytes) : smem_u32(base + HALO_STAGE);
-    mma_block<MODE, NT, NACC>(acc, halo_a, w_a, wg);
+    mma_block<NT>(acc, halo_a, w_a, wg);
     if (b == p.nblk - 1) {
       int n, y0, x0;
       tile_coords(it, n, y0, x0);
-      epilogue<MODE, NT, NACC>(acc, p, s_bias, n0, n, y0, x0);
+      epilogue<NT>(acc[0], p, s_bias, n0, n, y0, x0);
     }
     __syncthreads();   // every warpgroup's MMAs on this stage have completed: it may be refilled
   }
@@ -691,7 +683,7 @@ conv3x3_im2col_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_con
 // ------------------------------------------------------------------ fp32 output stage (64 -> 2 or 3 channels)
 // Mode 0, Cin = 64, the 16-channel packed Cout slice, an fp32 output of C = 2 or 3 channels with an optional fp32
 // residual and post scale / shift: the generator's output stage (64 -> 3, + bicubic, * 2 - 1) and FNet's flow head
-// (64 -> 2, tanh * 24).  The products are those of conv3x3_wgmma_kernel<0, 16>: per 64-pixel half of the 16 x 8 tile the
+// (64 -> 2, tanh * 24).  The products are those of conv3x3_wgmma_kernel<16>: per 64-pixel half of the 16 x 8 tile the
 // unswapped m64n16k16 of mma_issue, the halo as A and the packed weights as B, taps 0..8 x K-steps 0..3 (scale-d = 0
 // first); the epilogue runs epilogue()'s fp32 operations in its order, so the outputs are bit-identical to
 // teco_conv3x3_tc's.  What differs is the pipeline, after conv3x3_ws_kernel<0>:
@@ -1298,13 +1290,12 @@ int encode_im2col_maps(CUtensorMap* xmap, CUtensorMap* ymap, const void* x, cons
 
 using KernelT = void (*)(const CUtensorMap, const TcParams);
 
-// Mode 1 reaches these instances only with Cin > 64, Cout not a multiple of 64, a residual or an fp32 output; the
-// generator and the bf16 training transposed convolutions (64 -> 64, bf16, no residual) run on conv3x3_ws_kernel<1>.
-KernelT pick_kernel(int mode, int nt) {
-  if (mode == 1) return nt == 32 ? conv3x3_wgmma_kernel<1, 32> : conv3x3_wgmma_kernel<1, 16>;
-  if (nt == 64) return conv3x3_wgmma_kernel<0, 64>;
-  if (nt == 32) return conv3x3_wgmma_kernel<0, 32>;
-  return conv3x3_wgmma_kernel<0, 16>;
+// The mode-0 launches that conv3x3_ws_kernel does not take (Cin > 64, Cout not a multiple of 64 or an fp32 output), NT
+// output channels per CTA
+KernelT pick_kernel(int nt) {
+  if (nt == 64) return conv3x3_wgmma_kernel<64>;
+  if (nt == 32) return conv3x3_wgmma_kernel<32>;
+  return conv3x3_wgmma_kernel<16>;
 }
 
 using WsKernelT = void (*)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const TcParams);
@@ -1345,8 +1336,7 @@ int launch_conv3x3(const teco_tc_desc* d, const void* x, const void* wpk, const 
   p.wpk = (const uint8_t*)wpk; p.bias = bias; p.res = (const __nv_bfloat16*)res; p.y = (__nv_bfloat16*)y;
   p.res_f32 = res_f32; p.out_f32 = out_f32;
   p.nblk = d->Cin / CB;
-  // output channels per CTA: 64, or 32 for the transposed conv, whose four phase accumulators must stay in registers
-  const int nt = (d->Cout % 64 == 0 && d->mode == 0) ? 64 : (d->Cout % 32 == 0 ? 32 : 16);
+  const int nt = d->Cout % 64 == 0 ? 64 : (d->Cout % 32 == 0 ? 32 : 16);   // output channels per CTA
   const int nsplit = d->Cout / nt;
   p.w_blk_bytes = 9u * (uint32_t)nt * 128u;
   p.tiles_x = teco_ceil_div(d->W, TILE_COLS);
@@ -1364,8 +1354,8 @@ int launch_conv3x3(const teco_tc_desc* d, const void* x, const void* wpk, const 
   const int rc = encode_halo_map(&tmap, x, d->N, d->H, d->W, d->Cin, "teco_conv3x3_tc");
   if (rc != TECO_OK) return rc;
   int per_sm = 0;
-  // one K block, 64-channel bf16 output slices, and no residual in mode 1: the warp-specialised kernel
-  const bool ws = p.nblk == 1 && d->Cout % 64 == 0 && !out_f32 && (d->mode == 0 || !res);
+  // one K block and 64-channel bf16 output slices, as every mode-1 launch has: the warp-specialised kernel
+  const bool ws = p.nblk == 1 && d->Cout % 64 == 0 && !out_f32;
   TECO_CHECK_ARG(!d->pool || (ws && d->mode == 0 && !res && d->H >= 2 && d->W >= 2),
                  "teco_conv3x3_tc: pool needs mode 0, Cin 64, Cout a multiple of 64, H, W >= 2 and no residual or fp32 output");
   if (ws) {
@@ -1392,7 +1382,7 @@ int launch_conv3x3(const teco_tc_desc* d, const void* x, const void* wpk, const 
     TECO_CUDA_LAUNCH_CHECK("teco_conv3x3_tc");
     return TECO_OK;
   }
-  const KernelT kern = pick_kernel(d->mode, nt);
+  const KernelT kern = pick_kernel(nt);
   const int rc_occ = resident_ctas((const void*)kern, smem, &per_sm);
   if (rc_occ != TECO_OK) return rc_occ;
   // persistent: as many CTAs as are resident at once, spread over the Cout splits
@@ -1573,6 +1563,11 @@ extern "C" int teco_conv3x3_tc(const teco_tc_desc* d, const void* x, const void*
   TECO_CHECK_ARG(d->Cin >= 64 && d->Cin % 64 == 0 && d->Cin <= 512, "teco_conv3x3_tc: Cin must be a multiple of 64 in [64,512] (got %d)", d->Cin);
   TECO_CHECK_ARG(d->Cout >= 16 && d->Cout % 16 == 0 && d->Cout <= 512, "teco_conv3x3_tc: Cout must be a multiple of 16 in [16,512] (got %d)", d->Cout);
   TECO_CHECK_ARG(d->mode == 0 || d->mode == 1, "teco_conv3x3_tc: unknown mode %d", d->mode);
+  // mode 1 runs on conv3x3_ws_kernel<1> only
+  TECO_CHECK_ARG(d->mode == 0 || d->Cin == 64, "teco_conv3x3_tc: mode 1 needs Cin 64 (got %d)", d->Cin);
+  TECO_CHECK_ARG(d->mode == 0 || d->Cout % 64 == 0, "teco_conv3x3_tc: mode 1 needs Cout a multiple of 64 (got %d)", d->Cout);
+  TECO_CHECK_ARG(d->mode == 0 || !res, "teco_conv3x3_tc: mode 1 takes no residual");
+  TECO_CHECK_ARG(d->mode == 0 || !out_f32, "teco_conv3x3_tc: mode 1 takes no fp32 output, only a bf16 y");
   TECO_CHECK_ARG(d->act >= 0 && d->act <= TECO_ACT_SIGMOID, "teco_conv3x3_tc: unknown activation %d", d->act);
   TECO_CHECK_ARG(!out_f32 || (d->out_f32_c > 0 && d->out_f32_c <= d->Cout), "teco_conv3x3_tc: bad out_f32_c");
   TECO_CHECK_ARG((((uintptr_t)x) & 15) == 0 && (((uintptr_t)wpk) & 15) == 0 && (((uintptr_t)y) & 15) == 0 &&

@@ -646,7 +646,9 @@ def conv3x3_tc(x, wpk, bias, y=None, *, cout, act=ACT_NONE, res=None, mode=0, ou
                k_live=0, pool=False):
     """One launch of the wgmma kernel.  x [N,H,W,Cin] bf16; y [N,H(,x2),W(,x2),cout] bf16 (allocated if None and
     out_f32 is None).  k_live (Cin 64): x's channels from 16 * k_live on are zero, so their K-steps may be skipped;
-    pool: y is [N,H/2,W/2,cout], the 2x2 max-pool of the output (maxpool2_bf16's result)."""
+    pool: y is [N,H/2,W/2,cout], the 2x2 max-pool of the output (maxpool2_bf16's result).  mode 1 (the transposed
+    convolution) takes Cin 64, cout a multiple of 64 and a bf16 y, with no res and no out_f32; it raises ValueError
+    otherwise."""
     N, H, W, Cin = x.shape
     s = 2 if mode == 1 else 1
     if y is None and out_f32 is None:

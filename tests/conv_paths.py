@@ -1,13 +1,11 @@
 """Host restatement of how teco_conv3x3_tc, teco_conv3x3_lin_tc and teco_conv3x3_wgrad_tc split a launch into kernels,
 Cout slices and tiles (csrc/conv_tc.cu, csrc/conv_wgrad_tc.cu), and of which code paths a launch reaches.
 
-route() mirrors launch_conv3x3 and pick_kernel in conv_tc.cu:
-  * nt = 64 output channels per CTA when Cout % 64 == 0 in mode 0, else 32 when Cout % 32 == 0, else 16 (launch_conv3x3);
-  * one 64-channel input block, 64-channel output slices, no fp32 output, and no residual in mode 1 run on
-    conv3x3_ws_kernel<mode> (launch_conv3x3), whose 72 KB of weights are always resident;
-  * everything else runs on conv3x3_wgmma_kernel<mode, nt> (pick_kernel), with the weights resident when all Cin / 64
-    blocks fit next to two halo stages (launch_conv3x3's p.resident), otherwise streamed with each block.
-From that arithmetic: <0,64> is resident for Cin / 64 <= 2, <0,32> and <1,32> for Cin / 64 <= 4, <., 16> always.
+route() mirrors teco_conv3x3_tc, launch_conv3x3 and pick_kernel in conv_tc.cu.  One 64-channel input block, 64-channel
+output slices and no fp32 output run on conv3x3_ws_kernel<mode> (72 KB of weights, always resident); any other mode-1
+launch is 'refused' (TECO_E_INVALID).  The rest runs on conv3x3_wgmma_kernel<nt>: nt = 64 when Cout % 64 == 0, else 32
+when Cout % 32 == 0, else 16, the weights resident when all Cin / 64 blocks fit next to two halo stages (p.resident),
+else streamed with each block: <64> is resident for Cin / 64 <= 2, <32> for Cin / 64 <= 4, <16> always.
 
 features() names what one launch reaches: the kernel, its activation, residual kind, Cout, output split, whether the
 tile count exceeds the persistent grid, ragged edges, and the epilogue's fp32 features.  tests/test_gpu_conv_exact.py
@@ -33,18 +31,19 @@ Route = namedtuple("Route", "kernel nt nsplit resident")
 
 
 def route(mode, cin, cout, res=False, res_is_y=False, out_f32=False, y=True):
-    """Kernel instance ('ws<0>', 'wgmma<0,64>', ...), output channels per CTA, Cout splits (grid rows) and whether the
-    weights are loaded once per CTA.  res_is_y (in-place residual) and y change only which tensor maps the launch
-    encodes, not the kernel."""
+    """Kernel instance ('ws<0>', 'wgmma<64>', ..., or 'refused'), output channels per CTA, Cout splits (grid rows) and
+    whether the weights are loaded once per CTA.  res_is_y (in-place residual) and y select only tensor maps."""
     del res_is_y, y
+    if mode == 1 and (cin != 64 or cout % 64 or res or out_f32):
+        return Route("refused", 0, 0, False)
     nblk = cin // 64
-    if nblk == 1 and cout % 64 == 0 and not out_f32 and (mode == 0 or not res):
+    if nblk == 1 and cout % 64 == 0 and not out_f32:
         return Route("ws<%d>" % mode, 64, cout // 64, True)
-    nt = 64 if (cout % 64 == 0 and mode == 0) else (32 if cout % 32 == 0 else 16)
+    nt = 64 if cout % 64 == 0 else (32 if cout % 32 == 0 else 16)
     w_blk_bytes = 9 * nt * 128
     fixed = 1024 + 64 + nt * 4
     resident = fixed + 2 * HALO_STAGE + nblk * w_blk_bytes <= SMEM_MAX
-    return Route("wgmma<%d,%d>" % (mode, nt), nt, cout // nt, resident)
+    return Route("wgmma<%d>" % nt, nt, cout // nt, resident)
 
 
 def tiles(n, h, w):

@@ -61,33 +61,26 @@ CASES = {
     "ws1_lrelu_tiny": C(1, 2, 5, 6, 64, 64, LRELU, {"ws<1> act=lrelu", "ws<1> ragged"}),
     "ws1_tanh": C(1, 2, 16, 16, 64, 64, TANH24, {"ws<1> act=tanh24"}),
     "ws1_sigmoid": C(1, 2, 9, 12, 64, 64, SIGMOID, {"ws<1> act=sigmoid", "ws<1> ragged"}),
-    # conv3x3_wgmma_kernel<0, 64>
-    "wgmma064_resident_res": C(0, 2, 19, 21, 128, 64, RELU, {"wgmma<0,64> resident+res"}, res="sep"),
-    "wgmma064_streamed_res": C(0, 1, 16, 24, 192, 128, NONE, {"wgmma<0,64> streamed+res", "wgmma<0,64> nsplit>1"},
+    # conv3x3_wgmma_kernel<64>
+    "wgmma064_resident_res": C(0, 2, 19, 21, 128, 64, RELU, {"wgmma<64> resident+res"}, res="sep"),
+    "wgmma064_streamed_res": C(0, 1, 16, 24, 192, 128, NONE, {"wgmma<64> streamed+res", "wgmma<64> nsplit>1"},
                                res="inplace"),
-    "wgmma064_out_f32": C(0, 2, 17, 20, 64, 64, RELU, {"wgmma<0,64> out_f32 nblk=1"}, y=False, f32c=64, res_f32=True,
+    "wgmma064_out_f32": C(0, 2, 17, 20, 64, 64, RELU, {"wgmma<64> out_f32 nblk=1"}, y=False, f32c=64, res_f32=True,
                           post=(0.5, 0.25)),
-    # conv3x3_wgmma_kernel<0, 32>
-    "wgmma032_resident": C(0, 2, 16, 16, 256, 96, LRELU, {"wgmma<0,32> resident", "wgmma<0,32> nsplit>1"}),
-    "wgmma032_streamed": C(0, 2, 13, 11, 320, 32, NONE, {"wgmma<0,32> streamed", "wgmma<0,32> res=sep"}, res="sep"),
-    # conv3x3_wgmma_kernel<0, 16>
-    "wgmma016_output_stage": C(0, 2, 40, 24, 64, 16, NONE, {"wgmma<0,16> output stage"}, y=False, f32c=3, res_f32=True,
+    # conv3x3_wgmma_kernel<32>
+    "wgmma032_resident": C(0, 2, 16, 16, 256, 96, LRELU, {"wgmma<32> resident", "wgmma<32> nsplit>1"}),
+    "wgmma032_streamed": C(0, 2, 13, 11, 320, 32, NONE, {"wgmma<32> streamed", "wgmma<32> res=sep"}, res="sep"),
+    # conv3x3_wgmma_kernel<16>
+    "wgmma016_output_stage": C(0, 2, 40, 24, 64, 16, NONE, {"wgmma<16> output stage"}, y=False, f32c=3, res_f32=True,
                                post=(2.0, -1.0)),
-    "wgmma016_fnet_head": C(0, 2, 17, 25, 64, 16, TANH24, {"wgmma<0,16> fnet head"}, y=False, f32c=2),
-    "wgmma016_y_and_f32": C(0, 2, 19, 13, 128, 48, RELU, {"wgmma<0,16> y+out_f32", "wgmma<0,16> out_f32_c spans splits"},
+    "wgmma016_fnet_head": C(0, 2, 17, 25, 64, 16, TANH24, {"wgmma<16> fnet head"}, y=False, f32c=2),
+    "wgmma016_y_and_f32": C(0, 2, 19, 13, 128, 48, RELU, {"wgmma<16> y+out_f32", "wgmma<16> out_f32_c spans splits"},
                             f32c=48, res_f32=True, post=(0.5, 0.25)),
-    "wgmma016_f32c_two_splits": C(0, 2, 21, 19, 64, 48, NONE, {"wgmma<0,16> out_f32_c spans splits"}, y=False, f32c=20,
+    "wgmma016_f32c_two_splits": C(0, 2, 21, 19, 64, 48, NONE, {"wgmma<16> out_f32_c spans splits"}, y=False, f32c=20,
                                   res_f32=True),
-    "wgmma016_sigmoid_f32": C(0, 2, 16, 24, 64, 16, SIGMOID, {"wgmma<0,16> act=sigmoid", "wgmma<0,16> out_f32"}, y=False,
+    "wgmma016_sigmoid_f32": C(0, 2, 16, 24, 64, 16, SIGMOID, {"wgmma<16> act=sigmoid", "wgmma<16> out_f32"}, y=False,
                               f32c=16, shift=-10.0),
-    "wgmma016_inplace_res": C(0, 2, 19, 21, 64, 16, RELU, {"wgmma<0,16> res=inplace"}, res="inplace"),
-    # conv3x3_wgmma_kernel<1, NT>
-    "wgmma132_cin128_res_f32": C(1, 2, 9, 11, 128, 64, NONE, {
-        "wgmma<1,32> cin=128", "wgmma<1,32> res=sep", "wgmma<1,32> y+out_f32"}, res="sep", f32c=64, res_f32=True,
-        post=(0.5, 0.25)),
-    "wgmma132_lrelu_inplace": C(1, 3, 19, 21, 64, 32, LRELU, {"wgmma<1,32> act=lrelu", "wgmma<1,32> res=inplace"},
-                                res="inplace"),
-    "wgmma116_cout48": C(1, 2, 24, 20, 64, 48, RELU, {"wgmma<1,16> cout=48"}),
+    "wgmma016_inplace_res": C(0, 2, 19, 21, 64, 16, RELU, {"wgmma<16> res=inplace"}, res="inplace"),
 }
 
 REQUIRED = (
@@ -95,11 +88,10 @@ REQUIRED = (
     {"ws<0> res=none", "ws<0> res=sep", "ws<0> res=inplace", "ws<0> bias=None", "ws<0> cout=128", "ws<0> cout=512",
      "ws<0> ragged", "ws<0> smaller than a tile", "ws<0> tiles>grid",
      "ws<1> ragged", "ws<1> wg below image", "ws<1> tiles>grid", "ws<1> cout=128",
-     "wgmma<0,64> resident+res", "wgmma<0,64> streamed+res", "wgmma<0,64> out_f32 nblk=1",
-     "wgmma<0,32> resident", "wgmma<0,32> streamed",
-     "wgmma<0,16> output stage", "wgmma<0,16> fnet head", "wgmma<0,16> y+out_f32", "wgmma<0,16> out_f32_c spans splits",
-     "wgmma<0,16> res=inplace",
-     "wgmma<1,32> cin=128", "wgmma<1,32> res=sep", "wgmma<1,32> out_f32", "wgmma<1,16> cout=48"})
+     "wgmma<64> resident+res", "wgmma<64> streamed+res", "wgmma<64> out_f32 nblk=1",
+     "wgmma<32> resident", "wgmma<32> streamed",
+     "wgmma<16> output stage", "wgmma<16> fnet head", "wgmma<16> y+out_f32", "wgmma<16> out_f32_c spans splits",
+     "wgmma<16> res=inplace"})
 
 # teco_conv3x3_lin_tc: 32x32 images and trunk-shaped plans (the only ones it takes), with (input buffer, output buffer,
 # residual buffer or -1, activation) per layer.  LeakyReLU only on a last layer: 0.2 v leaves the grid the next layer needs.
@@ -132,7 +124,8 @@ def test_case_tables_reach_every_required_path():
     tables reach every kernel instance of teco_conv3x3_tc with each epilogue feature listed in REQUIRED, the chain's
     weight-ring wrap, in-place residuals on either buffer, more clips than clusters and clusters running three clips at
     an odd and an even layer count (on plans its entry takes), and the
-    weight gradient's ragged and narrow shapes."""
+    weight gradient's ragged and narrow shapes.  Mode 1 runs on conv3x3_ws_kernel<1> only, and route() refuses it for
+    exactly four conditions, each of which mode 0 takes."""
     from tecogan_b200 import kernels as K
     seen = set()
     for name, c in CASES.items():
@@ -145,10 +138,15 @@ def test_case_tables_reach_every_required_path():
         seen |= got
     assert REQUIRED <= seen, sorted(REQUIRED - seen)
     kernels = {route(c.mode, c.cin, c.cout, bool(c.res), c.res == "inplace", c.f32c > 0, c.y).kernel for c in CASES.values()}
-    assert kernels == {"ws<0>", "ws<1>", "wgmma<0,64>", "wgmma<0,32>", "wgmma<0,16>", "wgmma<1,32>", "wgmma<1,16>"}
+    assert kernels == {"ws<0>", "ws<1>", "wgmma<64>", "wgmma<32>", "wgmma<16>"}
     assert route(0, 128, 64).resident and not route(0, 192, 64).resident
-    assert route(0, 256, 32).resident and not route(0, 320, 32).resident and route(1, 256, 32, res=True).resident
-    assert route(0, 512, 16).resident and route(1, 512, 48).resident
+    assert route(0, 256, 32).resident and not route(0, 320, 32).resident
+    assert route(0, 512, 16).resident
+    assert route(1, 64, 64).kernel == route(1, 64, 128).kernel == "ws<1>"
+    for cin, cout, res, out_f32 in ((128, 64, False, False), (64, 32, False, False), (64, 48, False, False),
+                                    (64, 64, True, False), (64, 64, False, True)):
+        assert route(1, cin, cout, res=res, out_f32=out_f32).kernel == "refused", (cin, cout, res, out_f32)
+        assert route(0, cin, cout, res=res, out_f32=out_f32).kernel != "refused", (cin, cout, res, out_f32)
     lin = set().union(*(lin_features(*v) for v in LIN_CASES.values()))
     assert LIN_REQUIRED <= lin, sorted(LIN_REQUIRED - lin)
     for n, h, plan in LIN_CASES.values():
@@ -368,42 +366,32 @@ def test_conv3x3_tc_matches_float64_reference_bit_for_bit(name):
 
 _KERNEL_RE = re.compile(r"conv3x3_(ws|wgmma)_kernel<([^>]*)>")
 
-# Records, in a child process, the CUDA kernels of one zero-operand launch per case in one profiler session, and prints
-# their names in launch order as JSON.  Repeated profiler sessions in one process can leave later sessions with no
-# events, so the suite's own process never profiles here.
-_PROFILE_ROUTES = """
-import json, torch
+# Runs fn of module once, then again in one profiler session, and prints the names of the CUDA kernels of that session
+# in launch order as JSON.  Repeated profiler sessions in one process can leave later sessions with no events, so the
+# suite's own process never profiles here: _profiled_conv_kernels runs this in a child process.
+_PROFILE = """
+import json, sys, torch
+sys.path.insert(0, %r)
 from torch.profiler import ProfilerActivity, profile
-from tests.test_gpu_conv_exact import CASES, _zero_launch
-for c in CASES.values():
-    _zero_launch(c)                   # module load and the packing, outside the profile
+from %s import %s as fn
+fn()                                  # module load and the packing, outside the profile
 with profile(activities=[ProfilerActivity.CUDA]) as prof:
-    for c in CASES.values():
-        _zero_launch(c)
+    fn()
 ev = sorted((e.time_range.start, e.name) for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA)
 print(json.dumps([name for _, name in ev]))
 """
 
 
-def _zero_launch(c):
-    s = 2 if c.mode == 1 else 1
-    zeros = lambda *shape: torch.zeros(*shape, dtype=torch.float64)
-    wt = zeros(3, 3, c.cin, c.cout) if c.mode == 0 else zeros(3, 3, c.cout, c.cin)
-    _launch(c, zeros(c.n, c.h, c.w, c.cin), wt, zeros(c.cout), zeros(c.n, s * c.h, s * c.w, c.cout) if c.res else None,
-            zeros(c.n, s * c.h, s * c.w, c.f32c) if c.res_f32 else None)
-
-
-@pytest.mark.gpu
-def test_conv3x3_tc_runs_the_kernels_conv_paths_names():
-    """The kernel instance of each case's launch, as the profiler records it, is the one tests/conv_paths.py::route
-    restates, so the case table reaches the paths the CPU test says it does."""
+def _profiled_conv_kernels(module, fn):
+    """The teco_conv3x3_tc kernel instances ('ws<1>', 'wgmma<64>', ...) that fn of module launches, in order, recorded
+    by the profiler in a child process."""
     import json
     import os
     import subprocess
     import sys
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     flags = ["-I"] if sys.flags.isolated else (["-s"] if sys.flags.no_user_site else [])
-    script = "import sys\nsys.path.insert(0, %r)\n" % root + _PROFILE_ROUTES
+    script = _PROFILE % (root, module, fn)
     out = subprocess.run([sys.executable] + flags + ["-c", script], cwd=root, capture_output=True, text=True, timeout=600)
     assert out.returncode == 0, out.stderr[-4000:]
     kernels = json.loads(out.stdout.strip().splitlines()[-1])
@@ -414,6 +402,27 @@ def test_conv3x3_tc_runs_the_kernels_conv_paths_names():
         m = _KERNEL_RE.search(k)
         if m:
             got.append("%s<%s>" % (m.group(1), ",".join(re.findall(r"\d+", m.group(2)))))
+    return got
+
+
+def _zero_launch(c):
+    s = 2 if c.mode == 1 else 1
+    zeros = lambda *shape: torch.zeros(*shape, dtype=torch.float64)
+    wt = zeros(3, 3, c.cin, c.cout) if c.mode == 0 else zeros(3, 3, c.cout, c.cin)
+    _launch(c, zeros(c.n, c.h, c.w, c.cin), wt, zeros(c.cout), zeros(c.n, s * c.h, s * c.w, c.cout) if c.res else None,
+            zeros(c.n, s * c.h, s * c.w, c.f32c) if c.res_f32 else None)
+
+
+def _zero_launches():
+    for c in CASES.values():
+        _zero_launch(c)
+
+
+@pytest.mark.gpu
+def test_conv3x3_tc_runs_the_kernels_conv_paths_names():
+    """The kernel instance of each case's launch, as the profiler records it, is the one tests/conv_paths.py::route
+    restates, so the case table reaches the paths the CPU test says it does."""
+    got = _profiled_conv_kernels("tests.test_gpu_conv_exact", "_zero_launches")
     want = [route(c.mode, c.cin, c.cout, bool(c.res), c.res == "inplace", c.f32c > 0, c.y).kernel for c in CASES.values()]
     assert len(got) == len(want), (got, want)
     bad = [(name, g, w) for name, g, w in zip(CASES, got, want) if g != w]
@@ -421,11 +430,12 @@ def test_conv3x3_tc_runs_the_kernels_conv_paths_names():
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("mode", [0, 1])
+@pytest.mark.parametrize("mode", [0])
 def test_ws_and_wgmma_kernels_agree_bit_for_bit_on_continuous_operands(mode):
-    """DESIGN 4.1: conv3x3_ws_kernel<mode> runs the products of conv3x3_wgmma_kernel in the same tap and K order with the
+    """DESIGN 4.1: conv3x3_ws_kernel<0> runs the products of conv3x3_wgmma_kernel in the same tap and K order with the
     same epilogue, so their bf16 outputs are bit-identical on any operands.  Asking for an fp32 output as well moves the
-    same 64 -> 64 launch onto conv3x3_wgmma_kernel (<0,64> or <1,32>), which writes the bf16 output in the same launch."""
+    same 64 -> 64 launch onto conv3x3_wgmma_kernel<64>, which writes the bf16 output in the same launch.  Mode 1 has
+    one kernel; tools/ab_conv.py compares it between two builds."""
     from tecogan_b200 import kernels as K
     g = torch.Generator().manual_seed(5 + mode)
     n, h, w = 3, 37, 45
