@@ -246,6 +246,15 @@ int teco_gauss_blur_down4(const int64_t* frames, int32_t bits, int32_t N, int32_
  *   swap_rb != 0 stores the channels reversed (BGR in, RGB out). */
 int teco_area_half_u8(const int64_t* frames, int32_t N, int32_t H, int32_t W, uint8_t* out, int32_t swap_rb,
                       void* stream);
+/* Output resize of `main.py --outscale` (DESIGN.md section 4.11).  dst [H_out, W_out, 3] uint8 = cv2.resize(src,
+ * (W_out, H_out), interpolation=INTER_LANCZOS4), bit for bit with cv2 4.13's fixed-point path, for a uint8 RGB src
+ * [H_in, W_in, 3].  Rows start every src_pitch / dst_pitch bytes (>= 3 * width).  xtab int32 [W_out, 9] and ytab int32
+ * [H_out, 9] are the host-computed axis tables of tecogan_b200/resize.py: base source index, then the eight int16
+ * weights.  1 <= sides <= 65535 and at most a 4x down-scale per axis (H_in <= 4 H_out, W_in <= 4 W_out), else
+ * TECO_E_INVALID. */
+int teco_resize_lanczos4_u8(const uint8_t* src, int64_t src_pitch, int32_t H_in, int32_t W_in, uint8_t* dst,
+                            int64_t dst_pitch, int32_t H_out, int32_t W_out, const int32_t* xtab, const int32_t* ytab,
+                            void* stream);
 
 /* generic elementwise y = f(a*x + b) with f in TECO_ACT_*; n elements. preprocess/deprocess lib/ops.py:13-22 */
 int teco_affine_act_f32(const float* x, float* y, int64_t n, float a, float b, int32_t act, void* stream);

@@ -22,6 +22,10 @@ Differences forced by the environment, stated once:
     reductions: every gradient, batch-norm and loss sum, and the gradient sum over ranks, adds in an order set by the
     shapes alone, so two runs with the same seed, data, build, GPU model and rank count give bit-identical variables,
     Adam moments, losses and outputs (the default atomic kernels agree only to rounding);
+  * --outscale s (opt-in extension, absent from FLAGS unless given; inference only, 1 <= s <= 16) writes
+    int(w_LR * s) x int(h_LR * s) files, Real-ESRGAN's convention: the network still runs at 4x and each output frame is
+    resized on the GPU (tecogan_b200/csrc/resize.cu) to the bytes cv2.resize(frame, size, INTER_LANCZOS4) gives, before
+    it is encoded; --outscale 4 writes the files of a run without the flag;
   * under `torchrun` each rank trains on its own clip shard with one NCCL all-reduce per step;
   * monitoring (--summary_dir: TensorBoard scalars, logfile.txt, validation scalars, test-sequence frames at every
     checkpoint) runs on rank 0 only, in process: the held-out scenes end_dir+1..end_dir_val are optional (validation is
@@ -59,6 +63,9 @@ FLAG_DEFS = [  # (name, type, default) -- reference main.py:32-103
     # extension: fixed-order training reductions, bit-identical reruns of one seed.  Opt-in: absent from FLAGS unless
     # given (argparse.SUPPRESS), so the flag set of a run without it stays exactly the reference's.
     ('deterministic', bool, argparse.SUPPRESS),
+    # extension: inference files of int(w * s) x int(h * s) instead of 4x (1 <= s <= 16), resized on the GPU as
+    # cv2.resize(INTER_LANCZOS4) does.  Opt-in in the same way.
+    ('outscale', float, argparse.SUPPRESS),
 ]
 
 
@@ -204,8 +211,9 @@ def inference(FLAGS):
         if first is None:
             raise IndexError('no .png frame in the input directory')
         h, w = first.shape[:2]
+        out_hw = outscale_size(FLAGS, h, w)
         print("input shape:", [1, h, w, 3])
-        print("output shape:", [1, h * 4, w * 4, 3])
+        print("output shape:", [1] + list(out_hw) + [3])
         config.set_precision(FLAGS.precision)
         store = V.set_default_store(V.VariableStore(seed=FLAGS.rand_seed))
         load_checkpoint(store, FLAGS.checkpoint, FLAGS.num_resblock)
@@ -214,12 +222,22 @@ def inference(FLAGS):
         image_dir = FLAGS.output_dir if FLAGS.output_pre == "" else os.path.join(FLAGS.output_dir, FLAGS.output_pre)
         os.makedirs(image_dir, exist_ok=True)
         super_resolve_frames(eng, padded(paths), itertools.chain([first], frames), image_dir, FLAGS.output_name,
-                             FLAGS.output_ext)
+                             FLAGS.output_ext, out_hw)
     finally:
         frames.close()
 
 
-def super_resolve_frames(eng, paths_LR, frames, image_dir, output_name, output_ext):
+def outscale_size(FLAGS, h, w):
+    """(height, width) of the files inference writes for an h x w input: 4x, or with --outscale s
+    (int(h * s), int(w * s))."""
+    from tecogan_b200 import resize
+    if not hasattr(FLAGS, 'outscale'):
+        return 4 * h, 4 * w
+    resize.check_outscale(FLAGS.outscale)
+    return resize.out_size(h, w, FLAGS.outscale)
+
+
+def super_resolve_frames(eng, paths_LR, frames, image_dir, output_name, output_ext, out_hw=None):
     """The per-frame loop of reference main.py:253-268: every frame through `eng`, the 5 warm-up frames discarded, the
     rest saved as <output_name>_<frame name>.<output_ext>.  paths_LR is the padded file list and `frames` its [h, w, 3]
     float32 frames in the same order (lib/dataloader.py::stream_inputs: decoded a window ahead on a reader thread).
@@ -227,7 +245,9 @@ def super_resolve_frames(eng, paths_LR, frames, image_dir, output_name, output_e
     The host does not wait for the device: each step's next frame is already on its way when the step is enqueued
     (its flow is estimated while this frame is generated), and each output frame is copied to a FrameWriter slot,
     encoded and written behind the steps that follow.  The files and the printed lines are those of the serial loop;
-    "total time" is the sum of the steps' device times (CUDA events around each step)."""
+    "total time" is the sum of the steps' device times (CUDA events around each step).  `out_hw` (--outscale) is the
+    files' (height, width) when it is not the network's 4x: the writer resizes each frame to it on the device
+    (lib/writer.py::FrameWriter)."""
     import collections
     import torch
     from tecogan_b200.lib.writer import FrameWriter
@@ -255,7 +275,7 @@ def super_resolve_frames(eng, paths_LR, frames, image_dir, output_name, output_e
                 filename = output_name + '_' + name
                 print('saving image %s' % filename)
                 if writer is None:
-                    writer = FrameWriter(eng.out_u8.shape[1], eng.out_u8.shape[2], eng.device)
+                    writer = FrameWriter(*(out_hw or eng.out_u8.shape[1:3]), eng.device)
                 writer.put(eng.out_u8[0], os.path.join(image_dir, "%s.%s" % (filename, output_ext)))
             else:   # First 5 is a hard-coded symmetric frame padding, ignored but time added!
                 print("Warming up %d" % (5 - i))
@@ -571,6 +591,11 @@ def train(FLAGS):
 
 def main(argv=None):
     FLAGS = parse_flags(argv)
+    if hasattr(FLAGS, 'outscale'):             # refused before anything is set up
+        if FLAGS.mode != 'inference':
+            raise ValueError('--outscale applies to --mode inference only')
+        from tecogan_b200.resize import check_outscale
+        check_outscale(FLAGS.outscale)
     if 'LOCAL_RANK' not in os.environ:
         os.environ["CUDA_VISIBLE_DEVICES"] = FLAGS.cudaID       # reference main.py:107: overwritten unconditionally
     if FLAGS.output_dir is None:

@@ -75,6 +75,7 @@ SIGNATURES = {
     "teco_frames_to_f32": [_P, _I32, _I32, _I32, _I32, _P, _P],
     "teco_gauss_blur_down4": [_P, _I32, _I32, _I32, _I32, _P, _P],
     "teco_area_half_u8": [_P, _I32, _I32, _I32, _P, _I32, _P],
+    "teco_resize_lanczos4_u8": [_P, _I64, _I32, _I32, _P, _I64, _I32, _I32, _P, _P, _P],
     "teco_affine_act_f32": [_P, _P, _I64, _F, _F, _I32, _P],
     "teco_act_bwd_f32": [_P, _P, _P, _I64, _I32, _P],
     "teco_f32_to_bf16_pad": [_P, _P, _I64, _I32, _I32, _I32, _I32, _F, _F, _P],

@@ -589,6 +589,40 @@ def area_half(frames, swap_rb=False, out=None):
     return out
 
 
+def _rgb8_rows(t, what):
+    """Row pitch in bytes of a uint8 [H, W, 3] CUDA tensor whose rows are packed pixels (any row pitch, any offset)."""
+    if not torch.is_tensor(t) or not t.is_cuda or t.dtype != torch.uint8 or t.dim() != 3 or t.shape[2] != 3:
+        raise ValueError("resize_lanczos4: %s must be a uint8 [H, W, 3] CUDA tensor, got %s" % (
+            what, "%s %s on %s" % (t.dtype, tuple(t.shape), t.device) if torch.is_tensor(t) else type(t).__name__))
+    if t.stride(2) != 1 or t.stride(1) != 3 or t.stride(0) < 3 * t.shape[1]:
+        raise ValueError("resize_lanczos4: %s needs packed RGB rows, got strides %s" % (what, t.stride()))
+    return t.stride(0)
+
+
+def resize_lanczos4(src, dst, tables=None):
+    """dst[:] = cv2.resize(src, (W_out, H_out), interpolation=cv2.INTER_LANCZOS4) bit for bit (cv2 4.13), on the
+    current stream: the output resize of `main.py --outscale` (DESIGN.md section 4.11).  src and dst are uint8
+    [H, W, 3] RGB CUDA tensors on one device, rows packed at any pitch; 1 <= sides <= 65535 and H_in <= 4 H_out,
+    W_in <= 4 W_out.  `tables` is resize.tables(H_in, W_in, H_out, W_out, device), computed when not given.  Anything
+    else raises ValueError before a launch."""
+    from . import resize
+    sp, dp = _rgb8_rows(src, "src"), _rgb8_rows(dst, "dst")
+    if src.device != dst.device:
+        raise ValueError("resize_lanczos4: src on %s, dst on %s" % (src.device, dst.device))
+    (H, W), (h, w) = src.shape[:2], dst.shape[:2]
+    if not (0 < H <= 65535 and 0 < W <= 65535 and 0 < h <= 65535 and 0 < w <= 65535 and H <= 4 * h and W <= 4 * w):
+        raise ValueError("resize_lanczos4: %dx%d -> %dx%d: sides must be 1..65535, down-scaled at most 4x" % (H, W, h, w))
+    xtab, ytab = resize.tables(H, W, h, w, src.device) if tables is None else tables
+    for tab, n in ((xtab, w), (ytab, h)):
+        if not (torch.is_tensor(tab) and tab.dtype == torch.int32 and tuple(tab.shape) == (n, 9)
+                and tab.device == src.device and tab.is_contiguous()):
+            raise ValueError("resize_lanczos4: tables must be contiguous int32 [%d, 9] and [%d, 9] on %s"
+                             % (w, h, src.device))
+    call("teco_resize_lanczos4_u8", ctypes.c_void_p(src.data_ptr()), sp, H, W, ctypes.c_void_p(dst.data_ptr()), dp,
+         h, w, ptr(xtab, torch.int32), ptr(ytab, torch.int32), stream_ptr())
+    return dst
+
+
 def to_u8(x01):
     y = torch.empty(x01.shape, device=x01.device, dtype=torch.uint8)
     call("teco_to_u8", ptr(_cc(x01), f32), ptr(y, torch.uint8), x01.numel(), stream_ptr())

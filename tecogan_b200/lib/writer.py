@@ -6,11 +6,13 @@ WRITE_SLOTS = 3           # output frames between the producer and the files: en
 
 class FrameWriter:
     """The write-behind half of super_resolve_frames and data_prepare.  put(out_u8, path) copies a uint8 [h, w, 3] RGB
-    device frame into a free slot of a small ring on the current (the producer's) stream, then starts its encode -- on the slot's own stream, after an
-    event, with the slot's own encoder buffers -- or, for a format cv2 writes, the copy back to the host.  One writer
-    thread takes the slots in order, waits for each, writes its file (lib/ops.py::write_image, the rule save_img
-    follows) and hands the slot back; put() waits for a slot whose file is written.  An exception on the writer thread is
-    raised by the next put() and by close(); close() joins the thread on every exit."""
+    device frame into a free slot of a small ring on the current (the producer's) stream -- a frame of another size is
+    resized into the slot instead (kernels.resize_lanczos4, cv2's INTER_LANCZOS4: `main.py --outscale`) -- then starts
+    its encode -- on the slot's own stream, after an event, with the slot's own encoder buffers -- or, for a format cv2
+    writes, the copy back to the host.  Either way the frame is read on the producer's stream, before its next step can
+    overwrite it.  One writer thread takes the slots in order, waits for each, writes its file (lib/ops.py::write_image,
+    the rule save_img follows) and hands the slot back; put() waits for a slot whose file is written.  An exception on
+    the writer thread is raised by the next put() and by close(); close() joins the thread on every exit."""
 
     def __init__(self, h, w, device):
         import queue
@@ -32,12 +34,16 @@ class FrameWriter:
 
     def put(self, out_u8, path):
         import torch
+        from tecogan_b200 import kernels as K
         from tecogan_b200.lib import ops
         codec = ops.image_codec(path, self.h, self.w)
         slot = self.free.get()
         if isinstance(slot, BaseException):
             raise slot
-        slot.u8.copy_(out_u8)
+        if tuple(out_u8.shape[:2]) == (self.h, self.w):
+            slot.u8.copy_(out_u8)
+        else:
+            K.resize_lanczos4(out_u8, slot.u8)
         ready = torch.cuda.Event()
         ready.record()
         with torch.cuda.stream(slot.stream):
