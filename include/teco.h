@@ -255,6 +255,15 @@ int teco_area_half_u8(const int64_t* frames, int32_t N, int32_t H, int32_t W, ui
 int teco_resize_lanczos4_u8(const uint8_t* src, int64_t src_pitch, int32_t H_in, int32_t W_in, uint8_t* dst,
                             int64_t dst_pitch, int32_t H_out, int32_t W_out, const int32_t* xtab, const int32_t* ytab,
                             void* stream);
+/* Colour conversions of `main.py --input_y4m / --output_y4m` (DESIGN.md section 4.12), bit for bit with cv2 4.13's
+ * BT.601 limited-range fixed-point cvtColor.  An I420 frame is [3H/2, W] uint8: the Y plane, then U and V at
+ * (H/2) x (W/2), each packed.  Sides are even and 2..65534, else TECO_E_INVALID (nothing is launched).
+ * teco_rgb_to_i420_u8: dst = cvtColor(src, COLOR_RGB2YUV_I420) for a uint8 RGB src [H, W, 3] whose rows start every
+ *   src_pitch (>= 3 * W) bytes; U and V come from the top-left pixel of each 2 x 2 block, as in cv2.
+ * teco_i420_to_rgb_u8: dst [N, H, W, 3] uint8 RGB = cvtColor(frame, COLOR_YUV2RGB_I420) of N >= 1 packed I420 frames
+ *   src [N, 3H/2, W]. */
+int teco_rgb_to_i420_u8(const uint8_t* src, int64_t src_pitch, int32_t H, int32_t W, uint8_t* dst, void* stream);
+int teco_i420_to_rgb_u8(const uint8_t* src, int32_t N, int32_t H, int32_t W, uint8_t* dst, void* stream);
 
 /* generic elementwise y = f(a*x + b) with f in TECO_ACT_*; n elements. preprocess/deprocess lib/ops.py:13-22 */
 int teco_affine_act_f32(const float* x, float* y, int64_t n, float a, float b, int32_t act, void* stream);

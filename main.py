@@ -26,6 +26,11 @@ Differences forced by the environment, stated once:
     int(w_LR * s) x int(h_LR * s) files, Real-ESRGAN's convention: the network still runs at 4x and each output frame is
     resized on the GPU (tecogan_b200/csrc/resize.cu) to the bytes cv2.resize(frame, size, INTER_LANCZOS4) gives, before
     it is encoded; --outscale 4 writes the files of a run without the flag;
+  * --input_y4m PATH / --output_y4m PATH (opt-in extensions, absent from FLAGS unless given; inference only) read the
+    input from and write the output to a YUV4MPEG2 stream (8-bit 4:2:0, limited range; a file, a FIFO or /dev/stdin),
+    converted on the GPU (tecogan_b200/csrc/yuv.cu) byte for byte as cv2.cvtColor(COLOR_YUV2RGB_I420 /
+    COLOR_RGB2YUV_I420) converts; y4m input names its files <output_name>_<%04d frame number>.<output_ext>, y4m output
+    holds the frames the image path would write and no image file is written;
   * under `torchrun` each rank trains on its own clip shard with one NCCL all-reduce per step;
   * monitoring (--summary_dir: TensorBoard scalars, logfile.txt, validation scalars, test-sequence frames at every
     checkpoint) runs on rank 0 only, in process: the held-out scenes end_dir+1..end_dir_val are optional (validation is
@@ -66,6 +71,8 @@ FLAG_DEFS = [  # (name, type, default) -- reference main.py:32-103
     # extension: inference files of int(w * s) x int(h * s) instead of 4x (1 <= s <= 16), resized on the GPU as
     # cv2.resize(INTER_LANCZOS4) does.  Opt-in in the same way.
     ('outscale', float, argparse.SUPPRESS),
+    # extension: inference input / output as a YUV4MPEG2 stream (tecogan_b200/y4m.py).  Opt-in in the same way.
+    ('input_y4m', str, argparse.SUPPRESS), ('output_y4m', str, argparse.SUPPRESS),
 ]
 
 
@@ -199,19 +206,30 @@ def restore_train_state(train_state, spec):
 
 
 def inference(FLAGS):
-    from tecogan_b200 import config, variables as V
+    from tecogan_b200 import config, variables as V, y4m
     from tecogan_b200.engine import InferenceEngine
     from tecogan_b200.lib.dataloader import inference_paths, padded, stream_inputs
     if FLAGS.checkpoint is None:
         raise ValueError('The checkpoint file is needed to performing the test.')
-    paths, down = inference_paths(FLAGS)
-    frames = stream_inputs(paths, down)
+    sink = None
+    if hasattr(FLAGS, 'input_y4m'):            # the header is read and checked here, before anything is set up
+        reader = y4m.Y4MReader(FLAGS.input_y4m, FLAGS.input_dir_len)
+        rate, aspect = reader.header.rate, reader.header.aspect
+        frames, names = reader.frames(), reader.names()
+    else:
+        paths, down = inference_paths(FLAGS)
+        rate, aspect = y4m.PNG_INPUT_RATE, y4m.PNG_INPUT_ASPECT
+        frames, names = stream_inputs(paths, down), padded(paths)
     try:
         first = next(frames, None)
         if first is None:
-            raise IndexError('no .png frame in the input directory')
+            raise IndexError('no frame in the input y4m stream' if hasattr(FLAGS, 'input_y4m')
+                             else 'no .png frame in the input directory')
         h, w = first.shape[:2]
         out_hw = outscale_size(FLAGS, h, w)
+        if hasattr(FLAGS, 'output_y4m') and (out_hw[0] % 2 or out_hw[1] % 2):
+            raise ValueError('--output_y4m: the %dx%d output has an odd side; 4:2:0 needs even sides (choose another '
+                             '--outscale)' % (out_hw[1], out_hw[0]))
         print("input shape:", [1, h, w, 3])
         print("output shape:", [1] + list(out_hw) + [3])
         config.set_precision(FLAGS.precision)
@@ -220,11 +238,16 @@ def inference(FLAGS):
         eng = InferenceEngine(h, w, FLAGS.num_resblock)
         print('Finish building the network')
         image_dir = FLAGS.output_dir if FLAGS.output_pre == "" else os.path.join(FLAGS.output_dir, FLAGS.output_pre)
-        os.makedirs(image_dir, exist_ok=True)
-        super_resolve_frames(eng, padded(paths), itertools.chain([first], frames), image_dir, FLAGS.output_name,
-                             FLAGS.output_ext, out_hw)
+        if hasattr(FLAGS, 'output_y4m'):
+            sink = y4m.Y4MWriter(FLAGS.output_y4m, out_hw[1], out_hw[0], rate, aspect)
+        else:
+            os.makedirs(image_dir, exist_ok=True)
+        super_resolve_frames(eng, names, itertools.chain([first], frames), image_dir, FLAGS.output_name,
+                             FLAGS.output_ext, out_hw, sink)
     finally:
         frames.close()
+        if sink is not None:
+            sink.close()
 
 
 def outscale_size(FLAGS, h, w):
@@ -237,10 +260,13 @@ def outscale_size(FLAGS, h, w):
     return resize.out_size(h, w, FLAGS.outscale)
 
 
-def super_resolve_frames(eng, paths_LR, frames, image_dir, output_name, output_ext, out_hw=None):
+def super_resolve_frames(eng, paths_LR, frames, image_dir, output_name, output_ext, out_hw=None, sink=None):
     """The per-frame loop of reference main.py:253-268: every frame through `eng`, the 5 warm-up frames discarded, the
     rest saved as <output_name>_<frame name>.<output_ext>.  paths_LR is the padded file list and `frames` its [h, w, 3]
     float32 frames in the same order (lib/dataloader.py::stream_inputs: decoded a window ahead on a reader thread).
+    The loop runs to the end of `frames`, whose length need not be known; paths_LR may be any iterable of paths or
+    names taken in step with it (tecogan_b200/y4m.py::Y4MReader.names for --input_y4m).  With a `sink`
+    (y4m.Y4MWriter, --output_y4m) the frames that would be saved are appended to it instead, and no file is written.
 
     The host does not wait for the device: each step's next frame is already on its way when the step is enqueued
     (its flow is estimated while this frame is generated), and each output frame is copied to a FrameWriter slot,
@@ -251,16 +277,19 @@ def super_resolve_frames(eng, paths_LR, frames, image_dir, output_name, output_e
     import collections
     import torch
     from tecogan_b200.lib.writer import FrameWriter
-    it = iter(frames)
-    max_iter = len(paths_LR)
+    it, names = iter(frames), iter(paths_LR)
+    max_iter = 0
     srtime = 0.0
     timing = collections.deque()           # (start, end) events of steps whose time is not yet counted
     writer = None
     print('Frame evaluation starts!!')
     try:
         cur = next(it, None)
-        for i in range(max_iter):
-            nxt = next(it, None) if i + 1 < max_iter else None
+        for i in itertools.count():
+            if cur is None:
+                break
+            path = next(names)
+            nxt = next(it, None)
             t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             t0.record()
             eng.step(cur, next_lr=nxt)
@@ -270,12 +299,13 @@ def super_resolve_frames(eng, paths_LR, frames, image_dir, output_name, output_e
                 a, b = timing.popleft()
                 srtime += a.elapsed_time(b) / 1000.0
             cur = nxt
+            max_iter = i + 1
             if i >= 5:
-                name, _ = os.path.splitext(os.path.basename(str(paths_LR[i])))
+                name, _ = os.path.splitext(os.path.basename(str(path)))
                 filename = output_name + '_' + name
                 print('saving image %s' % filename)
                 if writer is None:
-                    writer = FrameWriter(*(out_hw or eng.out_u8.shape[1:3]), eng.device)
+                    writer = FrameWriter(*(out_hw or eng.out_u8.shape[1:3]), eng.device, sink=sink)
                 writer.put(eng.out_u8[0], os.path.join(image_dir, "%s.%s" % (filename, output_ext)))
             else:   # First 5 is a hard-coded symmetric frame padding, ignored but time added!
                 print("Warming up %d" % (5 - i))
@@ -591,6 +621,11 @@ def train(FLAGS):
 
 def main(argv=None):
     FLAGS = parse_flags(argv)
+    for flag in ('input_y4m', 'output_y4m'):    # refused before anything is set up
+        if hasattr(FLAGS, flag) and FLAGS.mode != 'inference':
+            raise ValueError('--%s applies to --mode inference only' % flag)
+    if hasattr(FLAGS, 'input_y4m') and (FLAGS.input_dir_LR is not None or FLAGS.input_dir_HR is not None):
+        raise ValueError('--input_y4m replaces --input_dir_LR / --input_dir_HR: give one input')
     if hasattr(FLAGS, 'outscale'):             # refused before anything is set up
         if FLAGS.mode != 'inference':
             raise ValueError('--outscale applies to --mode inference only')

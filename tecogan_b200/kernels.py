@@ -589,13 +589,13 @@ def area_half(frames, swap_rb=False, out=None):
     return out
 
 
-def _rgb8_rows(t, what):
+def _rgb8_rows(t, what, fn="resize_lanczos4"):
     """Row pitch in bytes of a uint8 [H, W, 3] CUDA tensor whose rows are packed pixels (any row pitch, any offset)."""
     if not torch.is_tensor(t) or not t.is_cuda or t.dtype != torch.uint8 or t.dim() != 3 or t.shape[2] != 3:
-        raise ValueError("resize_lanczos4: %s must be a uint8 [H, W, 3] CUDA tensor, got %s" % (
-            what, "%s %s on %s" % (t.dtype, tuple(t.shape), t.device) if torch.is_tensor(t) else type(t).__name__))
+        raise ValueError("%s: %s must be a uint8 [H, W, 3] CUDA tensor, got %s" % (
+            fn, what, "%s %s on %s" % (t.dtype, tuple(t.shape), t.device) if torch.is_tensor(t) else type(t).__name__))
     if t.stride(2) != 1 or t.stride(1) != 3 or t.stride(0) < 3 * t.shape[1]:
-        raise ValueError("resize_lanczos4: %s needs packed RGB rows, got strides %s" % (what, t.stride()))
+        raise ValueError("%s: %s needs packed RGB rows, got strides %s" % (fn, what, t.stride()))
     return t.stride(0)
 
 
@@ -621,6 +621,55 @@ def resize_lanczos4(src, dst, tables=None):
     call("teco_resize_lanczos4_u8", ctypes.c_void_p(src.data_ptr()), sp, H, W, ctypes.c_void_p(dst.data_ptr()), dp,
          h, w, ptr(xtab, torch.int32), ptr(ytab, torch.int32), stream_ptr())
     return dst
+
+
+def _i420_sides(H, W, fn):
+    if not (2 <= H <= 65534 and 2 <= W <= 65534 and H % 2 == 0 and W % 2 == 0):
+        raise ValueError("%s: I420 needs even sides 2..65534, got %dx%d" % (fn, H, W))
+
+
+def rgb_to_i420(src, dst):
+    """dst[:] = cv2.cvtColor(src, cv2.COLOR_RGB2YUV_I420) bit for bit (cv2 4.13), on the current stream: the writer half
+    of `main.py --output_y4m` (DESIGN.md section 4.12).  src is a uint8 [H, W, 3] RGB CUDA tensor, rows packed at any
+    pitch and offset; dst a contiguous uint8 [3H/2, W] CUDA tensor on its device, the Y, U and V planes of one Y4M frame.
+    Sides are even and 2..65534.  Anything else raises ValueError before a launch."""
+    sp = _rgb8_rows(src, "src", "rgb_to_i420")
+    H, W = src.shape[:2]
+    _i420_sides(H, W, "rgb_to_i420")
+    if not (torch.is_tensor(dst) and dst.is_cuda and dst.dtype == torch.uint8 and tuple(dst.shape) == (3 * H // 2, W)
+            and dst.is_contiguous() and dst.device == src.device):
+        raise ValueError("rgb_to_i420: dst must be a contiguous uint8 [%d, %d] tensor on %s, got %s" % (
+            3 * H // 2, W, src.device,
+            "%s %s on %s" % (dst.dtype, tuple(dst.shape), dst.device) if torch.is_tensor(dst) else type(dst).__name__))
+    call("teco_rgb_to_i420_u8", ctypes.c_void_p(src.data_ptr()), sp, H, W, ptr(dst, torch.uint8), stream_ptr())
+    return dst
+
+
+def i420_to_rgb(frames, out=None):
+    """uint8 [N, H, W, 3] RGB = cv2.cvtColor(frame, cv2.COLOR_YUV2RGB_I420) of each frame, bit for bit (cv2 4.13), on the
+    current stream: the reader half of `main.py --input_y4m` (DESIGN.md section 4.12).  `frames` is a contiguous uint8
+    CUDA tensor [N, 3H/2, W] of packed I420 frames (or one frame [3H/2, W]); sides are even and 2..65534.  `out` may be
+    given as a contiguous uint8 [N, H, W, 3] tensor on the frames' device.  Anything else raises ValueError before a
+    launch."""
+    if not (torch.is_tensor(frames) and frames.is_cuda and frames.dtype == torch.uint8 and frames.dim() in (2, 3)
+            and frames.is_contiguous()):
+        raise ValueError("i420_to_rgb: frames must be a contiguous uint8 [N, 3H/2, W] CUDA tensor, got %s" % (
+            "%s %s on %s" % (frames.dtype, tuple(frames.shape), frames.device) if torch.is_tensor(frames)
+            else type(frames).__name__))
+    f = frames if frames.dim() == 3 else frames[None]
+    N, rows, W = f.shape
+    if N < 1 or rows % 3:
+        raise ValueError("i420_to_rgb: %d frames of %d rows: need N >= 1 and 3H/2 rows" % (N, rows))
+    H = rows // 3 * 2
+    _i420_sides(H, W, "i420_to_rgb")
+    shape = (N, H, W, 3)
+    if out is None:
+        out = torch.empty(shape, device=f.device, dtype=torch.uint8)
+    elif not (torch.is_tensor(out) and out.dtype == torch.uint8 and tuple(out.shape) == shape and out.is_contiguous()
+              and out.device == f.device):
+        raise ValueError("i420_to_rgb: out must be a contiguous uint8 %s tensor on %s" % (shape, f.device))
+    call("teco_i420_to_rgb_u8", ptr(f, torch.uint8), N, H, W, ptr(out, torch.uint8), stream_ptr())
+    return out
 
 
 def to_u8(x01):

@@ -77,14 +77,10 @@ def stream_inputs(paths, down, window_bytes=None):
     (padded(paths) = paths[5:0:-1] + paths), without keeping the sequence on the device.
 
     A reader thread decodes the files window by window (input_windows) with read_inputs(window_paths, down) on a CUDA
-    stream of its own, one window ahead of the consumer.  Each file is decoded once: the warm-up entries are the same
-    tensors as frames 1..5, which are kept until the sequence passes them again.  A window's frames reach the consumer
-    after its current stream has waited for the reader's event, and are recorded on that stream so that the allocator
-    reuses their memory only once the consumer's work on them is done.  A decoding error is raised by the generator at the
-    frame that needs the window.  Closing the generator (or an exception in it) stops and joins the reader."""
-    import queue
-    import threading
-    import torch
+    stream of its own, one window ahead of the consumer (DeviceHandoff).  Each file is decoded once: the warm-up entries
+    are the same tensors as frames 1..5, which are kept until the sequence passes them again.  A decoding error is raised
+    by the generator at the frame that needs the window.  Closing the generator (or an exception in it) stops and joins
+    the reader."""
     windows = input_windows(paths, window_bytes)
     if not windows:
         return
@@ -94,65 +90,115 @@ def stream_inputs(paths, down, window_bytes=None):
     window_of = [w for w, (i, j) in enumerate(windows) for _ in range(i, j)]
     left = [j - i for i, j in windows]              # files of each window not yet past their last use
     # the warm-up needs every window up to file min(5, n - 1), window w5, before its first frame, and one more may be
-    # decoded ahead; the windows before w5 return no slot, so past the warm-up the reader is one window ahead
+    # decoded ahead; the windows before w5 return no credit, so past the warm-up the reader is one window ahead
     w5 = window_of[order[0]]
-    slots = threading.Semaphore(w5 + 2)
-    ready, stop = queue.Queue(), threading.Event()
-    cuda = torch.cuda.is_available()
-    device = torch.cuda.current_device() if cuda else None
 
-    def read():
-        try:
-            if cuda:
-                torch.cuda.set_device(device)
-            stream = torch.cuda.Stream() if cuda else None
-            for i, j in windows:
-                slots.acquire()
-                if stop.is_set():
-                    return
-                with torch.cuda.stream(stream):
-                    frames = list(read_inputs(paths[i:j], down))
-                    done = torch.cuda.Event() if cuda else None
-                    if cuda:
-                        done.record()
-                ready.put((i, frames, done))
-                del frames
-        except BaseException as e:                  # handed to the consumer, raised there
-            ready.put(e)
+    def decode():
+        for i, j in windows:
+            yield i, list(read_inputs(paths[i:j], down))
 
-    reader = threading.Thread(target=read, name='stream_inputs', daemon=True)
-    reader.start()
-    have = {}
+    feed = DeviceHandoff(decode(), w5 + 2, 'stream_inputs')
     try:
         for p, k in enumerate(order):
-            while k not in have:
-                got = ready.get()
-                if isinstance(got, BaseException):
-                    raise got
-                i, frames, done = got
-                if done is not None:
-                    consumer = torch.cuda.current_stream()
-                    consumer.wait_event(done)
-                    for t in frames:
-                        if torch.is_tensor(t) and t.is_cuda:
-                            t.record_stream(consumer)
-                have.update(zip(range(i, i + len(frames)), frames))
-                del got, frames
-            frame = have[k]
+            frame = feed.take(k)
             if last_use[k] == p:
-                del have[k]
+                feed.drop(k)
                 w = window_of[k]
                 left[w] -= 1
                 if left[w] == 0 and w >= w5:
-                    slots.release()
+                    feed.release()
             yield frame
             del frame
     finally:
-        stop.set()
-        for _ in windows:
-            slots.release()
-        reader.join()
-        have.clear()
+        feed.close()
+
+
+class DeviceHandoff:
+    """The reader half of a streamed inference input, shared by stream_inputs (PNG files) and
+    tecogan_b200/y4m.py::Y4MReader (a YUV4MPEG2 stream).
+
+    A reader thread runs `chunks` -- an iterator of (first frame index, [frames]) -- under a CUDA stream of its own, one
+    credit per chunk: it waits for a credit before it asks for the next chunk, and the consumer gives credits back with
+    release().  Each chunk is handed over with an event recorded on the reader's stream.  take(k) returns frame k: the
+    consumer's current stream first waits for the chunk's event, and the chunk's tensors are recorded on that stream, so
+    the allocator reuses their memory only once the consumer's work on them is done.  take() returns None once the
+    iterator has ended without frame k, and raises an exception of the reader at the frame that needs its chunk.  drop(k)
+    forgets frame k.  close() stops and joins the reader; the iterator is not asked for another chunk after it."""
+
+    def __init__(self, chunks, credits, name):
+        import queue
+        import threading
+        import torch
+        self.credits, self.ready, self.stop = threading.Semaphore(credits), queue.Queue(), threading.Event()
+        self.have, self.ended = {}, False
+        cuda = torch.cuda.is_available()
+        device = torch.cuda.current_device() if cuda else None
+
+        def read():
+            try:
+                if cuda:
+                    torch.cuda.set_device(device)
+                stream = torch.cuda.Stream() if cuda else None
+                it = iter(chunks)
+                while True:
+                    self.credits.acquire()
+                    if self.stop.is_set():
+                        return
+                    with torch.cuda.stream(stream):
+                        got = next(it, None)
+                        if got is None:
+                            self.ready.put(None)
+                            return
+                        i, frames = got
+                        done = torch.cuda.Event() if cuda else None
+                        if cuda:
+                            done.record()
+                    self.ready.put((i, frames, done))
+                    del got, frames
+            except BaseException as e:              # handed to the consumer, raised there
+                self.ready.put(e)
+            finally:
+                close = getattr(chunks, 'close', None)
+                if close is not None:               # a generator's own clean-up runs on this thread
+                    close()
+
+        self.thread = threading.Thread(target=read, name=name, daemon=True)
+        self.thread.start()
+
+    def take(self, k):
+        import torch
+        while k not in self.have:
+            if self.ended:
+                return None
+            got = self.ready.get()
+            if got is None:
+                self.ended = True
+                continue
+            if isinstance(got, BaseException):
+                self.ended = True
+                raise got
+            i, frames, done = got
+            if done is not None:
+                consumer = torch.cuda.current_stream()
+                consumer.wait_event(done)
+                for t in frames:
+                    if torch.is_tensor(t) and t.is_cuda:
+                        t.record_stream(consumer)
+            self.have.update(zip(range(i, i + len(frames)), frames))
+            del got, frames
+        return self.have[k]
+
+    def drop(self, k):
+        del self.have[k]
+
+    def release(self):
+        self.credits.release()
+
+    def close(self):
+        self.stop.set()
+        self.credits.release()                      # wakes a reader waiting for a credit; it sees `stop` and returns
+        self.thread.join()
+        self.have.clear()
 
 
 def _png_head(path):
