@@ -264,6 +264,12 @@ int teco_resize_lanczos4_u8(const uint8_t* src, int64_t src_pitch, int32_t H_in,
  *   src [N, 3H/2, W]. */
 int teco_rgb_to_i420_u8(const uint8_t* src, int64_t src_pitch, int32_t H, int32_t W, uint8_t* dst, void* stream);
 int teco_i420_to_rgb_u8(const uint8_t* src, int32_t N, int32_t H, int32_t W, uint8_t* dst, void* stream);
+/* Frame difference of `main.py --scene_threshold` (DESIGN.md section 4.13): *out = sum over i < n of
+ * |q(a[i]) - q(b[i])|, q(x) = clamp(rint(255 x), 0, 255) with 255 x rounded to float32 and then half-even to an integer.
+ * Exact 64-bit integer sum, independent of the launch.  The entry zeroes *out on `stream` itself, then adds to it;
+ * n == 0 gives 0.  a, b: n float32 values each, any 4-byte alignment (float4 loads when both are 16-byte aligned).
+ * NULL pointers or n < 0: TECO_E_INVALID, nothing is enqueued. */
+int teco_frame_sad_q8(const float* a, const float* b, int64_t n, uint64_t* out, void* stream);
 
 /* generic elementwise y = f(a*x + b) with f in TECO_ACT_*; n elements. preprocess/deprocess lib/ops.py:13-22 */
 int teco_affine_act_f32(const float* x, float* y, int64_t n, float a, float b, int32_t act, void* stream);

@@ -31,6 +31,12 @@ Differences forced by the environment, stated once:
     converted on the GPU (tecogan_b200/csrc/yuv.cu) byte for byte as cv2.cvtColor(COLOR_YUV2RGB_I420 /
     COLOR_RGB2YUV_I420) converts; y4m input names its files <output_name>_<%04d frame number>.<output_ext>, y4m output
     holds the frames the image path would write and no image file is written;
+  * --scene_threshold T (opt-in extension, absent from FLAGS unless given; inference only, 0 < T <= 100) restarts the
+    recurrence at scene cuts: a frame whose score (the 0..100 mean absolute difference of its 8-bit RGB values to the
+    previous frame's, or its change if smaller; computed on the GPU by tecogan_b200/csrc/scene.cu) is >= T starts a new
+    scene, and each scene is warmed up and super-resolved as a sequence of its own, every input frame written once
+    (lib/dataloader.py::scene_order; DESIGN.md section 4.13); a stream of 6 or more frames without a cut gives the files
+    of a run without the flag;
   * under `torchrun` each rank trains on its own clip shard with one NCCL all-reduce per step;
   * monitoring (--summary_dir: TensorBoard scalars, logfile.txt, validation scalars, test-sequence frames at every
     checkpoint) runs on rank 0 only, in process: the held-out scenes end_dir+1..end_dir_val are optional (validation is
@@ -73,6 +79,9 @@ FLAG_DEFS = [  # (name, type, default) -- reference main.py:32-103
     ('outscale', float, argparse.SUPPRESS),
     # extension: inference input / output as a YUV4MPEG2 stream (tecogan_b200/y4m.py).  Opt-in in the same way.
     ('input_y4m', str, argparse.SUPPRESS), ('output_y4m', str, argparse.SUPPRESS),
+    # extension: restart the inference recurrence at scene cuts (score >= T, 0 < T <= 100).  Opt-in in the same way;
+    # read as text and checked by main(), so that a malformed value raises ValueError as an out-of-range one does.
+    ('scene_threshold', str, argparse.SUPPRESS),
 ]
 
 
@@ -208,24 +217,31 @@ def restore_train_state(train_state, spec):
 def inference(FLAGS):
     from tecogan_b200 import config, variables as V, y4m
     from tecogan_b200.engine import InferenceEngine
-    from tecogan_b200.lib.dataloader import inference_paths, padded, stream_inputs
+    from tecogan_b200.lib.dataloader import inference_paths, padded, stream_inputs, stream_scenes
     if FLAGS.checkpoint is None:
         raise ValueError('The checkpoint file is needed to performing the test.')
     sink = None
+    scenes = hasattr(FLAGS, 'scene_threshold')
     if hasattr(FLAGS, 'input_y4m'):            # the header is read and checked here, before anything is set up
         reader = y4m.Y4MReader(FLAGS.input_y4m, FLAGS.input_dir_len)
         rate, aspect = reader.header.rate, reader.header.aspect
-        frames, names = reader.frames(), reader.names()
+        if scenes:
+            frames, names = reader.scenes(FLAGS.scene_threshold), reader.name
+        else:
+            frames, names = reader.frames(), reader.names()
     else:
         paths, down = inference_paths(FLAGS)
         rate, aspect = y4m.PNG_INPUT_RATE, y4m.PNG_INPUT_ASPECT
-        frames, names = stream_inputs(paths, down), padded(paths)
+        if scenes:
+            frames, names = stream_scenes(paths, down, FLAGS.scene_threshold), paths.__getitem__
+        else:
+            frames, names = stream_inputs(paths, down), padded(paths)
     try:
         first = next(frames, None)
         if first is None:
             raise IndexError('no frame in the input y4m stream' if hasattr(FLAGS, 'input_y4m')
                              else 'no .png frame in the input directory')
-        h, w = first.shape[:2]
+        h, w = (first.frame if scenes else first).shape[:2]
         out_hw = outscale_size(FLAGS, h, w)
         if hasattr(FLAGS, 'output_y4m') and (out_hw[0] % 2 or out_hw[1] % 2):
             raise ValueError('--output_y4m: the %dx%d output has an odd side; 4:2:0 needs even sides (choose another '
@@ -242,8 +258,8 @@ def inference(FLAGS):
             sink = y4m.Y4MWriter(FLAGS.output_y4m, out_hw[1], out_hw[0], rate, aspect)
         else:
             os.makedirs(image_dir, exist_ok=True)
-        super_resolve_frames(eng, names, itertools.chain([first], frames), image_dir, FLAGS.output_name,
-                             FLAGS.output_ext, out_hw, sink)
+        run = super_resolve_scenes if scenes else super_resolve_frames
+        run(eng, names, itertools.chain([first], frames), image_dir, FLAGS.output_name, FLAGS.output_ext, out_hw, sink)
     finally:
         frames.close()
         if sink is not None:
@@ -319,6 +335,66 @@ def super_resolve_frames(eng, paths_LR, frames, image_dir, output_name, output_e
     for a, b in timing:
         srtime += a.elapsed_time(b) / 1000.0
     print("total time " + str(srtime) + ", frame number " + str(max_iter))
+
+
+def super_resolve_scenes(eng, name_of, steps, image_dir, output_name, output_ext, out_hw=None, sink=None):
+    """super_resolve_frames for a stream cut into scenes (--scene_threshold): `steps` are the
+    lib/dataloader.py::SceneSteps of stream_scenes or Y4MReader.scenes.  Before a scene's first step the engine is reset
+    (pre_warp = 0) and, for a scene that starts at a cut, `scene cut before frame <i>, score <s>` is printed; its
+    warm-up steps print `Warming up <n>` and are not saved; each written step saves its frame as
+    <output_name>_<name>.<output_ext>, name_of(input index) giving the name (a path's stem, or y4m's %04d).  The next
+    frame's flow is computed ahead (step(cur, next_lr=nxt)) except across a scene boundary: a scene's last frame is
+    stepped alone, then the engine is reset.  "frame number" counts every step, warm-ups included.  Writing, timing and
+    errors are as in super_resolve_frames."""
+    import collections
+    import torch
+    from tecogan_b200.lib.writer import FrameWriter
+    it = iter(steps)
+    steps_run = 0
+    srtime = 0.0
+    timing = collections.deque()
+    writer = None
+    warm = 0
+    print('Frame evaluation starts!!')
+    try:
+        cur = next(it, None)
+        while cur is not None:
+            nxt = next(it, None)
+            if cur.reset:
+                if cur.score is not None:
+                    print('scene cut before frame %d, score %.4f' % (cur.start, cur.score))
+                eng.reset()
+                warm = cur.index - cur.start
+            t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            t0.record()
+            eng.step(cur.frame, next_lr=nxt.frame if nxt is not None and not nxt.reset else None)
+            t1.record()
+            timing.append((t0, t1))
+            while timing and timing[0][1].query():
+                a, b = timing.popleft()
+                srtime += a.elapsed_time(b) / 1000.0
+            steps_run += 1
+            if cur.write:
+                name, _ = os.path.splitext(os.path.basename(str(name_of(cur.index))))
+                filename = output_name + '_' + name
+                print('saving image %s' % filename)
+                if writer is None:
+                    writer = FrameWriter(*(out_hw or eng.out_u8.shape[1:3]), eng.device, sink=sink)
+                writer.put(eng.out_u8[0], os.path.join(image_dir, "%s.%s" % (filename, output_ext)))
+            else:
+                print("Warming up %d" % warm)
+                warm -= 1
+            cur = nxt
+        cur = nxt = None
+    finally:
+        if writer is not None:
+            writer.close()
+    if writer is not None and writer.error is not None:
+        raise writer.error
+    torch.cuda.synchronize()
+    for a, b in timing:
+        srtime += a.elapsed_time(b) / 1000.0
+    print("total time " + str(srtime) + ", frame number " + str(steps_run))
 
 
 TEST_SEQUENCE_DIR = './LR/calendar/'      # reference main.py:164, hard-coded there as well
@@ -626,6 +702,11 @@ def main(argv=None):
             raise ValueError('--%s applies to --mode inference only' % flag)
     if hasattr(FLAGS, 'input_y4m') and (FLAGS.input_dir_LR is not None or FLAGS.input_dir_HR is not None):
         raise ValueError('--input_y4m replaces --input_dir_LR / --input_dir_HR: give one input')
+    if hasattr(FLAGS, 'scene_threshold'):      # refused before anything is set up
+        if FLAGS.mode != 'inference':
+            raise ValueError('--scene_threshold applies to --mode inference only')
+        from tecogan_b200.lib.dataloader import scene_threshold
+        FLAGS.scene_threshold = scene_threshold(FLAGS.scene_threshold)
     if hasattr(FLAGS, 'outscale'):             # refused before anything is set up
         if FLAGS.mode != 'inference':
             raise ValueError('--outscale applies to --mode inference only')

@@ -672,6 +672,26 @@ def i420_to_rgb(frames, out=None):
     return out
 
 
+def frame_sad_q8(a, b, out):
+    """out[0] = sum of |q(a) - q(b)| over every value, q(x) = clamp(rint(255 x), 0, 255), an exact integer: the frame
+    difference behind the scene-cut score of `main.py --scene_threshold` (DESIGN.md section 4.13), on the current
+    stream.  a and b are contiguous float32 CUDA tensors of one shape on one device (any offset); out is a contiguous
+    one-element int64 tensor on that device (the sum of any frame is far below 2^63), zeroed by the launch itself.
+    Anything else raises ValueError before a launch."""
+    for t, what in ((a, "a"), (b, "b")):
+        if not (torch.is_tensor(t) and t.is_cuda and t.dtype == f32 and t.is_contiguous()):
+            raise ValueError("frame_sad_q8: %s must be a contiguous float32 CUDA tensor, got %s" % (
+                what, "%s %s on %s" % (t.dtype, tuple(t.shape), t.device) if torch.is_tensor(t) else type(t).__name__))
+    if a.shape != b.shape or a.device != b.device:
+        raise ValueError("frame_sad_q8: a %s on %s and b %s on %s differ" % (tuple(a.shape), a.device, tuple(b.shape),
+                                                                          b.device))
+    if not (torch.is_tensor(out) and out.dtype == torch.int64 and out.numel() == 1 and out.is_contiguous()
+            and out.device == a.device):
+        raise ValueError("frame_sad_q8: out must be a contiguous one-element int64 tensor on %s" % a.device)
+    call("teco_frame_sad_q8", ptr(a, f32), ptr(b, f32), a.numel(), ptr(out, torch.int64), stream_ptr())
+    return out
+
+
 def to_u8(x01):
     y = torch.empty(x01.shape, device=x01.device, dtype=torch.uint8)
     call("teco_to_u8", ptr(_cc(x01), f32), ptr(y, torch.uint8), x01.numel(), stream_ptr())

@@ -9,6 +9,7 @@ space), the same batches cut there by teco_gather_clips_u8 (teco_gather_clips_ho
 import collections
 import concurrent.futures
 import itertools
+import math
 import os
 import struct
 import time
@@ -45,6 +46,59 @@ def padded(seq):
     """The reference's hard-coded symmetric warm-up padding: entries 5, 4, 3, 2, 1 prepended (fewer for a shorter
     sequence)."""
     return seq[5:0:-1] + seq
+
+
+def scene_threshold(value):
+    """The threshold T of --scene_threshold as a float: 0 < T <= 100 and finite, else ValueError (also for a value that
+    is not a number)."""
+    try:
+        t = float(value)
+    except (TypeError, ValueError):
+        raise ValueError('--scene_threshold: %r is not a number' % (value,))
+    if not (math.isfinite(t) and 0.0 < t <= 100.0):
+        raise ValueError('--scene_threshold must be in (0, 100], got %r' % (value,))
+    return t
+
+
+def scene_score(sad, values, prev_mafd):
+    """(mafd, score) of a frame whose 8-bit difference to the previous frame sums to `sad` over `values` values (3 h w):
+    mafd = 100 sad / (255 values), the mean absolute frame difference on a 0..100 scale, and score = min(mafd,
+    |mafd - prev_mafd|), so that a sustained fast pan is not a cut.  Float64; a scene starts where score >= T."""
+    mafd = 100.0 * sad / (values * 255.0)
+    return mafd, min(mafd, abs(mafd - prev_mafd))
+
+
+def scene_order(cuts):
+    """The inference order of a stream cut into scenes, built as the stream arrives.  `cuts` yields (index, cut) in
+    stream order (index 0, 1, 2, ...; cut: a scene starts at that frame; frame 0 always starts one).  Yields
+    (input index, write, reset before) steps: each scene of L frames starting at frame c is run as the reference runs a
+    sequence (padded): warm-up frames c+m, ..., c+1 (not written), m = min(5, L - 1), then c, ..., c+L-1 (each written
+    once), with the recurrence reset before the scene's first step.  Without a cut and with n >= 6 frames this is
+    padded(range(n)) with writes from position 5.
+
+    `cuts` is read lazily: at most six pairs past a scene's first frame (enough to bound m) and, inside a scene, one
+    pair past the step last yielded (to know whether the next frame starts a scene)."""
+    it = iter(cuts)
+    ahead = collections.deque()                  # pairs read but not yet placed
+
+    def have(count):
+        while len(ahead) < count:
+            got = next(it, None)
+            if got is None:
+                return False
+            ahead.append(got)
+        return True
+    while have(1):
+        c = ahead.popleft()[0]                   # a scene starts here
+        extent = 1                               # the scene's frames within c .. c+5
+        while extent < 6 and have(extent) and not ahead[extent - 1][1]:
+            extent += 1
+        m = extent - 1
+        for k in range(c + m, c, -1):
+            yield k, False, k == c + m
+        yield c, True, m == 0
+        while have(1) and not ahead[0][1]:
+            yield ahead.popleft()[0], True, False
 
 
 def inference_data_loader(FLAGS):
@@ -113,6 +167,99 @@ def stream_inputs(paths, down, window_bytes=None):
         feed.close()
 
 
+# One step of a stream cut into scenes: the [h, w, 3] float32 frame, its input index, whether it is written (False: a
+# warm-up step), whether the recurrence is reset before it and, on a scene's first step, the scene's first frame and the
+# score that started it (None for the stream's first scene).
+SceneStep = collections.namedtuple('SceneStep', 'frame, index, write, reset, start, score')
+
+
+def scene_steps(feed, threshold, release):
+    """The steps of a stream cut into scenes (scene_order), its frames taken from `feed` (a DeviceHandoff whose chunks
+    carry each frame's 8-bit SAD to the previous frame, frame_sad_q8, in pinned memory) in stream order.  A frame's score
+    is read on the host after a wait on the reader's event for its chunk (DeviceHandoff.value), never on the consumer's
+    stream.  A frame is dropped once its written step has been handed out, then release(k) is called."""
+    cut_at = collections.deque()                 # (frame, score) of the cuts found and not yet reached
+
+    def cuts():
+        prev_mafd = 0.0
+        for k in itertools.count():
+            frame = feed.take(k)
+            if frame is None:
+                return
+            if k == 0:
+                yield 0, True
+                continue
+            prev_mafd, score = scene_score(feed.value(k), frame.numel(), prev_mafd)
+            del frame
+            if score >= threshold:
+                cut_at.append((k, score))
+            yield k, score >= threshold
+    first = True
+    for k, write, reset in scene_order(cuts()):
+        start = score = None
+        if reset:
+            start, score = (0, None) if first else cut_at.popleft()
+            first = False
+        frame = feed.take(k)
+        yield SceneStep(frame, k, write, reset, start, score)
+        del frame
+        if write:
+            feed.drop(k)
+            release(k)
+
+
+def scene_sads(frames, prev):
+    """The reader side of scene_steps: a pinned int64 tensor with frame_sad_q8 of each of `frames` against the frame
+    before it (`prev` for the first, 0 without one or for a frame of another size), copied on the current stream."""
+    import torch
+    sad = torch.zeros(len(frames), dtype=torch.int64, device=frames[0].device)
+    for t, f in enumerate(frames):
+        if prev is not None and prev.shape == f.shape:
+            K.frame_sad_q8(prev, f, sad[t:t + 1])
+        prev = f
+    host = torch.empty(len(frames), dtype=torch.int64, pin_memory=True)
+    host.copy_(sad, non_blocking=True)
+    return host
+
+
+def stream_scenes(paths, down, threshold, window_bytes=None):
+    """Generator over the SceneSteps of the PNG input of `main.py --scene_threshold T`: the frames of stream_inputs,
+    decoded the same way, in the order scene_order gives for the cuts where score >= T.
+
+    The reader thread computes each frame's SAD to the frame before it on its own stream, right after the window is
+    decoded (scene_sads; it keeps a reference to the window's last frame for the next window).  A window returns its
+    credit once every frame of it has been written.  The credits are the most windows any frames c .. c+5 span, plus
+    one to decode ahead: at a scene's first frame c every earlier window has returned its credit, and the scene's extent
+    within c .. c+5 must be known before its first step.  So the frames on the device stay bounded by that, whatever
+    the stream's length or number of cuts.  Errors, closing and the reader thread are as in stream_inputs."""
+    windows = input_windows(paths, window_bytes)
+    if not windows:
+        return
+    n = len(paths)
+    window_of = [w for w, (i, j) in enumerate(windows) for _ in range(i, j)]
+    left = [j - i for i, j in windows]
+    credits = max(window_of[min(c + 5, n - 1)] - window_of[c] + 1 for c in range(n)) + 1
+
+    def decode():
+        prev = None
+        for i, j in windows:
+            frames = list(read_inputs(paths[i:j], down))
+            yield i, frames, scene_sads(frames, prev)
+            prev = frames[-1]
+            del frames
+
+    def release(k):
+        w = window_of[k]
+        left[w] -= 1
+        if left[w] == 0:
+            feed.release()
+    feed = DeviceHandoff(decode(), credits, 'stream_scenes')
+    try:
+        yield from scene_steps(feed, threshold, release)
+    finally:
+        feed.close()
+
+
 class DeviceHandoff:
     """The reader half of a streamed inference input, shared by stream_inputs (PNG files) and
     tecogan_b200/y4m.py::Y4MReader (a YUV4MPEG2 stream).
@@ -123,14 +270,18 @@ class DeviceHandoff:
     consumer's current stream first waits for the chunk's event, and the chunk's tensors are recorded on that stream, so
     the allocator reuses their memory only once the consumer's work on them is done.  take() returns None once the
     iterator has ended without frame k, and raises an exception of the reader at the frame that needs its chunk.  drop(k)
-    forgets frame k.  close() stops and joins the reader; the iterator is not asked for another chunk after it."""
+    forgets frame k.  close() stops and joins the reader; the iterator is not asked for another chunk after it.
+
+    A chunk may carry a third item, a host tensor with one value per frame written on the reader's stream (the scene
+    scores' pinned SADs, scene_sads): value(k) returns frame k's entry after a host wait on the chunk's event alone, so
+    the consumer's stream is never synchronised to read it."""
 
     def __init__(self, chunks, credits, name):
         import queue
         import threading
         import torch
         self.credits, self.ready, self.stop = threading.Semaphore(credits), queue.Queue(), threading.Event()
-        self.have, self.ended = {}, False
+        self.have, self.values, self.ended = {}, {}, False
         cuda = torch.cuda.is_available()
         device = torch.cuda.current_device() if cuda else None
 
@@ -149,11 +300,11 @@ class DeviceHandoff:
                         if got is None:
                             self.ready.put(None)
                             return
-                        i, frames = got
+                        i, frames = got[:2]
                         done = torch.cuda.Event() if cuda else None
                         if cuda:
                             done.record()
-                    self.ready.put((i, frames, done))
+                    self.ready.put((i, frames, done) + tuple(got[2:]))
                     del got, frames
             except BaseException as e:              # handed to the consumer, raised there
                 self.ready.put(e)
@@ -177,7 +328,9 @@ class DeviceHandoff:
             if isinstance(got, BaseException):
                 self.ended = True
                 raise got
-            i, frames, done = got
+            i, frames, done = got[:3]
+            if len(got) > 3:
+                self.values.update((i + t, (done, got[3], t)) for t in range(len(frames)))
             if done is not None:
                 consumer = torch.cuda.current_stream()
                 consumer.wait_event(done)
@@ -188,8 +341,15 @@ class DeviceHandoff:
             del got, frames
         return self.have[k]
 
+    def value(self, k):
+        done, values, t = self.values[k]
+        if done is not None:
+            done.synchronize()
+        return int(values[t])
+
     def drop(self, k):
         del self.have[k]
+        self.values.pop(k, None)
 
     def release(self):
         self.credits.release()
@@ -199,6 +359,7 @@ class DeviceHandoff:
         self.credits.release()                      # wakes a reader waiting for a credit; it sees `stop` and returns
         self.thread.join()
         self.have.clear()
+        self.values.clear()
 
 
 def _png_head(path):

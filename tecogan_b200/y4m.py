@@ -123,14 +123,17 @@ class Y4MReader:
             raise
         self.warmup = None
 
-    def _chunks(self):
+    def _chunks(self, scores=False):
         """The reader thread's side: frame k read into a ring of pinned buffers, uploaded and converted on the thread's
-        stream; one frame per chunk."""
+        stream; one frame per chunk.  With `scores` each chunk also carries the frame's SAD to the frame before it
+        (lib/dataloader.py::scene_sads), computed on the same stream; the previous frame is kept for it."""
         import torch
         from . import kernels as K
+        from .lib.dataloader import scene_sads
         w, h = self.header.w, self.header.h
         ring = [torch.empty(frame_bytes(w, h), dtype=torch.uint8, pin_memory=True) for _ in range(READ_RING)]
         copied = [None] * READ_RING
+        prev = None
         try:
             for k in (itertools.count() if self.limit <= 0 else range(self.limit)):
                 r = k % READ_RING
@@ -142,7 +145,13 @@ class Y4MReader:
                 copied[r] = torch.cuda.Event()
                 copied[r].record()
                 rgb = K.i420_to_rgb(planes.view(3 * h // 2, w))
-                yield k, [K.frames_to_f32(rgb)[0]]
+                if not scores:
+                    yield k, [K.frames_to_f32(rgb)[0]]
+                    continue
+                frame = K.frames_to_f32(rgb)[0]
+                sad = scene_sads([frame], prev)
+                prev, frame = frame, None
+                yield k, [prev], sad
         finally:
             self.f.close()
 
@@ -169,6 +178,22 @@ class Y4MReader:
         finally:
             feed.close()
             self.f.close()
+
+    def scenes(self, threshold):
+        """The stream as lib/dataloader.py::SceneSteps for `main.py --scene_threshold`: scene_order over the cuts where
+        score >= threshold, each frame's score computed on the reader's stream.  READ_CREDITS frames cover every scene
+        start: its six frames c .. c+5, known before its first step, and two decoded ahead.  name(k) names frame k."""
+        from .lib.dataloader import DeviceHandoff, scene_steps
+        feed = DeviceHandoff(self._chunks(scores=True), READ_CREDITS, 'y4m_reader')
+        try:
+            yield from scene_steps(feed, threshold, lambda k: feed.release())
+        finally:
+            feed.close()
+            self.f.close()
+
+    @staticmethod
+    def name(k):
+        return '%04d' % (k + 1)
 
     def names(self):
         for k in itertools.chain(range(self.warmup, 0, -1), itertools.count()):
