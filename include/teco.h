@@ -270,6 +270,14 @@ int teco_i420_to_rgb_u8(const uint8_t* src, int32_t N, int32_t H, int32_t W, uin
  * n == 0 gives 0.  a, b: n float32 values each, any 4-byte alignment (float4 loads when both are 16-byte aligned).
  * NULL pointers or n < 0: TECO_E_INVALID, nothing is enqueued. */
 int teco_frame_sad_q8(const float* a, const float* b, int64_t n, uint64_t* out, void* stream);
+/* Frame differences of `dataPrepare.py --scene_threshold` (DESIGN.md section 4.14): out[i] = sum over j < frame_bytes of
+ * |f_i[j] - f_{i-1}[j]| for the n packed uint8 frames f_i = frames + i * frame_bytes, f_{-1} = prev; out[0] = 0 when
+ * prev is NULL.  Exact 64-bit integer sums, independent of the launch, in one launch for all n.  The entry zeroes
+ * out[0..n) on `stream` itself, then adds to it.  Any alignment (16-byte loads when frames, prev and frame_bytes are
+ * 16-byte aligned).  NULL frames or out, n < 1, frame_bytes < 1 or n * frame_bytes past 64 bits: TECO_E_INVALID,
+ * nothing is enqueued. */
+int teco_frame_sads_u8(const uint8_t* frames, int64_t frame_bytes, int32_t n, const uint8_t* prev, uint64_t* out,
+                       void* stream);
 
 /* generic elementwise y = f(a*x + b) with f in TECO_ACT_*; n elements. preprocess/deprocess lib/ops.py:13-22 */
 int teco_affine_act_f32(const float* x, float* y, int64_t n, float a, float b, int32_t act, void* stream);

@@ -79,6 +79,7 @@ SIGNATURES = {
     "teco_rgb_to_i420_u8": [_P, _I64, _I32, _I32, _P, _P],
     "teco_i420_to_rgb_u8": [_P, _I32, _I32, _I32, _P, _P],
     "teco_frame_sad_q8": [_P, _P, _I64, _P, _P],
+    "teco_frame_sads_u8": [_P, _I64, _I32, _P, _P, _P],
     "teco_affine_act_f32": [_P, _P, _I64, _F, _F, _I32, _P],
     "teco_act_bwd_f32": [_P, _P, _P, _I64, _I32, _P],
     "teco_f32_to_bf16_pad": [_P, _P, _I64, _I32, _I32, _I32, _I32, _F, _F, _P],

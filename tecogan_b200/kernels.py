@@ -692,6 +692,35 @@ def frame_sad_q8(a, b, out):
     return out
 
 
+def frame_sads_u8(frames, prev=None, out=None):
+    """out[i] = sum of |frames[i] - frames[i - 1]| over every byte, an exact integer, with frames[-1] = prev (out[0] = 0
+    without it): the frame differences behind the scene cuts of `dataPrepare.py --scene_threshold` (DESIGN.md section
+    4.14), all n in one launch on the current stream.  frames is a contiguous uint8 CUDA tensor [n, ...] of n >= 1
+    frames of at least one byte (any offset); prev a contiguous uint8 tensor of one frame's shape on their device; out
+    a contiguous int64 [n] tensor on it, zeroed by the launch itself.  Since q(u / 255) = u for a byte u,
+    out[i] == frame_sad_q8(frames[i - 1] / 255, frames[i] / 255).  Anything else raises ValueError before a launch."""
+    def what(t):
+        return "%s %s on %s" % (t.dtype, tuple(t.shape), t.device) if torch.is_tensor(t) else type(t).__name__
+    if not (torch.is_tensor(frames) and frames.is_cuda and frames.dtype == torch.uint8 and frames.is_contiguous()
+            and frames.dim() >= 1 and 1 <= frames.shape[0] < 2 ** 31 and frames[0].numel() >= 1):
+        raise ValueError("frame_sads_u8: frames must be a contiguous uint8 CUDA tensor of n >= 1 non-empty frames, "
+                         "got %s" % what(frames))
+    n = frames.shape[0]
+    if prev is not None and not (torch.is_tensor(prev) and prev.dtype == torch.uint8 and prev.is_contiguous()
+                                 and prev.shape == frames.shape[1:] and prev.device == frames.device):
+        raise ValueError("frame_sads_u8: prev must be a contiguous uint8 %s tensor on %s, got %s" % (
+            tuple(frames.shape[1:]), frames.device, what(prev)))
+    if out is None:
+        out = torch.empty(n, dtype=torch.int64, device=frames.device)
+    elif not (torch.is_tensor(out) and out.dtype == torch.int64 and tuple(out.shape) == (n,) and out.is_contiguous()
+              and out.device == frames.device):
+        raise ValueError("frame_sads_u8: out must be a contiguous int64 [%d] tensor on %s, got %s" % (
+            n, frames.device, what(out)))
+    call("teco_frame_sads_u8", ptr(frames, torch.uint8), frames[0].numel(), n, ptr(prev, torch.uint8),
+         ptr(out, torch.int64), stream_ptr())
+    return out
+
+
 def to_u8(x01):
     y = torch.empty(x01.shape, device=x01.device, dtype=torch.uint8)
     call("teco_to_u8", ptr(_cc(x01), f32), ptr(y, torch.uint8), x01.numel(), stream_ptr())
